@@ -1,4 +1,4 @@
-"""B200-native Conformer-encoder forward path for mpc001/auto_avsr (hot path only).
+"""H100-native (sm_90a) Conformer-encoder forward path for mpc001/auto_avsr (hot path only).
 
     import auto_avsr_b200; auto_avsr_b200.install()      # before importing the reference's E2E
     from auto_avsr_b200 import ConformerEncoder           # or use the class directly
@@ -19,14 +19,14 @@ def install():
 
 
 def install_head(model):
-    """Swap an already-built reference ``E2E``'s ``proj_encoder`` and ``ctc`` for the B200 drop-ins (same parameters)."""
+    """Swap an already-built reference ``E2E``'s ``proj_encoder`` and ``ctc`` for the CUDA drop-ins (same parameters)."""
     from .install import install_head as _install_head
     return _install_head(model)
 
 
 def install_decoder(model):
-    """Swap an already-built reference ``E2E``'s attention decoder for the B200 scoring drop-in and make
-    ``model.scorers()`` return the B200 CTC prefix scorer (inference / beam search only)."""
+    """Swap an already-built reference ``E2E``'s attention decoder for the CUDA scoring drop-in and make
+    ``model.scorers()`` return the CUDA CTC prefix scorer (inference / beam search only)."""
     from .install import install_decoder as _install_decoder
     return _install_decoder(model)
 

@@ -149,7 +149,7 @@ SIGNATURES = {
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-        "(nvcc, sm_100a).  auto_avsr_b200 has no CPU / PyTorch fallback for the encoder hot path.")
+        "(nvcc, sm_90a).  auto_avsr_b200 has no CPU / PyTorch fallback for the encoder hot path.")
 
 lib = C.CDLL(LIB_PATH)
 for _name, (_res, _args) in SIGNATURES.items():

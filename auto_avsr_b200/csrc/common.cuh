@@ -57,7 +57,7 @@ static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 
 // ---------------------------------------------------------------- programmatic dependent launch (PDL)
 // Every hot-path kernel is launched with cudaLaunchAttributeProgrammaticStreamSerialization: it may start (block
-// scheduling, barrier init, TMEM allocation, tensor-map prefetch) while its predecessor in the stream / graph is
+// scheduling, barrier init, tensor-map prefetch) while its predecessor in the stream / graph is
 // still draining, and blocks in pdl_wait() until the predecessor has completed and flushed before it touches any
 // global memory.  pdl_launch_dependents() at the top lets the successor do the same.  Without the attribute both
 // are no-ops, so the same kernels work under plain launches (AVSR_B200_PDL=0).
@@ -135,9 +135,9 @@ __device__ __forceinline__ float warp_max(float v) {
 // ---------------------------------------------------------------- tensor-core operand storage
 // How a tensor that feeds a tensor-core contraction is stored:
 //   OP_F32  : plain fp32 (CUDA-core reference path)
-//   OP_TF32 : fp32 container, value rounded to TF32 (10-bit mantissa) -> tcgen05 kind::tf32
-//   OP_F16  : IEEE half (same 10-bit mantissa as TF32, 5-bit exponent, saturating) -> tcgen05 kind::f16;
-//             half the bytes through L2/shared memory and twice the MMA rate of kind::tf32
+//   OP_TF32 : fp32 container, value rounded to TF32 (10-bit mantissa) -> wgmma .tf32
+//   OP_F16  : IEEE half (same 10-bit mantissa as TF32, 5-bit exponent, saturating) -> wgmma .f16;
+//             half the bytes through L2/shared memory and twice the MMA rate of .tf32
 enum OperandKind : int { OP_F32 = 0, OP_TF32 = 1, OP_F16 = 2 };
 
 __device__ __forceinline__ __half to_half_sat(float x) {
@@ -194,15 +194,7 @@ enum EpiMode : int {
                    // N == 3D): v into `vt` with the SAME head-major layout   -> (B,H,T,64) each
   EPI_VT = 2,      // A = W_v (m = feature), B = frames (n): v^T                     -> (B,H,64,Tp)
   EPI_GLU = 3,     // interleaved pointwise_cov1: value cols [g*128, +64), gate cols +64 -> out (M, N/2)
-  EPI_POS = 4,     // linear_pos of all layers: n = l*D + h*64 + d, m = table row      -> (L,H,Rp,64)
-  EPI_LSE = 5      // y = acc + bias[n] as fp32 logits (M, ldo) PLUS per (row, half column tile) log-sum-exp partials over
-                   // the columns n < n_valid -- the ctc_lo projection (two-SM kernel only, gemm_tc2_lse)
-};
-
-// one log-sum-exp partial: running maximum, sum of exp(x - maximum) and first index of the maximum
-struct LsePart {
-  float m, s;
-  int idx, pad;
+  EPI_POS = 4      // linear_pos of all layers: n = l*D + h*64 + d, m = table row      -> (L,H,Rp,64)
 };
 
 struct EpiParams {
@@ -219,8 +211,6 @@ struct EpiParams {
   const float* pos_v;
   float* partial;     // split-K: fp32 workspace [splits][M][ldo] for the partial tiles (deterministic fix-up)
   int* counters;      // split-K: one arrival counter per output tile, zero on entry, reset by the last arriver
-  int n_valid;        // LSE: columns >= n_valid are padding (stored, but excluded from the partials)
-  LsePart* lse_part;  // LSE: [2 * tiles_n][M] partials (two epilogue warps per lane quarter split a tile's columns)
   void* qu;           // operand-typed (float for OP_F32/OP_TF32, __half for OP_F16)
   void* qv;
   void* kk;
@@ -341,57 +331,24 @@ __device__ __forceinline__ void epi_store_glu(const EpiParams& p, int m, int n_v
 // ---------------------------------------------------------------- kernel launchers (defined in the .cu files)
 // fp32 CUDA-core GEMM (gemm_simt.cu)
 int gemm_simt(int mode, const float* A, const float* Bw, int M, int N, int K, const EpiParams& ep, cudaStream_t st);
-// tcgen05 GEMM (gemm_tc.cu); opk = OP_TF32 (A, Bw are float) or OP_F16 (A, Bw are __half)
+// wgmma GEMM (gemm_tc.cu); opk = OP_TF32 (A, Bw are float) or OP_F16 (A, Bw are __half)
 int gemm_tc(int mode, int opk, const void* A, const void* Bw, int M, int N, int K, const EpiParams& ep, cudaStream_t st);
-
-// two-SM (cta_group::2) GEMM for fp16 EPI_LINEAR / EPI_QK / EPI_GLU (gemm_tc2.cu): *handled = 1 when it took the problem
-int gemm_tc2_try(int mode, const void* A, const void* Bw, int M, int N, int K, const EpiParams& ep, cudaStream_t st,
-                 int* handled);
-
-// deferred split-K (gemm_tc2.cu): plan returns 1 and fills bnp / nsplit when the shape qualifies; the GEMM writes
-// partial[s][M][N] (raw fp32 k-slice sums) and the consuming LayerNorm finishes the residual update (LnParts)
-int gemm_tc2_splitk_plan(int M, int N, int K, int* bnp, int* nsplit);
-// true while the caller guarantees that B operands are prepared weights no kernel of the stream writes (the encoder
-// forward): lets the experimental AVSR_B200_PREB=1 variant fetch weights before griddepcontrol.wait
-extern thread_local bool g_tc2_weights_static;
-int gemm_tc2_splitk(const void* A, const void* Bw, int M, int N, int K, float* partial, int bnp, int nsplit,
-                    cudaStream_t st);
-
-// ctc_lo (gemm_tc2.cu): logits[M][ldo] = A Bw^T + bias (fp32; N a multiple of 512, padded columns included) and
-// part[nparts][M] log-sum-exp partials over the columns < n_valid; *nparts = 2 * N / 512.  Needs M >= 256, K % 64 == 0.
-int gemm_tc2_lse(const void* A, const void* Bw, const float* bias, int M, int N, int K, int n_valid, float* logits,
-                 long ldo, LsePart* part, int* nparts, cudaStream_t st);
-int gemm_tc2_lse_ok(int M, int N, int K);
-
-// Residual update folded into a LayerNorm's load: row = x + alpha * (bias + part[0] + part[1] + ... ) (fixed order,
-// so the result does not depend on scheduling); the updated row is written to x_out when that is not already the
-// LayerNorm's own fp32 output.
-struct LnParts {
-  const float* part = nullptr;   // [nparts][rows][d]
-  int nparts = 0;
-  long stride = 0;               // rows * d
-  const float* bias = nullptr;   // [d]
-  float alpha = 0.f;
-  float* x_out = nullptr;        // optional [rows][d]
-};
 
 // elementwise.cu
 int launch_embed_scale(const float* xs, float* x, long n, float scale, cudaStream_t st);
 // `out_kind` is an OperandKind: how y / pe is stored
 int launch_layernorm(const float* x, const float* g, const float* b, void* y, int rows, int d, int out_kind,
-                     cudaStream_t st, const LnParts* parts = nullptr);
+                     cudaStream_t st);
 // y_f32 = LN(x) as fp32 (may alias x) AND y_op = the same values in operand storage (after_norm feeding ctc_lo)
 int launch_layernorm_dual(const float* x, const float* g, const float* b, float* y_f32, void* y_op, int rows, int d,
                           int out_kind, cudaStream_t st);
 int launch_layernorm2(const float* x, const float* g1, const float* b1, const float* g2, const float* b2, float* y1,
-                      void* y2, int rows, int d, int out_kind, cudaStream_t st, const LnParts* parts = nullptr);
+                      void* y2, int rows, int d, int out_kind, cudaStream_t st);
 int launch_sinusoid(void* pe, int T, int d, int out_kind, cudaStream_t st);
 int launch_dwconv_bn_silu(const float* x, const float* wt /*(K,C)*/, const float* scale, const float* shift, void* y,
                           int B, int T, int C, int K, int out_kind, cudaStream_t st);
 
 // head.cu
-int launch_lse_finish(const float* logits, long ldx, const LsePart* part, int nparts, int rows, float* y, long ldy,
-                      int32_t* best, int n, cudaStream_t st);
 int launch_log_softmax_rows(const float* x, long ldx, float* y, long ldy, int32_t* best, int rows, int n, cudaStream_t st);
 
 // attention: q-side tensors (B,H,T,64), vt (B,H,64,Tp), pos (H,Rp,64) for one layer, ctx (B*T, H*64)
@@ -401,7 +358,7 @@ int attention_simt(const float* qu, const float* qv, const float* kk, const floa
 int attention_tc(const float* qu, const float* qv, const float* kk, const float* vt, const float* pos,
                  const int32_t* lengths, float* ctx, int B, int T, int H, int Tp, int Rp, int round_out,
                  cudaStream_t st);
-// fp16 operands (attention_f16.cu): qu, qv, kk, vv all (B,H,T,64) __half (V in its natural layout); ctx __half
+// fp16 operands (attention_tc.cu): qu, qv, kk, vv all (B,H,T,64) __half (V in its natural layout); ctx __half
 int attention_f16(const __half* qu, const __half* qv, const __half* kk, const __half* vv, const __half* pos,
                   const int32_t* lengths, __half* ctx, int B, int T, int H, int Rp, cudaStream_t st);
 

@@ -1,7 +1,7 @@
 // Device side of the attention-decoder scoring path and the CTC prefix scorer (SURVEY.md 8f #3): the backend that
 // runs decoder_body.cuh's schedule on the GPU, and the C ABI of include/avsr_b200.h for it.
 //
-// The projections are the library's GEMMs (tcgen05 gemm_tc for AVSR_PREC_F16 / TF32 -- at n <= 40 hypotheses they are
+// The projections are the library's GEMMs (wgmma gemm_tc for AVSR_PREC_F16 / TF32 -- at n <= 40 hypotheses they are
 // weight-streaming launches of the persistent one-CTA kernel, the S1 regime of the encoder --, CUDA-core gemm_simt for
 // AVSR_PREC_FP32), LayerNorm and log-softmax are the encoder path's kernels; the attention over the slot-addressed K/V
 // cache, the embedding and the CTC forward recursion are per-element functors launched as plain grids (one thread per

@@ -1,5 +1,5 @@
 // Attention-decoder scoring path (SURVEY.md 8f #3): buffer layouts, per-element functors and the launch schedule,
-// written against a small backend interface so that ONE source drives both the device library (decoder.cu: tcgen05 /
+// written against a small backend interface so that ONE source drives both the device library (decoder.cu: wgmma /
 // CUDA-core GEMMs, the LayerNorm / log-softmax kernels of the encoder path, functors as grid kernels) and the host
 // replay the CPU tests build (tests/emu/decoder_emu.cu: the same schedule and the same functors as plain loops --
 // test infrastructure, never loaded by the package).
@@ -10,7 +10,7 @@
 //   CTCPrefixScoreTH.__call__                           espnet/nets/ctc_prefix_score.py:72-200
 //   CTCPrefixScorer.select_state                        espnet/nets/scorers/ctc.py:37-60
 //
-// Design (B200-first, not the reference's): the reference caches every layer's OUTPUT per hypothesis and re-projects
+// Design (GPU-first, not the reference's): the reference caches every layer's OUTPUT per hypothesis and re-projects
 // K/V of the whole prefix -- and of the whole encoder memory -- at every step, then copies the caches around when
 // the beam is re-ordered.  Here K/V are projected once: the source-attention K/V of all layers when an utterance
 // starts, the self-attention K/V of a position when it is decoded, written straight into a slot (layer, position,

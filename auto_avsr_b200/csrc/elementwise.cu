@@ -27,7 +27,7 @@ int launch_embed_scale(const float* xs, float* x, long n, float scale, cudaStrea
   AVSR_REQUIRE(n % 4 == 0, "embed: element count %ld not a multiple of 4", n);
   long n4 = n / 4;
   int blocks = (int)((n4 + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   if (blocks < 1) blocks = 1;
   AVSR_LAUNCH(embed_scale_kernel, blocks, 256, 0, st, (const float4*)xs, (float4*)x, n4, scale);
   return AVSR_OK;
@@ -36,16 +36,12 @@ int launch_embed_scale(const float* xs, float* x, long n, float scale, cudaStrea
 // ------------------------------------------------------------------ LayerNorm (layer_norm.py:21, eps 1e-12)
 // A row (d <= 1024 channels) is held in registers by WPR warps (1, 2 or 4): HBM / L2 sees exactly one read and one
 // write per element.  Two-pass mean / centred variance; warp-shuffle reductions, combined across the row's warps
-// through shared memory in a fixed order (deterministic).  The r02 launch timeline showed these kernels to be bound by
-// the latency of one load -> reduce -> store chain per warp (1 600 warps on 148 SMs is a single, half-empty wave), so
-// the geometry is a launch parameter: more warps per row = shorter chains and more loads in flight per SM.
+// through shared memory in a fixed order (deterministic).  At the encoder's sizes a LayerNorm is bound by the latency of
+// one load -> reduce -> store chain per warp (1 600 rows are a single, partly filled wave), so the geometry is a launch
+// parameter: more warps per row = shorter chains and more loads in flight per SM.
 //   TWO = false : y = LN(x; g1, b1)                                   (y in operand storage or fp32)
 //   TWO = true  : y1 = LN(x; g1, b1) (fp32, may alias x) and y = LN(y1; g2, b2) in operand storage -- layer l's
 //                 norm_final followed by layer l+1's norm_ff_macaron (conformer_encoder.py:161-162 then :113).
-//   NP > 0      : deferred split-K residual update applied while the row is loaded (LnParts): row = x + alpha *
-//                 (bias + part[0] + ... + part[NP-1]), fixed order; the updated row is written to pp.x_out when that
-//                 is not already the kernel's own fp32 output.  All loads of the row are issued before the first use
-//                 and before any store (a store in between would serialise them: possible aliasing).
 constexpr int kLnMaxVec = 8;  // float4 per lane at WPR = 1: 8 * 32 lanes * 4 = 1024 channels
 
 __device__ __forceinline__ void ln_named_bar(int id, int nthreads) {
@@ -65,15 +61,15 @@ __device__ __forceinline__ float ln_row_sum(float v, float* slot, int wr, int la
   return t;
 }
 
-template <int NP, bool TWO, int WPR, int RPC, int V>   // V = float4 per lane: WPR * 32 * V * 4 >= d
+template <bool TWO, int WPR, int RPC, int V>   // V = float4 per lane: WPR * 32 * V * 4 >= d
 __global__ void __launch_bounds__(32 * WPR * RPC)
-ln_kernel(const float* x /* may alias y1 / pp.x_out */, const float* __restrict__ g1, const float* __restrict__ b1,
+ln_kernel(const float* x /* may alias y1 */, const float* __restrict__ g1, const float* __restrict__ b1,
           const float* __restrict__ g2, const float* __restrict__ b2, float* y1, void* y, int rows, int d,
-          int out_kind, LnParts pp) {
+          int out_kind) {
   constexpr int STEP = 32 * WPR;                // float4 stride between a lane's vectors
   __shared__ float red[4][RPC][WPR];
   pdl_launch_dependents();
-  AVSR_TSPAN_OPEN(TWO ? 110 : 100, NP | (WPR << 8) | (RPC << 12));
+  AVSR_TSPAN_OPEN(TWO ? 110 : 100, (WPR << 8) | (RPC << 12));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rl = warp / WPR, wr = warp - rl * WPR;      // row inside the CTA, warp inside the row
   const int row = blockIdx.x * RPC + rl;
@@ -90,14 +86,6 @@ ln_kernel(const float* x /* may alias y1 / pp.x_out */, const float* __restrict_
       if constexpr (TWO) { gg2[i] = reinterpret_cast<const float4*>(g2)[c]; bb2[i] = reinterpret_cast<const float4*>(b2)[c]; }
     }
   }
-  float4 pb[NP > 0 ? V : 1];
-  if constexpr (NP > 0) {
-#pragma unroll
-    for (int i = 0; i < V; ++i) {
-      const int c = c0 + i * STEP;
-      if (c < nvec) pb[i] = reinterpret_cast<const float4*>(pp.bias)[c];
-    }
-  }
   pdl_wait();
   AVSR_TSPAN_DEP();
   const long rv = (long)row * nvec;
@@ -107,25 +95,6 @@ ln_kernel(const float* x /* may alias y1 / pp.x_out */, const float* __restrict_
   for (int i = 0; i < V; ++i) {
     const int c = c0 + i * STEP;
     if (c < nvec) v[i] = xr[c];
-  }
-  if constexpr (NP > 0) {
-    const float4* p4 = reinterpret_cast<const float4*>(pp.part) + rv;
-    const long sv = pp.stride >> 2;
-    float4 t[NP][V];
-#pragma unroll
-    for (int s = 0; s < NP; ++s)
-#pragma unroll
-      for (int i = 0; i < V; ++i) {
-        const int c = c0 + i * STEP;
-        if (c < nvec) t[s][i] = p4[s * sv + c];
-      }
-#pragma unroll
-    for (int i = 0; i < V; ++i) {
-      float4 a = pb[i];
-#pragma unroll
-      for (int s = 0; s < NP; ++s) { a.x += t[s][i].x; a.y += t[s][i].y; a.z += t[s][i].z; a.w += t[s][i].w; }
-      v[i].x += pp.alpha * a.x; v[i].y += pp.alpha * a.y; v[i].z += pp.alpha * a.z; v[i].w += pp.alpha * a.w;
-    }
   }
   const int bar_id = 1 + rl;
   float s = 0.f;
@@ -146,7 +115,6 @@ ln_kernel(const float* x /* may alias y1 / pp.x_out */, const float* __restrict_
     for (int i = 0; i < V; ++i) {
       const int c = c0 + i * STEP;
       if (c < nvec) {
-        if (NP > 0 && pp.x_out) reinterpret_cast<float4*>(pp.x_out)[rv + c] = v[i];
         const float4 o = make_float4((v[i].x - mean) * rstd * gg[i].x + bb[i].x, (v[i].y - mean) * rstd * gg[i].y + bb[i].y,
                                      (v[i].z - mean) * rstd * gg[i].z + bb[i].z, (v[i].w - mean) * rstd * gg[i].w + bb[i].w);
         if (y1) reinterpret_cast<float4*>(y1)[rv + c] = o;       // dual output: the fp32 copy (after_norm -> features)
@@ -197,25 +165,28 @@ static LnGeom ln_geom(int d) {
     if (const char* e = getenv("AVSR_B200_LN")) { if (sscanf(e, "%dx%d", &g.wpr, &g.rpc) != 2) g = LnGeom{0, 0}; }
     return g;
   }();
-  LnGeom g = env.wpr ? env : LnGeom{2, 4};   // r02 sweep (profiles/r02_ln_sweep.txt): 2x4 best in situ
+  LnGeom g = env.wpr ? env : LnGeom{2, 4};   // 2 warps per row x 4 rows per CTA
   (void)d;
   return g;
 }
 
-template <int NP, bool TWO>
-static int launch_ln_np(const float* x, const float* g1, const float* b1, const float* g2, const float* b2, float* y1,
-                        void* y, int rows, int d, int out_kind, cudaStream_t st, const LnParts& pp) {
+template <bool TWO>
+static int launch_ln(const float* x, const float* g1, const float* b1, const float* g2, const float* b2, float* y1,
+                     void* y, int rows, int d, int out_kind, cudaStream_t st) {
+  AVSR_REQUIRE(d % 4 == 0 && d <= kLnMaxVec * 128 && d > 0, "layernorm: d=%d must be a multiple of 4 and <= %d", d,
+               kLnMaxVec * 128);
+  if (rows <= 0) return AVSR_OK;
   const LnGeom g = ln_geom(d);
   // vectors per lane: the reference's d = 768 needs 6 / 3 / 2 at 1 / 2 / 4 warps per row; up to 1024 channels 8 / 4 / 2
   const bool small = d <= 768;
 #define AVSR_LN_CASE(W, R, VS, VL)                                                                                  \
   if (g.wpr == W && g.rpc == R) {                                                                                   \
     if (small)                                                                                                      \
-      AVSR_LAUNCH((ln_kernel<NP, TWO, W, R, VS>), cdiv(rows, R), 32 * W * R, 0, st, x, g1, b1, g2, b2, y1, y, rows, \
-                  d, out_kind, pp);                                                                                 \
+      AVSR_LAUNCH((ln_kernel<TWO, W, R, VS>), cdiv(rows, R), 32 * W * R, 0, st, x, g1, b1, g2, b2, y1, y, rows, \
+                  d, out_kind);                                                                                     \
     else                                                                                                            \
-      AVSR_LAUNCH((ln_kernel<NP, TWO, W, R, VL>), cdiv(rows, R), 32 * W * R, 0, st, x, g1, b1, g2, b2, y1, y, rows, \
-                  d, out_kind, pp);                                                                                 \
+      AVSR_LAUNCH((ln_kernel<TWO, W, R, VL>), cdiv(rows, R), 32 * W * R, 0, st, x, g1, b1, g2, b2, y1, y, rows, \
+                  d, out_kind);                                                                                     \
     return AVSR_OK;                                                                                                 \
   }
   AVSR_LN_CASE(1, 8, 6, 8) AVSR_LN_CASE(1, 2, 6, 8)
@@ -226,36 +197,19 @@ static int launch_ln_np(const float* x, const float* g1, const float* b1, const 
   return AVSR_OK;
 }
 
-template <bool TWO>
-static int launch_ln(const float* x, const float* g1, const float* b1, const float* g2, const float* b2, float* y1,
-                     void* y, int rows, int d, int out_kind, cudaStream_t st, const LnParts* parts) {
-  AVSR_REQUIRE(d % 4 == 0 && d <= kLnMaxVec * 128 && d > 0, "layernorm: d=%d must be a multiple of 4 and <= %d", d,
-               kLnMaxVec * 128);
-  if (rows <= 0) return AVSR_OK;
-  const LnParts pp = parts ? *parts : LnParts{};
-  switch (pp.nparts) {
-    case 0: return launch_ln_np<0, TWO>(x, g1, b1, g2, b2, y1, y, rows, d, out_kind, st, pp);
-    case 2: return launch_ln_np<2, TWO>(x, g1, b1, g2, b2, y1, y, rows, d, out_kind, st, pp);
-    case 3: return launch_ln_np<3, TWO>(x, g1, b1, g2, b2, y1, y, rows, d, out_kind, st, pp);
-    case 4: return launch_ln_np<4, TWO>(x, g1, b1, g2, b2, y1, y, rows, d, out_kind, st, pp);
-    default: AVSR_REQUIRE(false, "layernorm: %d k-slices not instantiated (0, 2, 3, 4)", pp.nparts);
-  }
-  return AVSR_OK;
-}
-
 int launch_layernorm2(const float* x, const float* g1, const float* b1, const float* g2, const float* b2, float* y1,
-                      void* y2, int rows, int d, int out_kind, cudaStream_t st, const LnParts* parts) {
-  return launch_ln<true>(x, g1, b1, g2, b2, y1, y2, rows, d, out_kind, st, parts);
+                      void* y2, int rows, int d, int out_kind, cudaStream_t st) {
+  return launch_ln<true>(x, g1, b1, g2, b2, y1, y2, rows, d, out_kind, st);
 }
 
 int launch_layernorm(const float* x, const float* g, const float* b, void* y, int rows, int d, int out_kind,
-                     cudaStream_t st, const LnParts* parts) {
-  return launch_ln<false>(x, g, b, nullptr, nullptr, nullptr, y, rows, d, out_kind, st, parts);
+                     cudaStream_t st) {
+  return launch_ln<false>(x, g, b, nullptr, nullptr, nullptr, y, rows, d, out_kind, st);
 }
 
 int launch_layernorm_dual(const float* x, const float* g, const float* b, float* y_f32, void* y_op, int rows, int d,
                           int out_kind, cudaStream_t st) {
-  return launch_ln<false>(x, g, b, nullptr, nullptr, y_f32, y_op, rows, d, out_kind, st, nullptr);
+  return launch_ln<false>(x, g, b, nullptr, nullptr, y_f32, y_op, rows, d, out_kind, st);
 }
 
 // ------------------------------------------------------------------ rel-pos sinusoid table (embedding.py:139-184)
@@ -294,7 +248,7 @@ int launch_sinusoid(void* pe, int T, int d, int out_kind, cudaStream_t st) {
   AVSR_REQUIRE(T > 0 && d > 0 && d % 2 == 0, "sinusoid: bad T=%d d=%d", T, d);
   const long total = (long)(2 * T - 1) * (d / 2);
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   AVSR_LAUNCH(sinusoid_kernel, blocks, 256, 0, st, pe, T, d, out_kind);
   return AVSR_OK;
 }

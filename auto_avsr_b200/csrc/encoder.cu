@@ -125,7 +125,7 @@ __global__ void dw_fold_kernel(const float* __restrict__ w, const float* __restr
 static int copy_round(const float* src, void* dst, long n, int kind, cudaStream_t st, float scale = 1.0f) {
   if (n <= 0) return AVSR_OK;
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   copy_round_kernel<<<blocks, 256, 0, st>>>(src, dst, n, kind, scale);
   AVSR_CHECK_LAUNCH();
   return AVSR_OK;
@@ -219,7 +219,7 @@ static int count_saturated(const void* halfs, size_t nelems, unsigned long long*
   if (!count || nelems == 0) return AVSR_OK;
   AVSR_REQUIRE(nelems % 8 == 0 && (reinterpret_cast<uintptr_t>(halfs) & 15) == 0, "saturation scan: unaligned buffer");
   int blocks = (int)((nelems / 8 + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   count_saturated_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const uint4*>(halfs), (long)(nelems / 8), count);
   AVSR_CHECK_LAUNCH();
   return AVSR_OK;
@@ -278,10 +278,6 @@ static int forward_body(const AvsrEncoderConfig& c, const Prepared& P, const Wor
   const size_t stage_bytes = (size_t)N * D * sizeof(float);
   if (prec != AVSR_PREC_F16) sat = nullptr;     // only the fp16 operand storage saturates
   auto chk = [&](const void* buf, size_t nelems) -> int { return count_saturated(buf, nelems, sat, st); };
-  struct StaticWeights {                        // every GEMM below reads prepared weights (see g_tc2_weights_static)
-    StaticWeights() { g_tc2_weights_static = true; }
-    ~StaticWeights() { g_tc2_weights_static = false; }
-  } static_weights_scope;
 
   // split-K tile counters must be zero on entry (they re-arm themselves; this covers a first use / an aborted run)
   AVSR_CUDA_TRY(cudaMemsetAsync(W.counters, 0, kSplitCounters * sizeof(int), st));
@@ -299,16 +295,6 @@ static int forward_body(const AvsrEncoderConfig& c, const Prepared& P, const Wor
   if (W.Tp != T && prec != AVSR_PREC_F16)
     AVSR_CUDA_TRY(cudaMemsetAsync(W.vt, 0, (size_t)B * D * W.Tp * sizeof(float), st));
 
-  // FFN w_2 (K = linear_units) as a deferred split-K GEMM: k-slices land in W.splitk and the LayerNorm that follows
-  // applies x += 0.5 * (sum of slices + b) while it loads the row.  Not with `taps` (they read x between the two).
-  int w2_bnp = 0, w2_split = 0;
-  const bool w2_defer = prec == AVSR_PREC_F16 && !taps && gemm_tc2_splitk_plan(N, D, F, &w2_bnp, &w2_split);
-  auto w2_parts = [&](const float* bias, float* x_out) {
-    LnParts pp;
-    pp.part = W.splitk; pp.nparts = w2_split; pp.stride = (long)N * D; pp.bias = bias; pp.alpha = 0.5f; pp.x_out = x_out;
-    return pp;
-  };
-
   for (int l = 0; l < L; ++l) {
     const LayerPrep& w = P.layers[l];
     auto tap = [&](int s) -> int {
@@ -322,18 +308,11 @@ static int forward_body(const AvsrEncoderConfig& c, const Prepared& P, const Wor
     AVSR_TRY(chk(W.xn, (size_t)N * D));
     AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.xn, w.ffm_w1, N, F, D, epi_linear(N, F, w.ffm_b1, W.hid, nullptr, 0.f, 1, opr), st));
     AVSR_TRY(chk(W.hid, (size_t)N * F));
-    if (w2_defer) {
-      AVSR_TRY(gemm_tc2_splitk(W.hid, w.ffm_w2, N, D, F, W.splitk, w2_bnp, w2_split, st));
-    } else {
-      AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.hid, w.ffm_w2, N, D, F, epi_resid(N, D, w.ffm_b2, W.x, 0.5f, W.splitk, W.counters), st));
-      AVSR_TRY(tap(0));
-    }
+    AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.hid, w.ffm_w2, N, D, F, epi_resid(N, D, w.ffm_b2, W.x, 0.5f, W.splitk, W.counters), st));
+    AVSR_TRY(tap(0));
     // (2) rel-pos MHA: x += out(attn(LN(x)))                                  conformer_encoder.py:119-142
-    {
-      const LnParts pp = w2_parts(w.ffm_b2, W.x);
-      AVSR_TRY(launch_layernorm(W.x, w.ln_mha_w, w.ln_mha_b, W.xn, N, D, opk, st, w2_defer ? &pp : nullptr));
-      AVSR_TRY(chk(W.xn, (size_t)N * D));
-    }
+    AVSR_TRY(launch_layernorm(W.x, w.ln_mha_w, w.ln_mha_b, W.xn, N, D, opk, st));
+    AVSR_TRY(chk(W.xn, (size_t)N * D));
     {
       EpiParams e{};
       e.M = N; e.bias = w.qk_b; e.T = T; e.H = H; e.pos_u = w.pos_u; e.pos_v = w.pos_v;
@@ -384,24 +363,16 @@ static int forward_body(const AvsrEncoderConfig& c, const Prepared& P, const Wor
     AVSR_TRY(chk(W.xn, (size_t)N * D));
     AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.xn, w.ff_w1, N, F, D, epi_linear(N, F, w.ff_b1, W.hid, nullptr, 0.f, 1, opr), st));
     AVSR_TRY(chk(W.hid, (size_t)N * F));
-    if (w2_defer) {
-      AVSR_TRY(gemm_tc2_splitk(W.hid, w.ff_w2, N, D, F, W.splitk, w2_bnp, w2_split, st));
-    } else {
-      AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.hid, w.ff_w2, N, D, F, epi_resid(N, D, w.ff_b2, W.x, 0.5f, W.splitk, W.counters), st));
-      AVSR_TRY(tap(3));
-    }
+    AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.hid, w.ff_w2, N, D, F, epi_resid(N, D, w.ff_b2, W.x, 0.5f, W.splitk, W.counters), st));
+    AVSR_TRY(tap(3));
     // (5) x = LN_final(x)                                                     conformer_encoder.py:161-162
     //     fused with the next layer's norm_ff_macaron: one pass writes x (fp32) and xn (operand)
-    {
-      const LnParts pp = w2_parts(w.ff_b2, nullptr);   // the LayerNorm's own fp32 output replaces x
-      const LnParts* ppp = w2_defer ? &pp : nullptr;
-      if (l + 1 < L) {
-        const LayerPrep& nx = P.layers[l + 1];
-        AVSR_TRY(launch_layernorm2(W.x, w.ln_fin_w, w.ln_fin_b, nx.ln_ffm_w, nx.ln_ffm_b, W.x, W.xn, N, D, opk, st, ppp));
-        // (the next iteration's first check covers this xn)
-      } else {
-        AVSR_TRY(launch_layernorm(W.x, w.ln_fin_w, w.ln_fin_b, W.x, N, D, OP_F32, st, ppp));
-      }
+    if (l + 1 < L) {
+      const LayerPrep& nx = P.layers[l + 1];
+      AVSR_TRY(launch_layernorm2(W.x, w.ln_fin_w, w.ln_fin_b, nx.ln_ffm_w, nx.ln_ffm_b, W.x, W.xn, N, D, opk, st));
+      // (the next iteration's first check covers this xn)
+    } else {
+      AVSR_TRY(launch_layernorm(W.x, w.ln_fin_w, w.ln_fin_b, W.x, N, D, OP_F32, st));
     }
     AVSR_TRY(tap(4));
   }
@@ -438,7 +409,7 @@ static int plan_branches(int B, int T, int precision) {
   if (precision != AVSR_PREC_F16 || want < 2) return 1;
   if (want > kMaxBranches) want = kMaxBranches;
   if (want > B) want = B;
-  while (want > 1 && (long)(B / want) * T < 256) --want;   // every slice must still feed the two-SM GEMMs (M >= 256)
+  while (want > 1 && (long)(B / want) * T < 256) --want;   // slices of fewer than 256 rows leave GEMM tiles half empty
   return want;
 }
 
@@ -447,7 +418,7 @@ static int plan_branches(int B, int T, int precision) {
 // log_softmax behind (ctc.py:21,77-84).  Prepared once per parameter update: proj weights in operand storage, both
 // plain and pre-multiplied by sqrt(d_model) (the encoder's embed scale, embedding.py:178, folded into the projection
 // that writes the residual stream); ctc_lo weights in operand storage with odim padded to a multiple of 512 (zero
-// rows; the pair tile of the two-SM GEMM) and the bias padded likewise.
+// rows) and the bias padded likewise.
 struct HeadPrep {
   float *proj_w, *proj_b, *proj_ws, *proj_bs, *ctc_w, *ctc_b;
   int npad;
@@ -469,7 +440,6 @@ struct HeadWorkspace {
   void* enc;          // the encoder's own workspace (layout_workspace)
   size_t enc_bytes;
   float *fx, *logits;
-  LsePart* parts;
   size_t bytes;
 };
 static HeadWorkspace layout_head_workspace(const AvsrEncoderConfig& c, int B, int T, int idim, int odim, void* base) {
@@ -481,20 +451,14 @@ static HeadWorkspace layout_head_workspace(const AvsrEncoderConfig& c, int B, in
   Carver cv{reinterpret_cast<char*>(base) + W.enc_bytes};
   W.fx = cv.take(N * (size_t)(idim > c.d_model ? idim : c.d_model));   // operand copy of the features / of hs
   W.logits = cv.take(N * (size_t)npad);
-  W.parts = reinterpret_cast<LsePart*>(cv.take((size_t)2 * (npad / 512) * N * (sizeof(LsePart) / sizeof(float))));
   W.bytes = W.enc_bytes + cv.off;
   return W;
 }
 
 // hs_op (rows, d_model) in operand storage -> logp (rows, odim) fp32 log-probabilities [+ arg max]
 static int ctc_logprobs(const AvsrEncoderConfig& c, const HeadPrep& H, const void* hs_op, int rows, int odim, float* logits,
-                        LsePart* parts, float* logp, int32_t* argmax, int prec, cudaStream_t st) {
+                        float* logp, int32_t* argmax, int prec, cudaStream_t st) {
   const int D = c.d_model;
-  if (prec == AVSR_PREC_F16 && gemm_tc2_lse_ok(rows, H.npad, D)) {
-    int nparts = 0;
-    AVSR_TRY(gemm_tc2_lse(hs_op, H.ctc_w, H.ctc_b, rows, H.npad, D, odim, logits, H.npad, parts, &nparts, st));
-    return launch_lse_finish(logits, H.npad, parts, nparts, rows, logp, odim, argmax, odim, st);
-  }
   AVSR_TRY(run_gemm(prec, EPI_LINEAR, hs_op, H.ctc_w, rows, H.npad, D, epi_linear(rows, H.npad, H.ctc_b, logits, nullptr, 0.f, 0, 0), st));
   return launch_log_softmax_rows(logits, H.npad, logp, odim, argmax, rows, odim, st);
 }
@@ -515,8 +479,8 @@ static int head_forward_body(const AvsrEncoderConfig& c, const Prepared& P, cons
   // (3) after_norm: fp32 features for the caller (attention decoder / beam search) + the operand of ctc_lo in one pass
   float* feat_out = enc_out ? enc_out : W.x;
   AVSR_TRY(launch_layernorm_dual(W.x, P.after_w, P.after_b, feat_out, W.xn, N, D, operand_kind(precision), st));
-  // (4) ctc_lo + log_softmax: GEMM with log-sum-exp partials in its epilogue, one finishing pass
-  return ctc_logprobs(c, H, W.xn, N, odim, HW.logits, HW.parts, logp, argmax, precision, st);
+  // (4) ctc_lo + log_softmax: GEMM into fp32 logits, then the row-wise log-softmax / arg-max kernel
+  return ctc_logprobs(c, H, W.xn, N, odim, HW.logits, logp, argmax, precision, st);
 }
 
 }  // namespace avsr
@@ -537,12 +501,10 @@ struct AvsrPlan {
 
 #ifdef AVSR_TRACE
 namespace avsr {
-int trace_bind_gemm_tc2(unsigned long long*);
-int trace_bind_attention_f16(unsigned long long*);
 int trace_bind_elementwise(unsigned long long*);
 int trace_bind_gemm_tc(unsigned long long*);
 static int trace_bind_all(unsigned long long* p) {
-  return trace_bind_gemm_tc2(p) | trace_bind_attention_f16(p) | trace_bind_elementwise(p) | trace_bind_gemm_tc(p);
+  return trace_bind_elementwise(p) | trace_bind_gemm_tc(p);
 }
 }
 // diagnostic build only (scripts/build_trace.py): device buffer of `words` 64-bit words, see common.cuh "phase trace"
@@ -858,7 +820,7 @@ int avsr_relpos_attention(const float* q, const float* k, const float* v, const 
   Carver cv{reinterpret_cast<char*>(workspace)};
   float *qu = cv.take(N * D), *qv = cv.take(N * D), *kk = cv.take(N * D), *vt = cv.take((size_t)B * D * Tp),
         *pos = cv.take((size_t)R * D), *ctxh = cv.take(N * D);
-  const int blocks = 148 * 4;
+  const int blocks = 132 * 4;
   if (Tp != T) AVSR_CUDA_TRY(cudaMemsetAsync(vt, 0, (size_t)B * D * Tp * sizeof(float), st));
   split_heads_kernel<<<blocks, 256, 0, st>>>(q, pos_bias_u, qu, B, T, H, Tp, 0, kind); AVSR_CHECK_LAUNCH();
   split_heads_kernel<<<blocks, 256, 0, st>>>(q, pos_bias_v, qv, B, T, H, Tp, 0, kind); AVSR_CHECK_LAUNCH();
@@ -983,8 +945,7 @@ int avsr_proj_encoder(const AvsrEncoderConfig* cfg, const void* prepared_head, c
 size_t avsr_ctc_workspace_bytes(const AvsrEncoderConfig* cfg, int rows, int odim) {
   if (check_cfg(cfg) != AVSR_OK || rows < 0 || odim <= 0) return 0;
   const size_t npad = align_up((size_t)odim, 512);
-  return align_up((size_t)rows * cfg->d_model * 4, 256) + align_up((size_t)rows * npad * 4, 256) +
-         align_up((size_t)2 * (npad / 512) * rows * sizeof(LsePart), 256) + 256;
+  return align_up((size_t)rows * cfg->d_model * 4, 256) + align_up((size_t)rows * npad * 4, 256) + 256;
 }
 
 int avsr_ctc_logprobs(const AvsrEncoderConfig* cfg, const void* prepared_head, const float* hs, int rows, int idim,
@@ -1003,10 +964,9 @@ int avsr_ctc_logprobs(const AvsrEncoderConfig* cfg, const void* prepared_head, c
   Carver cv{reinterpret_cast<char*>(workspace)};
   float* hx = cv.take((size_t)rows * cfg->d_model);
   float* logits = cv.take((size_t)rows * H.npad);
-  LsePart* parts = reinterpret_cast<LsePart*>(cv.take((size_t)2 * (H.npad / 512) * rows * (sizeof(LsePart) / sizeof(float))));
   const void* hs_op = hs;
   if (precision != AVSR_PREC_FP32) { AVSR_TRY(copy_round(hs, hx, (long)rows * cfg->d_model, operand_kind(precision), st)); hs_op = hx; }
-  return ctc_logprobs(*cfg, H, hs_op, rows, odim, logits, parts, logp, argmax, precision, st);
+  return ctc_logprobs(*cfg, H, hs_op, rows, odim, logits, logp, argmax, precision, st);
 }
 
 int avsr_features_to_logprobs(const AvsrEncoderConfig* cfg, const void* prepared, const void* prepared_head,

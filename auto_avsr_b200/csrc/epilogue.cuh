@@ -1,16 +1,15 @@
-// Staged (coalesced) epilogue helpers shared by gemm_tc.cu (1-CTA, persistent) and gemm_tc2.cu (two-SM).
+// Staged (coalesced) epilogue helpers of the tensor-core GEMM (gemm_tc.cu).
 #pragma once
 #include "common.cuh"
 
 namespace avsr {
 
 // ---------------------------------------------------------------- staged (coalesced) epilogue
-// Each epilogue warp drains 32 accumulator rows x CW columns at a time: lane = row out of TMEM (tcgen05.ld), per-
+// Each epilogue warp drains 32 accumulator rows x CW columns at a time: lane = row of the fp32 accumulator tile, per-
 // column math (bias / ReLU / GLU / pos biases, vectors read from shared memory), conversion to the destination
-// storage, then a transpose through a private 32 x 144-byte staging buffer (carved from the pipeline stages, which
-// are idle once the accumulator is complete) so that global memory sees, per quarter-warp, 8 lanes x 16 B = one full
-// 128-byte row segment -- instead of 32 partial sectors per store instruction (r01 profile: the direct
-// lane-per-row stores made the epilogue 4x longer than the MMA main loop).  Residual reads use the same mapping.
+// storage, then a transpose through a private 32 x 144-byte staging buffer so that global memory sees, per
+// quarter-warp, 8 lanes x 16 B = one full 128-byte row segment -- instead of 32 partial sectors per store instruction
+// of direct lane-per-row stores.  Residual reads use the same mapping.
 constexpr int STG_ROW = 144;            // 128 B payload + 16 B pad: conflict-free lane-per-row 16-byte writes
 constexpr int STG_WARP = 32 * STG_ROW;  // 4608 B per epilogue warp
 

@@ -79,52 +79,6 @@ __global__ void __launch_bounds__(256) log_softmax_rows_kernel(const float* __re
   for (int c = threadIdx.x; c < n; c += 256) yr[c] = xr[c] - shift;
 }
 
-// Second half of the fused CTC head: the ctc_lo GEMM's epilogue (gemm_tc2.cu, EPI_LSE) left fp32 logits and, per row,
-// `nparts` log-sum-exp partials (max, sum exp(x - max), first arg max) over disjoint column ranges.  One CTA per row:
-// warp 0 merges the partials (fixed order: deterministic), then all threads write y = logit - lse over the n valid
-// columns -- ONE read of the logits instead of the two passes of log_softmax_rows_kernel.
-__global__ void __launch_bounds__(256) lse_finish_kernel(const float* __restrict__ logits, long ldx,
-                                                         const LsePart* __restrict__ part, int nparts, long rows_ld,
-                                                         float* __restrict__ y, long ldy, int32_t* __restrict__ best,
-                                                         int n) {
-  pdl_launch_dependents();
-  __shared__ float s_shift;
-  const int row = blockIdx.x;
-  pdl_wait();
-  if (threadIdx.x < 32) {
-    MaxSum acc{-INFINITY, 0.f, 0x7fffffff};
-    for (int p = threadIdx.x; p < nparts; p += 32) {
-      const LsePart t = part[(long)p * rows_ld + row];
-      acc = ms_merge(acc, MaxSum{t.m, t.s, t.idx});
-    }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      MaxSum o;
-      o.m = __shfl_xor_sync(0xffffffffu, acc.m, off);
-      o.s = __shfl_xor_sync(0xffffffffu, acc.s, off);
-      o.i = __shfl_xor_sync(0xffffffffu, acc.i, off);
-      acc = ms_merge(acc, o);
-    }
-    if (threadIdx.x == 0) {
-      s_shift = acc.m + logf(acc.s);
-      if (best) best[row] = acc.i;
-    }
-  }
-  __syncthreads();
-  if (!y) return;
-  const float shift = s_shift;
-  const float* xr = logits + (long)row * ldx;
-  float* yr = y + (long)row * ldy;
-  for (int c = threadIdx.x; c < n; c += 256) yr[c] = xr[c] - shift;
-}
-
-int launch_lse_finish(const float* logits, long ldx, const LsePart* part, int nparts, int rows, float* y, long ldy,
-                      int32_t* best, int n, cudaStream_t st) {
-  if (rows <= 0) return AVSR_OK;
-  AVSR_LAUNCH(lse_finish_kernel, rows, 256, 0, st, logits, ldx, part, nparts, (long)rows, y, ldy, best, n);
-  return AVSR_OK;
-}
-
 int launch_log_softmax_rows(const float* x, long ldx, float* y, long ldy, int32_t* best, int rows, int n, cudaStream_t st) {
   if (rows <= 0) return AVSR_OK;
   AVSR_LAUNCH(log_softmax_rows_kernel, rows, 256, 0, st, x, ldx, y, ldy, best, rows, n);

@@ -1,6 +1,6 @@
 // Training slice of the encoder path (SURVEY.md 8f #2, first slice): backward of the HBM-bound kernels and the pieces a
 // Linear's backward needs around the tensor-core GEMMs -- LayerNorm backward, bias gradients (column sums), fp32
-// transpose (so that dgrad / wgrad are the SAME tcgen05 GEMMs on transposed operands), ReLU backward, and the
+// transpose (so that dgrad / wgrad are the SAME wgmma GEMMs on transposed operands), ReLU backward, and the
 // depthwise-conv + BatchNorm(batch statistics) + SiLU block forward / backward incl. the running-statistics update.
 // Reference: lightning.py:86-94 (training_step), conformer_encoder.py:26,30-35 (BatchNorm1d in train mode sees ALL B*T
 // frames incl. padding), layer_norm.py:21, positionwise_feed_forward.py:28-30.  fp32 math; every cross-row reduction is
@@ -11,7 +11,7 @@
 
 namespace avsr {
 
-constexpr int kRedBlocks = 148;      // first-stage CTAs of every column reduction (one per SM)
+constexpr int kRedBlocks = 132;      // first-stage CTAs of every column reduction (one per SM)
 constexpr int kTrMaxVec = 8;         // float4 per lane: rows of up to 1024 channels
 
 // ------------------------------------------------------------------ LayerNorm backward
@@ -264,7 +264,7 @@ __global__ void fill_kernel(float* p, int n, float v) {
   if (i < n) p[i] = v;
 }
 
-static inline int grid_for(long n, int per = 256, int cap = 148 * 8) {
+static inline int grid_for(long n, int per = 256, int cap = 132 * 8) {
   long g = (n + per - 1) / per;
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }

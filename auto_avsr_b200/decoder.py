@@ -38,7 +38,7 @@ class _Ctx:
 
     def require(self, t: torch.Tensor, what: str, dtype=torch.float32) -> None:
         if not t.is_cuda and not self.emulated:
-            raise RuntimeError(f"{what}: tensor is on {t.device}; the B200 decoder path has no CPU fallback "
+            raise RuntimeError(f"{what}: tensor is on {t.device}; the CUDA decoder path has no CPU fallback "
                                "(move the module and its inputs to a CUDA device)")
         if t.dtype != dtype:
             raise TypeError(f"{what}: expected {dtype}, got {t.dtype}")

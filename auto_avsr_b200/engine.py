@@ -30,7 +30,7 @@ def _stream_handle(device) -> int:
 def require_cuda(t: torch.Tensor, what: str) -> None:
     if not t.is_cuda:
         raise RuntimeError(
-            f"{what}: tensor is on {t.device}; the B200 encoder path has no CPU fallback "
+            f"{what}: tensor is on {t.device}; the CUDA encoder path has no CPU fallback "
             "(move the module and its inputs to a CUDA device)")
     if t.dtype != torch.float32:
         raise TypeError(f"{what}: expected float32, got {t.dtype}")

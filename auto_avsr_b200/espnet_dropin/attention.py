@@ -24,7 +24,7 @@ def mask_to_lengths(mask: torch.Tensor, B: int, T: int, check: bool = False) -> 
     if check:
         prefix = torch.arange(T, device=mask.device)[None, :] < lengths[:, None]
         if not bool(torch.equal(prefix, m)):
-            raise NotImplementedError("key mask is not prefix-contiguous (holes / left padding): the B200 path takes "
+            raise NotImplementedError("key mask is not prefix-contiguous (holes / left padding): the CUDA path takes "
                                       "lengths, i.e. make_non_pad_mask-style masks only")
     return lengths
 

@@ -3,7 +3,7 @@
 Same class names, constructor signatures, sub-module / parameter names and state-dict keys as the
 reference (espnet/nets/pytorch_backend/encoder/conformer_encoder.py:19,38,186), so ``E2E``
 (e2e_asr_conformer.py:33-39), ``lightning.py`` and the released checkpoints keep working unchanged;
-only ``forward`` differs: on a CUDA tensor it runs the hand-written sm_100a kernels of libavsr_b200.so.
+only ``forward`` differs: on a CUDA tensor it runs the hand-written sm_90a kernels of libavsr_b200.so.
 
 Scope: inference forward (``eval()``: one fused C-ABI call, outputs carry no autograd graph) plus the FIRST SLICE of
 training (SURVEY.md section 8f item 2): ``LayerNorm``, ``PositionwiseFeedForward`` and ``ConvolutionModule`` run forward
@@ -33,7 +33,7 @@ from .repeat import repeat
 def _inference_only(module: torch.nn.Module, what: str) -> None:
     if module.training:
         raise NotImplementedError(
-            f"{what}: the B200 path implements the inference forward only (call .eval()); training "
+            f"{what}: the CUDA path implements the inference forward only (call .eval()); training "
             "forward/backward is the next scope row (SURVEY.md 8f #2) and is not silently routed to PyTorch")
 
 
@@ -104,11 +104,11 @@ class EncoderLayer(torch.nn.Module):
     def forward(self, x_input, mask, cache=None):
         if cache is not None or self.concat_after or not self.normalize_before:
             raise NotImplementedError("EncoderLayer: only normalize_before=True, concat_after=False, cache=None "
-                                      "(the configuration auto_avsr instantiates) runs on the B200 path")
+                                      "(the configuration auto_avsr instantiates) runs on the CUDA path")
         if isinstance(x_input, tuple):
             x, pos_emb = x_input[0], x_input[1]
         else:
-            raise NotImplementedError("EncoderLayer: the B200 path needs the (x, pos_emb) rel-pos input")
+            raise NotImplementedError("EncoderLayer: the CUDA path needs the (x, pos_emb) rel-pos input")
         if self.training:
             # the reference's schedule with its dropouts (conformer_encoder.py:110-162); every sub-module runs forward and
             # backward in libavsr_b200, torch adds the residuals and draws the dropout masks
@@ -227,10 +227,10 @@ class ConformerEncoder(torch.nn.Module):
     def forward(self, xs, masks, taps: Optional[torch.Tensor] = None):
         if not self._device_path_ok:
             raise NotImplementedError("ConformerEncoder: only the auto_avsr configuration (normalize_before, macaron, "
-                                      "cnn module, d_k = 64, zero_triu=False) runs on the B200 path")
+                                      "cnn module, d_k = 64, zero_triu=False) runs on the CUDA path")
         if not xs.is_cuda:
             raise RuntimeError("ConformerEncoder.forward: input is on the CPU; auto_avsr_b200 has no CPU fallback -- "
-                               "move the encoder and its input to a CUDA (B200) device")
+                               "move the encoder and its input to a CUDA (H100) device")
         precision = self.precision or default_precision()
         if self.training:
             # training (SURVEY.md 8f #2): module by module under autograd, every module's forward AND backward in

@@ -18,7 +18,7 @@ class ProjEncoder(torch.nn.Linear):
 
     def forward(self, x):
         if self.training:
-            raise NotImplementedError("ProjEncoder: inference forward only on the B200 path (call .eval())")
+            raise NotImplementedError("ProjEncoder: inference forward only on the CUDA path (call .eval())")
         require_cuda(x, "ProjEncoder input")
         if self._head is None:
             self._head = PreparedHead(self.out_features, max(1, self.out_features // 64))
@@ -45,10 +45,10 @@ class CTC(torch.nn.Module):
 
     # ------------------------------------------------------------------ helpers
     def _run(self, hs_pad, want_logp=True, want_argmax=False):
-        """ctc_lo GEMM (weights prepared + padded once per parameter update, log-sum-exp partials in its epilogue)
-        followed by one finishing pass -- libavsr_b200 ``avsr_ctc_logprobs``."""
+        """ctc_lo GEMM into fp32 logits (weights prepared + padded once per parameter update) followed by one row-wise
+        log-softmax / arg-max pass -- libavsr_b200 ``avsr_ctc_logprobs``."""
         if self.training:
-            raise NotImplementedError("CTC: inference methods only on the B200 path (call .eval())")
+            raise NotImplementedError("CTC: inference methods only on the CUDA path (call .eval())")
         require_cuda(hs_pad, "CTC input")
         if self._head is None:
             d = self.ctc_lo.in_features
@@ -57,10 +57,10 @@ class CTC(torch.nn.Module):
 
     # ------------------------------------------------------------------ reference surface
     def forward(self, hs_pad, hlens, ys_pad):
-        raise NotImplementedError("CTC.forward (the training loss, ctc.py:41-65) is not on the B200 inference path")
+        raise NotImplementedError("CTC.forward (the training loss, ctc.py:41-65) is not on the CUDA inference path")
 
     def loss_fn(self, th_pred, th_target, th_ilen, th_olen):
-        raise NotImplementedError("CTC.loss_fn (ctc.py:32-39) is not on the B200 inference path")
+        raise NotImplementedError("CTC.loss_fn (ctc.py:32-39) is not on the CUDA inference path")
 
     def log_softmax(self, hs_pad):
         """(B, Tmax, eprojs) -> (B, Tmax, odim) log-probs (ctc.py:77-84)."""

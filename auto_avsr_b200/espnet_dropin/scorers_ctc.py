@@ -69,7 +69,7 @@ class CTCPrefixScorer(_si.BatchPartialScorerInterface):
 
     # ---------------------------------------------------------------- not on the batch path
     def init_state(self, x):
-        raise NotImplementedError("CTCPrefixScorer: the non-batch numpy path (scorers/ctc.py:25-36) is not on the B200 path; "
+        raise NotImplementedError("CTCPrefixScorer: the non-batch numpy path (scorers/ctc.py:25-36) is not on the CUDA path; "
                                   "use BatchBeamSearch / DeviceBeamSearch")
 
     def score_partial(self, y, ids, state, x):

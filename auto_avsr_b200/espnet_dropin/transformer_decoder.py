@@ -90,7 +90,7 @@ class TransformerDecoder(_si.BatchScorerInterface, torch.nn.Module):
                  concat_after=False, layer_drop_rate=0.0):
         torch.nn.Module.__init__(self)
         if input_layer != "embed" or not use_output_layer or not normalize_before or concat_after:
-            raise NotImplementedError("B200 decoder path: input_layer='embed', use_output_layer, normalize_before and "
+            raise NotImplementedError("CUDA decoder path: input_layer='embed', use_output_layer, normalize_before and "
                                       "not concat_after (what E2E builds, e2e_asr_conformer.py:41-47)")
         self._register_load_state_dict_pre_hook(_pre_hook)
         self.embed = torch.nn.Sequential(torch.nn.Embedding(odim, attention_dim),
@@ -127,7 +127,7 @@ class TransformerDecoder(_si.BatchScorerInterface, torch.nn.Module):
     # ---------------------------------------------------------------- reference surface
     def forward(self, tgt, tgt_mask, memory, memory_mask):
         raise NotImplementedError("TransformerDecoder.forward (the teacher-forced training pass, transformer_decoder.py:231-258)"
-                                  " is not on the B200 scoring path")
+                                  " is not on the CUDA scoring path")
 
     def forward_one_step(self, tgt, tgt_mask, memory, memory_mask=None, cache=None):
         raise NotImplementedError("forward_one_step exposes the reference's per-layer output cache, which this path does not "
@@ -144,7 +144,7 @@ class TransformerDecoder(_si.BatchScorerInterface, torch.nn.Module):
         slots this method returned for its parent; xs (n, T, d) the encoder output repeated per hypothesis (row 0 is
         read).  -> ((n, odim) log-probabilities, next states)."""
         if self.training:
-            raise NotImplementedError("TransformerDecoder: inference scoring only on the B200 path (call .eval())")
+            raise NotImplementedError("TransformerDecoder: inference scoring only on the CUDA path (call .eval())")
         n, ylen = ys.shape
         eng = self.engine()
         step = ylen - 1

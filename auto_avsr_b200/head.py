@@ -115,7 +115,7 @@ def features_to_log_probs(proj: torch.nn.Linear, encoder, ctc, feats: torch.Tens
     ``proj`` is E2E.proj_encoder, ``encoder`` the drop-in ConformerEncoder, ``ctc`` E2E.ctc (anything with a ``ctc_lo``
     Linear): the reference's inference path e2e_asr_conformer.py:70-71 + ctc.py:77-84 in ONE library call --
     proj_encoder writes sqrt(d)-scaled rows straight into the residual stream, after_norm emits ctc_lo's operand, the
-    ctc_lo GEMM leaves log-sum-exp partials for a single finishing pass.  A (B, T) shape that keeps coming back is replayed
+    ctc_lo GEMM writes fp32 logits and one row-wise pass turns them into log-probs / arg max.  A (B, T) shape that keeps coming back is replayed
     from a CUDA graph (``encoder.use_graph`` / ``graph_after``): then the returned tensors belong to the plan and are
     overwritten by the next call with that shape -- clone them to keep them."""
     from .espnet_dropin.attention import mask_to_lengths

@@ -1,8 +1,8 @@
-"""Make the reference pick up the B200 encoder without touching its sources.
+"""Make the reference pick up the CUDA encoder without touching its sources.
 
 ``auto_avsr_b200.install()`` registers this package's modules under the reference's import paths, so
 ``from espnet.nets.pytorch_backend.encoder.conformer_encoder import ConformerEncoder``
-(e2e_asr_conformer.py:12) resolves to the B200 implementation and train.py / eval.py / lightning.py keep
+(e2e_asr_conformer.py:12) resolves to the CUDA implementation and train.py / eval.py / lightning.py keep
 driving it unchanged.  Call it before importing ``espnet.nets.pytorch_backend.e2e_asr_conformer`` (or after:
 already-imported E2E modules get their ``ConformerEncoder`` symbol re-pointed).
 """
@@ -64,7 +64,7 @@ def install_decoder(model):
     a class it imports by name and ``E2E.scorers()`` builds the CTC scorer likewise (e2e_asr_conformer.py:13,17,41-47,58-59):
     this re-homes the decoder of an existing ``E2E`` instance onto the drop-in (the very same ``Parameter`` objects) and
     re-points the two names in the already-imported E2E module, so ``model.scorers()`` -- what
-    ``get_beam_search_decoder`` feeds to ``BatchBeamSearch`` (lightning.py:126-157) -- returns the B200 scorers.
+    ``get_beam_search_decoder`` feeds to ``BatchBeamSearch`` (lightning.py:126-157) -- returns the CUDA scorers.
     Inference only: the teacher-forced ``decoder.forward`` of the training loss stays with the reference module, so call
     this on a model that is used for decoding."""
     from .espnet_dropin import scorer_interface, scorers_ctc

@@ -1,5 +1,5 @@
 """Training slice of the encoder path (SURVEY.md 8f #2, first slice): ``torch.autograd.Function``s whose forward AND
-backward run in libavsr_b200 -- LayerNorm, Linear (+ReLU) with dgrad / wgrad as the same tcgen05 GEMMs on transposed
+backward run in libavsr_b200 -- LayerNorm, Linear (+ReLU) with dgrad / wgrad as the same wgmma GEMMs on transposed
 operands, GLU, and the depthwise-conv + BatchNorm(batch statistics) + SiLU block.  Gradients land on the original
 ``nn.Parameter``s (autograd accumulates what ``backward`` returns), so DDP hooks, ``clip_grad_norm_`` and AdamW
 (lightning.py:49, train.py:37-41) see them unchanged.  torch supplies device memory, the autograd tape, dropout masks
@@ -59,7 +59,7 @@ def colsum(y):
     cols = y.size(-1)
     rows = y.numel() // cols
     out = torch.empty(cols, dtype=torch.float32, device=y.device)
-    ws = _workspace(y.device, 148 * cols * 4 + 1024)
+    ws = _workspace(y.device, 132 * cols * 4 + 1024)
     with torch.cuda.device(y.device):
         check(lib.avsr_colsum(y.data_ptr(), out.data_ptr(), rows, cols, ws.data_ptr(), ws.numel(), _stream_handle(y.device)))
     return out
@@ -175,7 +175,7 @@ def _chan_sums(v, dy=None, mean=None, invstd=None, gamma=None, beta=None):
     Cc = v.size(-1)
     rows = v.numel() // Cc
     out = torch.empty(2, Cc, dtype=torch.float32, device=v.device)
-    ws = _workspace(v.device, 148 * 2 * Cc * 4 + 1024)
+    ws = _workspace(v.device, 132 * 2 * Cc * 4 + 1024)
     with torch.cuda.device(v.device):
         check(lib.avsr_chan_sums(v.data_ptr(), _ptr(dy), _ptr(mean), _ptr(invstd), _ptr(gamma), _ptr(beta), out.data_ptr(),
                                  rows, Cc, ws.data_ptr(), ws.numel(), _stream_handle(v.device)))

@@ -2,6 +2,7 @@
 """Benchmark of the hot path: Conformer encoder forward, frames/sec at max-frames=1600 (BASELINE.json).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--precision tf32|fp32]
+                    [--dump-outputs DIR]
 
 A step = one ConformerEncoder.forward (embed + 12 layers + after_norm, eval) over one synthetic max-frames=1600
 bucket per GPU (workload S2 = 4 utterances x 400 frames, d=768, BASELINE.json configs[1]); weak scaling: every
@@ -62,11 +63,12 @@ def measured_peaks():
             p = json.load(f)
         return dict(bf16_tflops=p["bf16_tflops"], bf16_tflops_sustained=p.get("bf16_tflops_sustained"),
                     hbm_gbs=p["hbm_gbs"], source="measured")
-    return dict(bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, hbm_gbs=6650.0, source="fallback")
+    # NVIDIA H100 SXM data sheet (dense BF16, HBM3 at a 700 W power limit): a ceiling, never a measured figure
+    return dict(bf16_tflops=989.0, bf16_tflops_sustained=None, hbm_gbs=3350.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -153,7 +155,7 @@ class CpuEncoder:
 
 def pick_threads(lengths):
     """Both CPU implementations are many mid-sized torch ops; on a many-core host all-threads is far from optimal (128
-    threads were 30x slower than 32 on the first B200 box).  Probe a 1-layer forward at a few thread counts and keep
+    threads were 30x slower than 32 on one many-core host).  Probe a 1-layer forward at a few thread counts and keep
     the fastest: 'all the host threads it can use' productively."""
     ncpu = os.cpu_count() or 1
     cands = sorted({c for c in (4, 8, 16, 32, 64, ncpu) if c <= ncpu})
@@ -201,15 +203,13 @@ def run_reference(args):
     torch.set_num_threads(threads)
     cpu = CpuEncoder(CFG)
     xs = encoder_input(lengths, CFG["d_model"], 1234)
-    t0 = time.perf_counter()
     cpu.forward(xs, lengths)                                        # warm-up (1 forward; each is a full S2 bucket)
-    warm = time.perf_counter() - t0
-    if warm * args.steps > 120:                                     # keep the arm within a few minutes
-        args.steps = max(1, int(120 / warm))
     t0 = time.perf_counter()
     for _ in range(args.steps):
-        cpu.forward(xs, lengths)
+        last = cpu.forward(xs, lengths)
     dt = time.perf_counter() - t0
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, (last, non_pad_mask(lengths, "cpu")))
     fps = sum(lengths) * args.steps / dt
     note = ("the reference's own espnet ConformerEncoder (oracle/_ref: unmodified copy made by oracle/build_ref.py)"
             if cpu.kind == "reference" else
@@ -227,7 +227,7 @@ def run_reference(args):
 
 # ------------------------------------------------------------------------------------------------ GPU arm
 def kernel_roofline(dev, peaks, precision):
-    """Dominant kernel = the tcgen05 GEMM (92% of the forward's algorithmic FLOPs).  Times its largest instance, the
+    """Dominant kernel = the wgmma GEMM (92% of the forward's algorithmic FLOPs).  Times its largest instance, the
     FFN w_1 projection (1600 x 3072 x 768, bias+ReLU epilogue, operand-typed output; 24 launches per forward), over
     24 distinct weight matrices back to back with CUDA events on the launch stream, operands already in operand
     storage exactly as inside the encoder; achieved = algorithmic 2*M*N*K per launch / mean launch duration."""
@@ -270,20 +270,12 @@ def kernel_roofline(dev, peaks, precision):
     flops = 2.0 * M * N * K
     achieved = flops / per_launch_s / 1e12
     peak = peaks["bf16_tflops"]
-    prof = os.path.join(ROOT, "profiles", "gemm_traffic.json")
-    traffic = None
-    if os.path.exists(prof):
-        try:
-            traffic = json.load(open(prof)).get("dram_bytes_per_launch")
-        except Exception:
-            traffic = None
-    kind = "kind::f16, fp16 operands" if precision == "f16" else "kind::tf32"
-    kname = ("gemm_tc2_kernel<EPI_LINEAR,384> (cta_group::2 pair tile 256x384, 56 clusters)" if precision == "f16"
-             else "gemm_tc_kernel<EPI_LINEAR> (persistent, 1-CTA)")
-    out = {"bound": "tensor", "kernel": f"{kname} FFN w_1 1600x3072x768 (tcgen05 {kind}, fp32 accumulate)",
+    kind = "f16 operands" if precision == "f16" else "tf32 operands"
+    out = {"bound": "tensor", "kernel": f"gemm_tc_kernel<EPI_LINEAR> (persistent) FFN w_1 1600x3072x768 (wgmma, {kind}, "
+                                        "fp32 accumulate)",
            "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-           "peak_source": f"MEASURED_PEAKS.json bf16_tflops ({peaks['source']}, cuBLAS bf16 8192^3 burst)",
-           "us_per_launch": per_launch_s * 1e6, "algorithmic_flops_per_launch": flops, "traffic": traffic}
+           "peak_source": f"bf16_tflops ({peaks['source']})",
+           "us_per_launch": per_launch_s * 1e6, "algorithmic_flops_per_launch": flops}
     if precision == "tf32":
         out["frac_of_tf32_nominal"] = achieved / (0.5 * peak)
     return out
@@ -311,7 +303,7 @@ def extras(dev, enc, args, peaks):
     sustained   S2 replayed back to back for >= 3 s, against MEASURED_PEAKS' sustained bf16 figure
     gpu_eager_baseline   the same op sequence in stock eager PyTorch on this GPU (cuBLAS / ATen kernels): the torch
                 restatement oracle/conformer_oracle.py moved to cuda, fp32 with and without allow_tf32 -- SURVEY.md
-                section 2b's per-kernel bar ("beat eager PyTorch-on-B200 of the same op sequence")."""
+                section 2b's per-kernel bar ("beat eager PyTorch on the same GPU, same op sequence")."""
     out = {"shapes": {}, "precisions": {}}
     prec0 = enc.precision
     for name in ("S1", "S2r", "S3", "S4"):
@@ -485,6 +477,18 @@ def extras(dev, enc, args, peaks):
     return out
 
 
+def dump_outputs(path, result):
+    """The arrays ConformerEncoder.forward handed back in the last timed step: the (B, T, d) features and the
+    (B, 1, T) non-pad mask, as float32 .npy files (4.9 MB at workload S2).  In both arms the last timed step runs on
+    the same input (encoder_input seed 1234 on rank 0), so dumps of two builds or of the two arms compare element-wise."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    feats, masks = result
+    np.save(os.path.join(path, "encoder_features.npy"), feats.detach().float().cpu().numpy())
+    np.save(os.path.join(path, "encoder_masks.npy"), masks.detach().float().cpu().numpy())
+    log(f"outputs of the last timed step written to {path}")
+
+
 def run_ours(args):
     rank, local_rank, world = dist_env()
     assert torch.cuda.is_available(), "bench.py needs a GPU (the encoder path has no CPU fallback)"
@@ -504,7 +508,7 @@ def run_ours(args):
     enc.precision = args.precision
     enc.assume_frozen = True
     mask = non_pad_mask(lengths, dev)
-    nbuf = 4     # rotating inputs; the 682 MB of weights streamed every step already exceed the 126 MB L2
+    nbuf = 4     # rotating inputs; the 682 MB of weights streamed every step already exceed the 50 MB L2
     host_in = [encoder_input(lengths, D, 1234 + rank * 100 + i).pin_memory() for i in range(nbuf)]
     dev_in = [h.to(dev) for h in host_in]
     host_out = torch.empty(B, T, D).pin_memory()
@@ -537,12 +541,14 @@ def run_ours(args):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for i in range(args.steps):
-            enc(dev_in[i % nbuf], mask)
+            last = enc(dev_in[(args.steps - 1 - i) % nbuf], mask)   # the last step runs on dev_in[0] (seed 1234 + 100 * rank)
         e1.record()
         barrier()
         ms = e0.elapsed_time(e1)
         launches = _cabi.launch_count() - l0
         log(f"device-timed region done: {ms / args.steps:.3f} ms/step")
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, last)
         # ---- end to end through the public API: every step copies its inputs from pinned host memory (H2D), runs
         # ConformerEncoder.forward, and copies the features back to pinned host memory (D2H).  PipelinedEncoder
         # (auto_avsr_b200/pipeline.py) overlaps the copies of neighbouring steps with the forward on 3 streams.
@@ -583,7 +589,7 @@ def run_ours(args):
             "config": {"workload": workload_string(),
                        "global_frames_per_step": sum(lengths) * world, "parallelism": f"dp{world} (one bucket per GPU, "
                                                                                        "no data-path collective)",
-                       "l2": "682 MB of weights streamed per step > 126 MB L2; 4 rotating input buffers",
+                       "l2": "682 MB of weights streamed per step > 50 MB L2; 4 rotating input buffers",
                        "pos_cache": "cold: linear_pos(pos_emb) recomputed every step", "precision": args.precision,
                        "assume_frozen": True, "graph_after": enc._engine.graph_after,
                        "untimed_steps_before_timing": n_warm},
@@ -624,12 +630,14 @@ def main():
     ap.add_argument("--precision", default=os.environ.get("AVSR_B200_PRECISION", "f16"),
                     choices=["f16", "tf32", "fp32"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (encoder features, non-pad mask) as DIR/<name>.npy")
     ap.add_argument("--no-extras", action="store_true", help="skip the extras (other shapes / precisions, sustained "
                                                                "loop, eager-PyTorch GPU comparator)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     if args.impl == "reference":
-        if args.steps > 20:
-            args.steps = 20          # ~1 s per CPU forward: keep the arm within a few minutes
         run_reference(args)
     else:
         run_ours(args)

@@ -1,5 +1,5 @@
 /*
- * avsr_b200.h -- C ABI of libavsr_b200.so: the B200 (sm_100a) Conformer-encoder forward path.
+ * avsr_b200.h -- C ABI of libavsr_b200.so: the H100 (sm_90a) Conformer-encoder forward path.
  *
  * The reference (mpc001/auto_avsr @ 182b628) has no FFI layer: its boundary for this path is the
  * Python nn.Module surface (SURVEY.md section 8b).  These entry points are what a binding for that
@@ -39,8 +39,8 @@ enum {
 /* Arithmetic of the GEMM / attention contractions. */
 enum {
   AVSR_PREC_FP32 = 0,  /* CUDA-core fp32 FMA kernels: the on-device exact reference path (slow) */
-  AVSR_PREC_TF32 = 1,  /* tcgen05 kind::tf32: operands kept as fp32 rounded to TF32, fp32 accumulate */
-  AVSR_PREC_F16 = 2    /* tcgen05 kind::f16: operands stored as IEEE half (same 10-bit mantissa as TF32, saturating
+  AVSR_PREC_TF32 = 1,  /* wgmma .tf32: operands kept as fp32 rounded to TF32, fp32 accumulate */
+  AVSR_PREC_F16 = 2    /* wgmma .f16: operands stored as IEEE half (same 10-bit mantissa as TF32, saturating
                           conversion), fp32 accumulate; residual stream, LayerNorm, softmax, conv stay fp32.
                           Half the operand bytes and twice the MMA rate of TF32: the product path. */
 };
@@ -200,7 +200,7 @@ int avsr_prepare_head(const AvsrEncoderConfig *cfg, int idim, int odim, const fl
  * (e2e_asr_conformer.py:70-71 + ctc.py:77-84; lightning.py:70-72 for B = 1, lengths NULL):
  *   x = proj_encoder(feats) * sqrt(d) -> written by the GEMM epilogue straight into the residual stream,
  *   12 x EncoderLayer, after_norm -> enc_out (B,T,d_model) fp32 (NULL: not needed) AND ctc_lo's fp16 operand,
- *   ctc_lo GEMM whose epilogue leaves per-row log-sum-exp partials, one finishing pass -> logp (B,T,odim) fp32,
+ *   ctc_lo GEMM into fp32 logits, one row-wise log-softmax pass -> logp (B,T,odim) fp32,
  *   argmax (B*T) int32 greedy ids (either may be NULL, not both).
  * feats (B,T,idim) fp32.  workspace >= avsr_head_workspace_bytes. */
 size_t avsr_head_workspace_bytes(const AvsrEncoderConfig *cfg, int B, int T, int idim, int odim);

@@ -5,7 +5,8 @@
 TEST / MEASUREMENT INFRASTRUCTURE ONLY (never imported by auto_avsr_b200).  The reference is pure Python, so "building"
 it is a file copy; nothing is edited and nothing under oracle/_ref is committed (.gitignore).  Users:
   * bench.py --impl reference and bench.py's cpu_baseline leg time THIS code (kind "reference") on the host cores;
-  * tests/test_oracle_golden.py::test_ref_copy_reproduces_golden checks the copy against the committed fixtures.
+  * tests/test_oracle_golden.py::test_ref_copy_reproduces_golden checks the copy against the committed fixtures;
+  * tests/test_boundary_cpu.py and tests/test_decoder_dropin_cpu.py drive the drop-ins from the reference's own modules.
 Run:  python oracle/build_ref.py [/root/reference]
 """
 import filecmp
@@ -37,6 +38,12 @@ FILES = [
     "espnet/nets/e2e_asr_common.py",
     "espnet/nets/beam_search.py",
     "espnet/nets/batch_beam_search.py",
+    # the E2E model that builds the encoder / CTC head (tests/test_boundary_cpu.py: install() / install_head())
+    "espnet/nets/pytorch_backend/e2e_asr_conformer.py",
+    "espnet/nets/pytorch_backend/frontend/resnet.py",
+    "espnet/nets/pytorch_backend/frontend/resnet1d.py",
+    "espnet/nets/pytorch_backend/transformer/add_sos_eos.py",
+    "espnet/nets/pytorch_backend/transformer/label_smoothing_loss.py",
 ]
 
 

@@ -1,7 +1,8 @@
 #!/usr/bin/env python3
 """Diagnostic build: the same sources compiled with -DAVSR_TRACE into auto_avsr_b200/csrc/libavsr_b200_trace.so.
-The two-SM GEMM and the fp16 attention kernel then record clock64() at their phase boundaries, one record per CTA
-(common.cuh, "phase trace").  Use with AVSR_B200_LIB=<that file>; scripts/phase_probe.py does it."""
+The GEMM and the elementwise kernels then record %globaltimer when a CTA opens, when its dependency resolved and when
+it is done, one record per CTA (common.cuh, "phase trace"); avsr_trace_set binds the buffer.  Use with
+AVSR_B200_LIB=<that file>."""
 import os
 import subprocess
 import sys

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Observed errors of the row 8f#3 schedule / functors on the CPU (host replay of csrc/decoder_body.cuh, tests/emu) against
-the reference-generated fixtures: what the CPU suite asserts, printed.  -> profiles/r02_decoder_cpu_verification.txt"""
+the reference-generated fixtures: what the CPU suite asserts, printed."""
 import os
 import sys
 

@@ -1,6 +1,6 @@
 // Torch-free GPU check of the row 8f#3 entries of libavsr_b200 (decoder step over a forked beam, CTC prefix scorer)
 // against oracle outputs prepared by scripts/make_decoder_check_blob.py.  Starts in seconds on a fresh box:
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O2 -std=c++17 -Iinclude scripts/decoder_gpu_check.cu \
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O2 -std=c++17 -Iinclude scripts/decoder_gpu_check.cu \
 //        -Lauto_avsr_b200/csrc -lavsr_b200 -Xlinker -rpath -Xlinker '$ORIGIN/../../auto_avsr_b200/csrc' -o scripts/bin/decoder_gpu_check
 //   scripts/bin/decoder_gpu_check scripts/bin/decoder_check.blob
 // TEST INFRASTRUCTURE (calls the library only through include/avsr_b200.h).

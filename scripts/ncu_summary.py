@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """One line per profiled launch of an .ncu-rep (run where ncu is installed; no GPU needed):
-    python scripts/ncu_summary.py gpurun_out/r02_layer_kernels.ncu-rep > profiles/....summary.txt
+    python scripts/ncu_summary.py layer_kernels.ncu-rep > layer_kernels.summary.txt
 Columns: duration, DRAM bytes read / written, achieved DRAM GB/s, tensor-pipe active %, issue-slot %, warps active %,
 registers, grid, and the kernel name."""
 import csv

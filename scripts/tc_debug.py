@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""On-GPU bring-up diagnostics for the tcgen05 kernels: each case runs in its own subprocess (a trapped kernel
+"""On-GPU bring-up diagnostics for the tensor-core (wgmma) kernels: each case runs in its own subprocess (a trapped kernel
 poisons the CUDA context) and prints the error structure against the fp32 CUDA-core path of the same library."""
 import os
 import subprocess

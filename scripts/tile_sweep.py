@@ -44,7 +44,7 @@ run("out", 1600, 768, 768, 0, 0, 1)
 run("n1536", 1600, 1536, 768, 0, 1, 0)
 '''
 prec = sys.argv[1] if len(sys.argv) > 1 else "f16"
-for tile in (sys.argv[2:] or ["auto", "64,1", "128,1", "128,2", "256,1", "256,2"]):
+for tile in (sys.argv[2:] or ["auto", "64", "128"]):          # AVSR_B200_TILE = "BN[,SPLITS]"
     env = dict(os.environ)
     if tile != "auto":
         env["AVSR_B200_TILE"] = tile

@@ -1,11 +1,7 @@
 """Bodies of the row 8f#3 GPU parity cases (tests/test_zzz_gpu_decoder.py calls them in-process; each can also run alone in
 its own process / CUDA context:  python tests/decoder_gpu_cases.py <case> [args...]).
 
-First B200 run: round 2, last session (profiles/r02_decoder_gpu_check.txt, r02_decoder_parity_observed.txt): all cases
-passed; the bounds below are <= 4x the errors observed there (max-abs on log-probabilities of O(5..10) magnitude):
-  decoder log-probs   fp32 6.2e-7 (d 128) / 2.3e-6 (d 768, 6 layers);  tf32 6.5e-4 / 7.9e-4;  f16 6.7e-4 / 7.9e-4
-  forked beam         fp32 1.4e-6, f16 7.5e-4        CTC prefix scores 3.2e-6 / 4.1e-6 (scaled, see ctc_prefix)
-  beam search         fp32 n-best scores within 7.6e-6 / 1.5e-5 of the reference's; f16 best score within 1.5e-3 / 3.2e-4"""
+The bounds below are about 4x the errors observed on the GPU (max-abs on log-probabilities of O(5..10) magnitude)."""
 import os
 import sys
 

@@ -19,7 +19,7 @@ def build() -> str:
     if not os.path.exists(OUT) or any(os.path.getmtime(d) > os.path.getmtime(OUT) for d in DEPS):
         os.makedirs(os.path.dirname(OUT), exist_ok=True)
         nvcc = os.environ.get("NVCC") or "/usr/local/cuda/bin/nvcc"
-        cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O2", "-std=c++17", "-Xcompiler", "-fPIC",
+        cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-Xcompiler", "-fPIC",
                "--expt-relaxed-constexpr", "-shared", "-o", OUT, SRC]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

@@ -4,7 +4,7 @@
 // There is no GPU in the build container, so the CPU suite checks the part of csrc/decoder.cu that is NOT one of the
 // already GPU-verified kernels -- the launch schedule, the buffer layouts, the slot / ancestor addressing and every
 // per-element functor of decoder_body.cuh -- by compiling that same header against this backend: functors run as plain
-// loops, the GEMM / LayerNorm / log-softmax launchers (verified on the B200 by the encoder tests) are replaced by
+// loops, the GEMM / LayerNorm / log-softmax launchers (verified on the GPU by the encoder tests) are replaced by
 // naive fp32 loops.  Same extern "C" names and signatures as include/avsr_b200.h, HOST pointers, AVSR_PREC_FP32 only.
 #include <stdarg.h>
 

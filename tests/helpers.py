@@ -43,7 +43,7 @@ _OBS = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
 
 def record(test, case, observed, bound):
     """Print the observed error next to its bound and append it to gpurun_out/parity_observed.jsonl (the GPU runs'
-    scratch directory) so that the bounds in the tests can be kept at <= 4x what a B200 actually produces."""
+    scratch directory) so that the bounds in the tests can be kept at about 4x what the GPU actually produces."""
     import json
     line = {"test": test, "case": str(case), "observed": observed, "bound": bound}
     print("PARITY", json.dumps(line))

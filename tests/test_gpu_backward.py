@@ -1,10 +1,10 @@
-"""Training slice (SURVEY.md 8f #2, first slice) on a B200: forward AND backward of the drop-in LayerNorm,
+"""Training slice (SURVEY.md 8f #2, first slice) on the GPU: forward AND backward of the drop-in LayerNorm,
 PositionwiseFeedForward and ConvolutionModule in train() mode run in libavsr_b200 (auto_avsr_b200/train.py) and must
 reproduce outputs, input gradients, parameter gradients and BatchNorm running statistics of the UNMODIFIED reference
 modules (fixtures tests/golden/train_*.npz from oracle/make_golden_train.py: float64, dropout p = 0).
 
 Bounds: forward like the inference tests; gradients relative to the largest reference gradient entry -- backward GEMMs
-run on TF32 operands (f16 / tf32 precision) or fp32 FMAs (fp32 precision); bounds are <= 4x what a B200 produced."""
+run on TF32 operands (f16 / tf32 precision) or fp32 FMAs (fp32 precision); bounds are about 4x the observed errors."""
 import os
 
 import numpy as np

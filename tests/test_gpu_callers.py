@@ -1,4 +1,4 @@
-"""The reference's CALLERS driving the drop-in on a B200 (VERDICT r01: 'no GPU test goes through the reference's
+"""The reference's CALLERS driving the drop-in on the GPU (VERDICT r01: 'no GPU test goes through the reference's
 caller'): auto_avsr_b200.shim replays E2E.forward (e2e_asr_conformer.py:63-71) and ModelModule.test_step
 (lightning.py:69-72) line by line; plus the on-device collate of row 8f #4."""
 import numpy as np

@@ -2,8 +2,7 @@
 fixtures generated from the reference's own TransformerDecoder / CTCPrefixScoreTH / BatchBeamSearch
 (tests/golden/decoder_*.npz) and the fp64 oracle.  Bodies and bounds: tests/decoder_gpu_cases.py.
 
-First B200 run: round 2, last session -- the torch-free check (scripts/decoder_gpu_check.cu) and all cases passed at the
-first attempt; observed errors in profiles/r02_decoder_parity_observed.txt, bounds pinned at <= 4x those."""
+Bounds are pinned at about 4x the errors observed on the GPU."""
 import os
 
 import pytest
