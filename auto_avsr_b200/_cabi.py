@@ -123,6 +123,9 @@ SIGNATURES = {
     "avsr_dwconv_wgrad": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _Z, _P]),
     "avsr_relpos_attention_bwd_workspace_bytes": (_Z, [_I, _I, _I]),
     "avsr_relpos_attention_bwd": (_I, [_P] * 14 + [_I, _I, _I, _P, _Z, _P]),
+    "avsr_ctc_loss_state_bytes": (_Z, [_I, _I, _I]),
+    "avsr_ctc_loss_fwd": (_I, [_P, C.c_long, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _Z, _P]),
+    "avsr_ctc_loss_bwd": (_I, [_P, C.c_long, _P, _P, _I, _I, _I, _I, _P, _P, _Z, _P, C.c_long, _P]),
     "avsr_pack_padded": (_I, [_P, _P, _P, _P, _I, _I, _I, _F, _P]),
     "avsr_unpack_padded": (_I, [_P, _P, _P, _I, _I, _I, _P]),
     "avsr_head_prepared_bytes": (_Z, [_CFG, _I, _I]),

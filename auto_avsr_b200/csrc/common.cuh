@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 #include <stdio.h>
 
@@ -110,6 +111,9 @@ inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block
   } while (0)
 
 // ---------------------------------------------------------------- device helpers
+// code shared by a kernel and the host replay the CPU tests build (tests/emu): decoder_body.cuh, ctc_loss_body.cuh
+#define AVSR_HD __host__ __device__ __forceinline__
+
 __device__ __forceinline__ float round_tf32(float x) {
   // round-to-nearest (ties away) to the 10-bit TF32 mantissa; the tensor core then truncates nothing.
   uint32_t r;

@@ -25,8 +25,6 @@
 namespace avsr {
 namespace dec {
 
-#define AVSR_HD __host__ __device__ __forceinline__
-
 constexpr int kMaxDecLayers = 16;
 constexpr float kLogZero = -10000000000.0f;   // ctc_prefix_score.py:31
 

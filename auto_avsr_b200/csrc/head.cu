@@ -6,35 +6,9 @@
 // float4 where the padded GEMM output allows it -- then a warp-shuffle + shared-memory reduction of the triples;
 // pass 2 re-reads the row (20 KB: still in L1/L2) and writes x - (max + log sum).  HBM-bound: 4 B read + 4 B
 // written per logit.
-#include "common.cuh"
+#include "maxsum.cuh"
 
 namespace avsr {
-
-struct MaxSum {
-  float m, s;   // running max, sum of exp(x - m)
-  int i;        // index of the first maximal element
-};
-
-__device__ __forceinline__ void ms_push(MaxSum& a, float x, int idx) {
-  if (x > a.m) {
-    a.s = a.s * __expf(a.m - x) + 1.f;   // a.m = -inf on the first element: exp(-inf) = 0
-    a.m = x;
-    a.i = idx;
-  } else {
-    a.s += (x == -INFINITY) ? 0.f : __expf(x - a.m);   // x = m = -inf would give exp(nan); F.log_softmax ignores -inf logits
-  }
-}
-
-__device__ __forceinline__ MaxSum ms_merge(const MaxSum& a, const MaxSum& b) {
-  MaxSum r;
-  const bool take_b = b.m > a.m || (b.m == a.m && b.i < a.i);
-  r.m = take_b ? b.m : a.m;
-  r.i = take_b ? b.i : a.i;
-  const float ea = a.m == -INFINITY ? 0.f : __expf(a.m - r.m);
-  const float eb = b.m == -INFINITY ? 0.f : __expf(b.m - r.m);
-  r.s = a.s * ea + b.s * eb;
-  return r;
-}
 
 __global__ void __launch_bounds__(256) log_softmax_rows_kernel(const float* __restrict__ x, long ldx,
                                                                float* __restrict__ y, long ldy,
@@ -42,9 +16,6 @@ __global__ void __launch_bounds__(256) log_softmax_rows_kernel(const float* __re
   pdl_launch_dependents();
   const int row = blockIdx.x;
   const float* xr = x + (long)row * ldx;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  __shared__ MaxSum part[8];
-  __shared__ float s_shift;
   pdl_wait();
 
   MaxSum acc{-INFINITY, 0.f, 0x7fffffff};
@@ -56,25 +27,10 @@ __global__ void __launch_bounds__(256) log_softmax_rows_kernel(const float* __re
   }
   for (int c = n4 + threadIdx.x; c < n; c += 256) ms_push(acc, xr[c], c);
 
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) {
-    MaxSum o;
-    o.m = __shfl_xor_sync(0xffffffffu, acc.m, off);
-    o.s = __shfl_xor_sync(0xffffffffu, acc.s, off);
-    o.i = __shfl_xor_sync(0xffffffffu, acc.i, off);
-    acc = ms_merge(acc, o);
-  }
-  if (lane == 0) part[warp] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    MaxSum t = part[0];
-    for (int w = 1; w < 8; ++w) t = ms_merge(t, part[w]);
-    s_shift = t.m + logf(t.s);
-    if (best) best[row] = t.i;
-  }
-  __syncthreads();
+  const MaxSum t = ms_block_reduce_256(acc);
+  if (best && threadIdx.x == 0) best[row] = t.i;
   if (!y) return;
-  const float shift = s_shift;
+  const float shift = t.m + logf(t.s);
   float* yr = y + (long)row * ldy;
   for (int c = threadIdx.x; c < n; c += 256) yr[c] = xr[c] - shift;
 }

@@ -1,34 +1,39 @@
-"""Drop-in for the inference surface of espnet.nets.pytorch_backend.ctc.CTC (reference ctc.py:9-93) and for the
-``proj_encoder`` Linear in front of the encoder (e2e_asr_conformer.py:31): SURVEY.md 8f #1, the steps either side of
-the encoder hot path."""
-from typing import Optional, Tuple
+"""Drop-in for espnet.nets.pytorch_backend.ctc.CTC (reference ctc.py:9-93) and for the ``proj_encoder`` Linear in front
+of the encoder (e2e_asr_conformer.py:31): SURVEY.md 8f #1, the steps either side of the encoder hot path, and the CTC
+loss of the training step (e2e_asr_conformer.py:77)."""
+from typing import Optional
 
 import torch
+import torch.nn.functional as F
 
+from .. import ops
 from ..engine import default_precision, require_cuda
 from ..head import PreparedHead, ctc_log_probs, proj_forward
+from ..train import CtcLossFn, LinearFn, ctc_loss_forward
 
 
 class ProjEncoder(torch.nn.Linear):
-    """``torch.nn.Linear(512, 768)`` whose eval forward runs in libavsr_b200 (same parameters, same state-dict keys).
-    Training / CPU tensors are refused rather than silently computed elsewhere."""
+    """``torch.nn.Linear(512, 768)`` that runs in libavsr_b200 (same parameters, same state-dict keys).  Eval: on the
+    prepared weights.  Train: ``LinearFn`` (forward GEMM in the module's precision, dgrad / wgrad as TF32 GEMMs), so the
+    input gradient flows back to the front-end.  CPU tensors are refused rather than silently computed elsewhere."""
 
     precision: Optional[str] = None
     _head: Optional[PreparedHead] = None
 
     def forward(self, x):
+        prec = self.precision or default_precision()
         if self.training:
-            raise NotImplementedError("ProjEncoder: inference forward only on the CUDA path (call .eval())")
+            return LinearFn.apply(x, self.weight, self.bias, False, prec)
         require_cuda(x, "ProjEncoder input")
         if self._head is None:
             self._head = PreparedHead(self.out_features, max(1, self.out_features // 64))
-        return proj_forward(self._head, self, x, self.precision or default_precision())
+        return proj_forward(self._head, self, x, prec)
 
 
 class CTC(torch.nn.Module):
     """Same constructor, attributes and state-dict keys (``ctc_lo.weight``, ``ctc_lo.bias``) as the reference's CTC
-    module.  ``log_softmax`` / ``softmax`` / ``argmax`` (what CTCPrefixScorer and greedy decoding call) run on the
-    GPU: ctc_lo as a tensor-core GEMM, then one row-wise log-sum-exp kernel.  The training loss is row 8f #2."""
+    module.  ``forward`` (the training loss) and ``log_softmax`` / ``softmax`` / ``argmax`` (what CTCPrefixScorer and
+    greedy decoding call, eval mode) run on the GPU: ctc_lo as a tensor-core GEMM, then the library's row kernels."""
 
     def __init__(self, odim, eprojs, dropout_rate, reduce=True):
         super().__init__()
@@ -57,10 +62,38 @@ class CTC(torch.nn.Module):
 
     # ------------------------------------------------------------------ reference surface
     def forward(self, hs_pad, hlens, ys_pad):
-        raise NotImplementedError("CTC.forward (the training loss, ctc.py:41-65) is not on the CUDA inference path")
+        """CTC loss (ctc.py:41-65) -> (loss, ys_hat).  hs_pad (B, Tmax, eprojs), hlens (B), ys_pad (B, Lmax) with
+        ``ignore_id`` (-1) entries dropped wherever they sit; loss = CTCLoss(zero_infinity) / B, summed when ``reduce``;
+        ys_hat = the (Tmax, B, odim) logits.  ctc_lo is ``LinearFn`` on the weight padded to a multiple of 8 rows (the
+        tensor-core GEMM's N), the loss ``CtcLossFn``; labels and lengths stay on the device.  Without autograd
+        (``torch.no_grad()``, as in Lightning's validation step, or when nothing involved needs a gradient) the loss is
+        computed without the beta recursion and nothing is kept for a backward."""
+        if not hs_pad.is_cuda:
+            raise NotImplementedError("CTC.forward: the CTC loss runs on CUDA tensors only (no CPU fallback)")
+        require_cuda(hs_pad, "CTC input")
+        prec = self.precision or default_precision()
+        B = hs_pad.size(0)
+        odim = self.ctc_lo.out_features
+        w, b = self.ctc_lo.weight, self.ctc_lo.bias
+        npad = (odim + 7) // 8 * 8
+        if npad != odim:
+            w, b = F.pad(w, (0, 0, 0, npad - odim)), F.pad(b, (0, npad - odim))
+        x = self.dropout(hs_pad)
+        if torch.is_grad_enabled() and (x.requires_grad or w.requires_grad or b.requires_grad):
+            logits = LinearFn.apply(x, w, b, False, prec)
+            nll = CtcLossFn.apply(logits, hlens, ys_pad, odim, self.ignore_id)
+        else:
+            with torch.no_grad():
+                logits = ops.linear(x, w, b, precision=prec)
+                nll, _ = ctc_loss_forward(logits, hlens, ys_pad, odim, self.ignore_id, want_grad=False)
+        loss = nll / B
+        if self.reduce:
+            loss = loss.sum()
+        self.loss = loss
+        return self.loss, logits[..., :odim].transpose(0, 1)
 
     def loss_fn(self, th_pred, th_target, th_ilen, th_olen):
-        raise NotImplementedError("CTC.loss_fn (ctc.py:32-39) is not on the CUDA inference path")
+        raise NotImplementedError("CTC.loss_fn (ctc.py:32-39) is not on the CUDA path: CTC.forward computes the loss")
 
     def log_softmax(self, hs_pad):
         """(B, Tmax, eprojs) -> (B, Tmax, odim) log-probs (ctc.py:77-84)."""

@@ -42,7 +42,10 @@ def install_head(model):
     """The steps either side of the encoder (SURVEY.md 8f #1).  The reference builds ``proj_encoder`` as a bare
     ``torch.nn.Linear`` and ``ctc`` from a module it imports by name (e2e_asr_conformer.py:11, :31, :56), so instead of
     shadowing an import this re-homes the two sub-modules of an existing ``E2E`` instance: the drop-ins take over the
-    very same ``Parameter`` objects (state dict, optimizer and checkpoint loading are unaffected)."""
+    very same ``Parameter`` objects (state dict, optimizer and checkpoint loading are unaffected).  The drop-ins keep
+    the old modules' train / eval mode and serve both: in ``train()`` ``proj_encoder`` is a Linear with a library
+    backward and ``ctc(x, lengths, label)`` -- the CTC loss ``E2E.forward`` computes (e2e_asr_conformer.py:77), in the
+    training step and in the validation step alike -- runs forward and backward in libavsr_b200."""
     from .espnet_dropin.ctc import CTC, ProjEncoder
 
     old = model.proj_encoder

@@ -291,6 +291,58 @@ class AttentionCoreFn(torch.autograd.Function):
         return dq_k + dq_p, dk, dv, dp, du, dvb, None, None, None
 
 
+def ctc_loss_forward(logits, hlens, ys_pad, odim: int, ignore_id: int = -1, want_grad: bool = False):
+    """torch.nn.CTCLoss(reduction="none", zero_infinity=True), blank 0, on log_softmax of ``logits`` (B, Tmax, ld) fp32
+    (first ``odim`` columns valid) -> (nll (B), state).  ``state`` is what ``ctc_loss_backward`` needs (beta included
+    only when ``want_grad``).  ``hlens`` / ``ys_pad`` (B, Lmax) stay on the device: the label rows are compacted there."""
+    require_cuda(logits, "CTC logits")
+    B, T, ld = logits.shape
+    dev = logits.device
+    hl = hlens.to(device=dev, dtype=torch.int32).contiguous()
+    ys = ys_pad.to(device=dev, dtype=torch.int64).contiguous()
+    L = ys.size(1) if ys.dim() == 2 else 0
+    nll = torch.empty(B, dtype=torch.float32, device=dev)
+    nbytes = int(lib.avsr_ctc_loss_state_bytes(B, T, L))
+    state = torch.empty(max(nbytes, 256), dtype=torch.uint8, device=dev)
+    x = _c(logits)
+    with torch.cuda.device(dev):
+        check(lib.avsr_ctc_loss_fwd(x.data_ptr(), ld, hl.data_ptr(), ys.data_ptr(), B, T, L, odim, ignore_id,
+                                    int(want_grad), nll.data_ptr(), state.data_ptr(), state.numel(), _stream_handle(dev)))
+    return nll, (hl, ys, state)
+
+
+def ctc_loss_backward(logits, saved, odim: int, dnll):
+    """d sum_b(dnll[b] * nll[b]) / d logits, (B, Tmax, ld) with zero padding columns / frames."""
+    hl, ys, state = saved
+    x = _c(logits)
+    B, T, ld = x.shape
+    dnll = dnll.to(torch.float32).contiguous()
+    dx = torch.empty_like(x)
+    with torch.cuda.device(x.device):
+        check(lib.avsr_ctc_loss_bwd(x.data_ptr(), ld, hl.data_ptr(), ys.data_ptr(), B, T, ys.size(1) if ys.dim() == 2 else 0,
+                                    odim, dnll.data_ptr(), state.data_ptr(), state.numel(), dx.data_ptr(), ld,
+                                    _stream_handle(x.device)))
+    return dx
+
+
+class CtcLossFn(torch.autograd.Function):
+    """nll (B) = CTC negative log-likelihood of each utterance (ctc.py:32-39 without the division by B):
+    torch.nn.CTCLoss(reduction="none", zero_infinity=True) on log_softmax(logits).  Forward and backward run in
+    libavsr_b200 (alpha, beta and the gradient on the device, no host synchronisation); the backward returns d logits."""
+
+    @staticmethod
+    def forward(ctx, logits, hlens, ys_pad, odim: int, ignore_id: int):
+        nll, saved = ctc_loss_forward(logits, hlens, ys_pad, odim, ignore_id, want_grad=True)
+        ctx.save_for_backward(logits, *saved)
+        ctx.odim = odim
+        return nll
+
+    @staticmethod
+    def backward(ctx, dnll):
+        logits, *saved = ctx.saved_tensors
+        return ctc_loss_backward(logits, saved, ctx.odim, dnll), None, None, None, None
+
+
 # ------------------------------------------------------------------------------------------------ module forwards (train)
 def feed_forward_train(m, x, precision: str):
     """PositionwiseFeedForward.forward in train mode: w_2(dropout(relu(w_1 x)))."""

@@ -279,6 +279,26 @@ int avsr_relpos_attention_bwd(const float *q, const float *k, const float *v, co
                               float *dq_k, float *dq_p, float *dk, float *dv, float *dp, int B, int T, int H,
                               void *workspace, size_t workspace_bytes, void *stream);
 
+/* CTC loss of the head (espnet/nets/pytorch_backend/ctc.py:32-65: CTC.forward -> loss_fn):
+ * torch.nn.CTCLoss(reduction="none", zero_infinity=True), blank 0, on log_softmax of the logits, per utterance.
+ *   logits  (B*Tmax, ld) fp32 = ctc_lo(hs_pad), rows r = b*Tmax + t; the first odim columns are the vocabulary
+ *   hlens   (B) int32 frames per utterance;  ys_pad (B, Lmax) int64 padded label rows: every entry equal to ignore_id is
+ *           dropped wherever it sits (ctc.py:52, y[y != ignore_id]); the rows are compacted on the device
+ *   nll     (B) fp32 negative log-likelihoods (0 where it is +inf: zero_infinity)
+ * The forward leaves in `state` (>= avsr_ctc_loss_state_bytes) what the backward needs: the compacted labels, the
+ * per-frame log-sum-exp, the log-probs of blank and of the labels, alpha and -- want_grad != 0 only -- beta.  The
+ * backward writes dlogits (B*Tmax, ldd >= odim) = dnll[b] * d nll_b / d logits: 0 on frames t >= hlens[b], on columns
+ * [odim, ldd) and on utterances whose nll is +inf.  dnll (B) is a DEVICE array (nothing is read on the host).
+ * A label outside [1, odim) or hlens[b] outside [0, Tmax] makes that utterance's nll NaN.  Lmax <= 1024.  Every sum has
+ * a fixed order: repeated calls give identical bits. */
+size_t avsr_ctc_loss_state_bytes(int B, int Tmax, int Lmax);
+int avsr_ctc_loss_fwd(const float *logits, long ld, const int32_t *hlens, const int64_t *ys_pad, int B, int Tmax,
+                      int Lmax, int odim, int ignore_id, int want_grad, float *nll, void *state, size_t state_bytes,
+                      void *stream);
+int avsr_ctc_loss_bwd(const float *logits, long ld, const int32_t *hlens, const int64_t *ys_pad, int B, int Tmax,
+                      int Lmax, int odim, const float *dnll, const void *state, size_t state_bytes, float *dlogits,
+                      long ldd, void *stream);
+
 /* ---- on-device collate (SURVEY.md 8f #4) ------------------------------------------------------------------------
  * datamodule/data_module.py:10-41 (`pad` / `collate_pad`) on the GPU: the utterances of a max-frames bucket lie back to
  * back in `flat` (sum of lengths rows x d; offsets[B+1] int64 DEVICE prefix sums), the zero-padded (B, Tmax, d) batch and
