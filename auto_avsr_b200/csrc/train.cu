@@ -157,13 +157,15 @@ __global__ void glu_bwd_kernel(const float* __restrict__ in, const float* __rest
 }
 
 // ------------------------------------------------------------------ BatchNorm (batch statistics) + SiLU
-// per-channel partial sums of v and v^2 over a block of rows: part[blk][2][C]
-__global__ void __launch_bounds__(256) chan_stats_partial_kernel(const float* __restrict__ v, float* __restrict__ part, int rows,
-                                                                 int C, int rows_per_cta) {
+// per-channel partial sums of v - shift and (v - shift)^2 over a block of rows: part[blk][2][C] (shift NULL: 0).  With
+// shift = a provisional mean the sums are centred, so the variance does not come from the difference of two large sums.
+__global__ void __launch_bounds__(256) chan_stats_partial_kernel(const float* __restrict__ v, const float* __restrict__ shift,
+                                                                 float* __restrict__ part, int rows, int C, int rows_per_cta) {
   const int r0 = blockIdx.x * rows_per_cta, r1 = min(rows, r0 + rows_per_cta);
   for (int c = threadIdx.x; c < C; c += 256) {
+    const float m = shift ? shift[c] : 0.f;
     float s = 0.f, q = 0.f;
-    for (int r = r0; r < r1; ++r) { const float t = v[(long)r * C + c]; s += t; q += t * t; }
+    for (int r = r0; r < r1; ++r) { const float t = v[(long)r * C + c] - m; s += t; q += t * t; }
     part[((long)blockIdx.x * 2) * C + c] = s;
     part[((long)blockIdx.x * 2 + 1) * C + c] = q;
   }
@@ -284,14 +286,15 @@ size_t avsr_train_workspace_bytes(int rows, int d, int K) {
 
 int avsr_layernorm_bwd(const float* x, const float* gamma, const float* dy, float* dx, float* dgamma, float* dbeta,
                        int rows, int d, void* workspace, size_t workspace_bytes, void* stream) {
-  AVSR_REQUIRE(x && gamma && dy && dx && dgamma && dbeta && workspace, "NULL argument");
+  AVSR_REQUIRE(gamma && dgamma && dbeta, "NULL argument");
   AVSR_REQUIRE(d > 0 && d % 4 == 0 && d <= kTrMaxVec * 128, "layernorm_bwd: d=%d must be a multiple of 4 and <= 1024", d);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (rows <= 0) {
+  if (rows <= 0) {               // no rows: zero dgamma / dbeta (x, dy, dx of an empty batch may be NULL)
     AVSR_CUDA_TRY(cudaMemsetAsync(dgamma, 0, d * sizeof(float), st));
     AVSR_CUDA_TRY(cudaMemsetAsync(dbeta, 0, d * sizeof(float), st));
     return AVSR_OK;
   }
+  AVSR_REQUIRE(x && dy && dx && workspace, "NULL argument");
   const int nblk = rows < kRedBlocks * 8 ? cdiv(rows, 8) : kRedBlocks;
   const int rpc = cdiv(rows, nblk);
   const int nb = cdiv(rows, rpc);
@@ -381,7 +384,8 @@ int avsr_dwconv_raw(const float* x, const float* w, const float* b, float* y, in
   return launch_dwconv_bn_silu(x, wt, ones, b ? b : zeros, y, B, T, C, K, /*out_kind=*/-1, st);
 }
 
-// sums (2, C): dy == NULL -> [sum v, sum v^2] over the rows; else the BatchNorm+SiLU backward sums [sum ds, sum ds*x_hat]
+// sums (2, C): dy == NULL -> [sum v, sum v^2] over the rows, or with mean given the centred [sum (v - mean),
+// sum (v - mean)^2] (the second pass of the batch statistics); else the BatchNorm+SiLU backward sums [sum ds, sum ds*x_hat]
 // with h = x_hat * gamma + beta, ds = dL/dh of y = silu(h)
 int avsr_chan_sums(const float* v, const float* dy, const float* mean, const float* invstd, const float* gamma,
                    const float* beta, float* sums, int rows, int C, void* workspace, size_t workspace_bytes, void* stream) {
@@ -393,7 +397,7 @@ int avsr_chan_sums(const float* v, const float* dy, const float* mean, const flo
   if ((size_t)nb * 2 * C * sizeof(float) > workspace_bytes) { set_error("chan_sums workspace too small"); return AVSR_E_WORKSPACE; }
   float* part = reinterpret_cast<float*>(workspace);
   if (dy) bn_bwd_partial_kernel<<<nb, 256, 0, st>>>(v, dy, mean, invstd, gamma, beta, part, rows, C, rpc);
-  else chan_stats_partial_kernel<<<nb, 256, 0, st>>>(v, part, rows, C, rpc);
+  else chan_stats_partial_kernel<<<nb, 256, 0, st>>>(v, mean, part, rows, C, rpc);
   AVSR_CHECK_LAUNCH();
   reduce_partials_kernel<<<cdiv(2 * C, 256), 256, 0, st>>>(part, sums, nb, 2 * C);
   AVSR_CHECK_LAUNCH();

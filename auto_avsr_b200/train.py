@@ -171,7 +171,8 @@ class GluFn(torch.autograd.Function):
 
 
 def _chan_sums(v, dy=None, mean=None, invstd=None, gamma=None, beta=None):
-    """(2, C): [sum v, sum v^2] over all rows, or (dy given) the BatchNorm+SiLU backward sums [sum ds, sum ds * x_hat]."""
+    """(2, C): [sum v, sum v^2] over all rows, with ``mean`` alone the centred [sum (v - mean), sum (v - mean)^2], or
+    (dy given) the BatchNorm+SiLU backward sums [sum ds, sum ds * x_hat]."""
     Cc = v.size(-1)
     rows = v.numel() // Cc
     out = torch.empty(2, Cc, dtype=torch.float32, device=v.device)
@@ -199,7 +200,13 @@ class DwConvBnSiluFn(torch.autograd.Function):
 
     The heavy passes (conv, per-channel sums, normalise + SiLU, their backward, tap gradients) run in libavsr_b200; the
     C-length statistics vectors are finalised here between them, which is where SyncBatchNorm's all-reduce goes
-    (one packed [sum, sum^2, count] message forward, [sum ds, sum ds*x_hat] backward: torch/_functions.py:49-159)."""
+    (forward: a packed [sum, count] message, then the centred sums; backward: [sum ds, sum ds*x_hat];
+    torch/_functions.py:49-159).
+
+    The batch statistics take two passes over the conv output: ``sum v`` gives a provisional mean m1, then the centred
+    sums S = sum (v - m1) and Q = sum (v - m1)^2 give mean = m1 + S/n and var = Q/n - (S/n)^2.  The one-pass
+    ``sum v^2 / n - mean^2`` cancels in fp32 once a channel's mean is a few times its standard deviation (the conv bias
+    alone can put it there), which the centred sums do not."""
 
     @staticmethod
     def forward(ctx, x, w, b, bn_w, bn_b, running_mean, running_var, momentum: float, eps: float, group):
@@ -207,15 +214,20 @@ class DwConvBnSiluFn(torch.autograd.Function):
         x, w, b, bn_w, bn_b = _c(x), _c(w), _c(b), _c(bn_w), _c(bn_b)
         B, T, Cc = x.shape
         conv = _dwconv_raw(x, w, b, False)
-        sums = _chan_sums(conv)
+        s1 = _chan_sums(conv)[0]
         n = float(B * T)
         if group is not None:
-            packed = torch.cat([sums.reshape(-1), torch.full((1,), n, dtype=torch.float32, device=x.device)])
+            packed = torch.cat([s1, torch.full((1,), n, dtype=torch.float32, device=x.device)])
             torch.distributed.all_reduce(packed, group=group)
-            sums, n = packed[:-1].reshape(2, Cc), float(packed[-1].item())      # global row count (one host sync)
-        sums64 = sums.double()
-        mean = sums64[0] / n
-        var = (sums64[1] / n - mean * mean).clamp_min_(0.0)
+            s1, n = packed[:-1], float(packed[-1].item())                      # global row count (one host sync)
+        m1 = (s1.double() / n).float().contiguous()                            # provisional mean
+        cs = _chan_sums(conv, mean=m1)                                         # [sum (v - m1), sum (v - m1)^2]
+        if group is not None:
+            torch.distributed.all_reduce(cs, group=group)
+        cs64 = cs.double()
+        dm = cs64[0] / n
+        mean = m1.double() + dm
+        var = (cs64[1] / n - dm * dm).clamp_min_(0.0)
         invstd = torch.rsqrt(var + eps)
         if running_mean is not None:
             with torch.no_grad():
@@ -274,21 +286,29 @@ class AttentionCoreFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx_, dctx):
         q, k, v, p, u, vb, out, lengths = ctx_.saved_tensors
-        q, k, v, p, u, vb, out, dctx = (_c(t) for t in (q, k, v, p, u, vb, out, dctx))
-        B, T, D = q.shape
-        H = ctx_.n_heads
-        dq_k, dq_p, dk, dv = (torch.empty_like(q) for _ in range(4))
-        dp = torch.empty_like(p)
-        ln = lengths.to(torch.int32).contiguous() if ctx_.masked else None
-        ws = _workspace(q.device, int(lib.avsr_relpos_attention_bwd_workspace_bytes(B, T, H)))
-        with torch.cuda.device(q.device):
-            check(lib.avsr_relpos_attention_bwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), p.data_ptr(), u.data_ptr(),
-                                                vb.data_ptr(), _ptr(ln), out.data_ptr(), dctx.data_ptr(), dq_k.data_ptr(),
-                                                dq_p.data_ptr(), dk.data_ptr(), dv.data_ptr(), dp.data_ptr(), B, T, H,
-                                                ws.data_ptr(), ws.numel(), _stream_handle(q.device)))
+        D = q.size(-1)
+        dq_k, dq_p, dk, dv, dp = relpos_attention_bwd(q, k, v, p, u, vb, lengths if ctx_.masked else None, out, dctx,
+                                                      ctx_.n_heads)
         du = colsum(dq_k.reshape(-1, D)).reshape(u.shape)        # d pos_bias_u = sum over (b, t) of the k part of dq
         dvb = colsum(dq_p.reshape(-1, D)).reshape(vb.shape)
         return dq_k + dq_p, dk, dv, dp, du, dvb, None, None, None
+
+
+def relpos_attention_bwd(q, k, v, p, u, vb, lengths, out, dctx, n_heads: int):
+    """avsr_relpos_attention_bwd -> (dq_k, dq_p, dk, dv, dp): the two parts of dq (through the content scores and through
+    the rel-pos scores), the key / value gradients (B, T, H*64) and the pos-table gradient (2T-1, H*64)."""
+    q, k, v, p, u, vb, out, dctx = (_c(t) for t in (q, k, v, p, u, vb, out, dctx))
+    B, T, D = q.shape
+    dq_k, dq_p, dk, dv = (torch.empty_like(q) for _ in range(4))
+    dp = torch.empty_like(p)
+    ln = lengths.to(torch.int32).contiguous() if lengths is not None else None
+    ws = _workspace(q.device, int(lib.avsr_relpos_attention_bwd_workspace_bytes(B, T, n_heads)))
+    with torch.cuda.device(q.device):
+        check(lib.avsr_relpos_attention_bwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), p.data_ptr(), u.data_ptr(),
+                                            vb.data_ptr(), _ptr(ln), out.data_ptr(), dctx.data_ptr(), dq_k.data_ptr(),
+                                            dq_p.data_ptr(), dk.data_ptr(), dv.data_ptr(), dp.data_ptr(), B, T, n_heads,
+                                            ws.data_ptr(), ws.numel(), _stream_handle(q.device)))
+    return dq_k, dq_p, dk, dv, dp
 
 
 def ctc_loss_forward(logits, hlens, ys_pad, odim: int, ignore_id: int = -1, want_grad: bool = False):

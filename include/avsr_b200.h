@@ -252,7 +252,8 @@ int avsr_glu_bwd(const float *in, const float *dy, float *din, long rows, int C,
  * (Sync)BatchNorm needs: the per-channel sums leave the library so that the host can all-reduce them over the ranks
  * (train.py:31 sync_batchnorm=True) before it finalises mean / invstd / the running statistics.
  *   avsr_dwconv_raw      y = conv(x) + b, raw fp32 (flip != 0: taps reversed, b may be NULL = the input gradient)
- *   avsr_chan_sums       sums (2,C): [sum v, sum v^2] (dy NULL) or the backward sums [sum ds, sum ds*x_hat]
+ *   avsr_chan_sums       sums (2,C): [sum v, sum v^2] (dy, mean NULL), the centred [sum (v-mean), sum (v-mean)^2]
+ *                        (dy NULL, mean given) or the backward sums [sum ds, sum ds*x_hat] (dy given)
  *   avsr_bn_silu_fwd     y = silu((v - mean) * invstd * gamma + beta)
  *   avsr_bn_silu_bwd_dx  dv from dy with the GLOBAL sums and 1 / (global row count)
  *   avsr_dwconv_wgrad    dw (C,1,K), db (C) */
