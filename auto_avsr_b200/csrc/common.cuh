@@ -72,24 +72,32 @@ inline bool pdl_enabled() {
 
 template <typename... KArgs, typename... Args, size_t... I>
 inline cudaError_t launch_kernel_impl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
-                                      std::index_sequence<I...>, Args&&... args) {
+                                      unsigned cluster, std::index_sequence<I...>, Args&&... args) {
   std::tuple<KArgs...> params(static_cast<KArgs>(args)...);
   void* ptrs[] = {const_cast<void*>(static_cast<const void*>(&std::get<I>(params)))...};
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute attr[2];
+  int n = 0;
+  if (pdl_enabled()) {
+    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n++].val.programmaticStreamSerializationAllowed = 1;
+  }
+  if (cluster > 1) {
+    attr[n].id = cudaLaunchAttributeClusterDimension;
+    attr[n].val.clusterDim.x = cluster; attr[n].val.clusterDim.y = 1; attr[n++].val.clusterDim.z = 1;
+  }
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = n;
   return cudaLaunchKernelExC(&cfg, reinterpret_cast<const void*>(kernel), ptrs);
 }
-// launch `kernel<<<grid, block, smem, st>>>(args...)` with the PDL attribute
+// launch `kernel<<<grid, block, smem, st>>>(args...)` with the PDL attribute, in clusters of `cluster` CTAs along x
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
-                                 Args&&... args) {
+                                 unsigned cluster, Args&&... args) {
   static_assert(sizeof...(KArgs) == sizeof...(Args), "kernel argument count mismatch");
-  return launch_kernel_impl(kernel, grid, block, smem, st, std::index_sequence_for<KArgs...>{}, std::forward<Args>(args)...);
+  return launch_kernel_impl(kernel, grid, block, smem, st, cluster, std::index_sequence_for<KArgs...>{},
+                            std::forward<Args>(args)...);
 }
 
 // opt a kernel into > 48 KB of dynamic shared memory; remembered per device (one process may drive several GPUs)
@@ -107,7 +115,14 @@ inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block
 #define AVSR_LAUNCH(kernel, grid, block, smem, st, ...)                                                \
   do {                                                                                                 \
     ::avsr::g_launches.fetch_add(1);                                                                   \
-    AVSR_CUDA_TRY(::avsr::launch_kernel(kernel, dim3(grid), dim3(block), (size_t)(smem), st, __VA_ARGS__)); \
+    AVSR_CUDA_TRY(::avsr::launch_kernel(kernel, dim3(grid), dim3(block), (size_t)(smem), st, 1u, __VA_ARGS__)); \
+  } while (0)
+// the same, in clusters of `cluster` CTAs along x (grid a multiple of it)
+#define AVSR_LAUNCH_CLUSTER(kernel, grid, block, smem, st, cluster, ...)                                         \
+  do {                                                                                                          \
+    ::avsr::g_launches.fetch_add(1);                                                                            \
+    AVSR_CUDA_TRY(::avsr::launch_kernel(kernel, dim3(grid), dim3(block), (size_t)(smem), st, (unsigned)(cluster), \
+                                        __VA_ARGS__));                                                          \
   } while (0)
 
 // ---------------------------------------------------------------- device helpers

@@ -7,15 +7,15 @@ namespace avsr {
 // ---------------------------------------------------------------- staged (coalesced) epilogue
 // Each epilogue warp drains 32 accumulator rows x CW columns at a time: lane = row of the fp32 accumulator tile, per-
 // column math (bias / ReLU / GLU / pos biases, vectors read from shared memory), conversion to the destination
-// storage, then a transpose through a private 32 x 144-byte staging buffer so that global memory sees, per
-// quarter-warp, 8 lanes x 16 B = one full 128-byte row segment -- instead of 32 partial sectors per store instruction
-// of direct lane-per-row stores.  Residual reads use the same mapping.
-constexpr int STG_ROW = 144;            // 128 B payload + 16 B pad: conflict-free lane-per-row 16-byte writes
-constexpr int STG_WARP = 32 * STG_ROW;  // 4608 B per epilogue warp
+// storage, then a transpose through shared memory so that global memory sees, per quarter-warp, 8 lanes x 16 B = one
+// full 128-byte row segment -- instead of 32 partial sectors per store instruction of direct lane-per-row stores.
+// Residual reads use the same mapping.  The transpose goes through the accumulator rows the lane has just read
+// (`stg` = first of the warp's 32 rows at the chunk's first column, rows `row_bytes` apart): a row stride of 4 banks
+// mod 32 keeps the lane-per-row 16-byte writes conflict-free.
 
 // lane writes its row: 32 fp32 values, optionally rounded to TF32
-__device__ __forceinline__ void stage_write_f32(uint8_t* stg, int lane, const float* o, bool round) {
-  uint8_t* row = stg + lane * STG_ROW;
+__device__ __forceinline__ void stage_write_f32(uint8_t* stg, int row_bytes, int lane, const float* o, bool round) {
+  uint8_t* row = stg + lane * row_bytes;
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     float4 t = make_float4(o[4 * j], o[4 * j + 1], o[4 * j + 2], o[4 * j + 3]);
@@ -24,8 +24,8 @@ __device__ __forceinline__ void stage_write_f32(uint8_t* stg, int lane, const fl
   }
 }
 // lane writes its row: 64 values converted to half (128 bytes)
-__device__ __forceinline__ void stage_write_f16(uint8_t* stg, int lane, const float* o) {
-  uint8_t* row = stg + lane * STG_ROW;
+__device__ __forceinline__ void stage_write_f16(uint8_t* stg, int row_bytes, int lane, const float* o) {
+  uint8_t* row = stg + lane * row_bytes;
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     uint4 t;
@@ -41,15 +41,19 @@ __device__ __forceinline__ void stage_write_f16(uint8_t* stg, int lane, const fl
 template <typename TOp> struct StageOp;
 template <> struct StageOp<float> {
   static constexpr int kCols = 32;   // operand columns per 128-byte row segment
-  __device__ static void write(uint8_t* stg, int lane, const float* o) { stage_write_f32(stg, lane, o, true); }
+  __device__ static void write(uint8_t* stg, int row_bytes, int lane, const float* o) {
+    stage_write_f32(stg, row_bytes, lane, o, true);
+  }
 };
 template <> struct StageOp<__half> {
   static constexpr int kCols = 64;
-  __device__ static void write(uint8_t* stg, int lane, const float* o) { stage_write_f16(stg, lane, o); }
+  __device__ static void write(uint8_t* stg, int row_bytes, int lane, const float* o) {
+    stage_write_f16(stg, row_bytes, lane, o);
+  }
 };
 // transposed read: iteration `it` (0..7) gives this lane the 16-byte piece (lane & 7) of row it*4 + (lane >> 3)
-__device__ __forceinline__ uint4 stage_read(const uint8_t* stg, int it, int lane) {
-  return *reinterpret_cast<const uint4*>(stg + (it * 4 + (lane >> 3)) * STG_ROW + (lane & 7) * 16);
+__device__ __forceinline__ uint4 stage_read(const uint8_t* stg, int row_bytes, int it, int lane) {
+  return *reinterpret_cast<const uint4*>(stg + (it * 4 + (lane >> 3)) * row_bytes + (lane & 7) * 16);
 }
 
 // ---- per-mode emit of one 16-byte piece: row m, first column n (global indices of the GEMM) ----

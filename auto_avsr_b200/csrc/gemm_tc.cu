@@ -14,6 +14,7 @@
 // epilogue.  The tile width is chosen per problem by a small cost model (bytes through L2 vs tensor-pipe time).
 #include "common.cuh"
 #include "epilogue.cuh"
+#include "gemm_schedule.cuh"
 #include "sm90.cuh"
 
 namespace avsr {
@@ -87,8 +88,7 @@ struct TcCfg {
   static constexpr int kAccLd = BN + 4;                 // fp32 accumulator tile row stride (conflict-free float4 rows)
   static constexpr int kAccBytes = TC_BM * kAccLd * 4;
   static constexpr int kVecBytes = 3 * BN * 4;          // bias / pos_bias_u / pos_bias_v of the tile's columns
-  static constexpr int kStagingBytes = 8 * STG_WARP;    // epilogue transpose buffers
-  static constexpr int kFixedBytes = 1024 /*align slack*/ + 256 /*barriers*/ + kAccBytes + kVecBytes + kStagingBytes;
+  static constexpr int kFixedBytes = 1024 /*align slack*/ + 256 /*barriers*/ + kAccBytes + kVecBytes;
   static constexpr int kStagesFit = (TC_SMEM_BUDGET - kFixedBytes) / kStageBytes;
   static constexpr int kStages = kStagesFit > 8 ? 8 : kStagesFit;
   static constexpr int kSmem = kStages * kStageBytes + kFixedBytes;
@@ -111,15 +111,21 @@ template <> struct OpTraits<__half> {
   }
 };
 
-template <int MODE, int BN, typename TOp>
+template <int MODE, int BN, typename TOp, int CM, int CN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int K, int tiles_m,
                int tiles_n, int splits, EpiParams ep) {
-  // PERSISTENT: CTA c processes tiles c, c + gridDim.x, ... (n fastest, so concurrently running CTAs share A rows in
-  // L2).  The TMA ring never drains between tiles: the producer fetches the next tile's k-blocks while the consumer
-  // warpgroups run the epilogue of the current one.
+  // PERSISTENT: cluster c processes cluster tiles c, c + clusters, ... (n fastest, so concurrently running CTAs share
+  // A rows in L2; gemm_schedule.cuh).  The TMA ring never drains between tiles: the producer fetches the next tile's
+  // k-blocks while the consumer warpgroups run the epilogue of the current one.
+  // Clusters of CM x CN CTAs (tensor maps with boxes of BN / CM rows of Bw and 128 / CN rows of A): the CM CTAs of a
+  // cluster column share their Bw tile and each loads 1/CM of it, multicast to all of them; likewise the CN CTAs of a
+  // cluster row share A.  Every consumer warp releases a stage to the producer of every CTA of the cluster, so a
+  // stage is refilled (by any peer) only after all CTAs it lands in are done with it.
   using Cfg = TcCfg<BN>;
   using Op = OpTraits<TOp>;
+  constexpr int CS = CM * CN;
+  static_assert(CS == 1 || (CM <= 2 && CN <= 2), "cluster shapes: 1x1, 2x1, 1x2, 2x2");
   constexpr int S = Cfg::kStages;
   constexpr int KE = Op::kElemsPerBlock;
   constexpr int LD = Cfg::kAccLd;
@@ -131,54 +137,69 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   int* s_flag = reinterpret_cast<int*>(gen + S * Cfg::kStageBytes + 2 * S * 8);   // split-K: "this CTA arrived last"
   float* s_acc = reinterpret_cast<float*>(gen + S * Cfg::kStageBytes + 256);      // [TC_BM][LD]
   float* s_vec = s_acc + TC_BM * LD;                                               // [3][BN]
-  uint8_t* stg_base = reinterpret_cast<uint8_t*>(s_vec + 3 * BN);
   auto full_bar = [&](int s) { return bars + 8u * s; };
   auto empty_bar = [&](int s) { return bars + 8u * (S + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nkb = K / KE;
-  const int total_tiles = tiles_m * tiles_n;
-  // split-K (LINEAR into the residual stream only): work item = (tile, K-slice); slice-major order so that CTAs
-  // running at the same time reduce into different tiles.
-  const int total_items = total_tiles * splits;
+  // split-K (LINEAR into the residual stream only, 1 x 1 clusters): work item = (tile, K-slice); slice-major order so
+  // that CTAs running at the same time reduce into different tiles.
+  const int crank = CS > 1 ? (int)cluster_ctarank() : 0;
+  const int cluster_id = blockIdx.x / CS, clusters = gridDim.x / CS;
+  const int total_items = tc_cluster_items(tiles_m, tiles_n, splits, CM, CN);
 
   pdl_launch_dependents();
   AVSR_TSPAN_OPEN(400 + MODE, (unsigned)BN);
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8); }   // 8 consumer warps
+    // empty: 8 consumer warps of each CTA the stage's loads land in
+    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8 * CS); }
     fence_barrier_init();
   }
   __syncthreads();
+  if constexpr (CS > 1) cluster_sync();   // peers' barriers are initialised before any multicast or remote arrive
   pdl_wait();   // everything above overlapped the previous kernel's tail; from here on we touch its outputs
   AVSR_TSPAN_DEP();
 
-  if (warp == 0) {
-    // TMA producer: warp-uniform loop, only the instruction issue is guarded by elect.sync
-    int it = 0;                                         // running k-block counter across tiles
-    for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-      const int tile = item % total_tiles, split = item / total_tiles;
-      const int m0 = (tile / tiles_n) * TC_BM, n0 = (tile % tiles_n) * BN;
-      const int kb0 = split * nkb / splits, kb1 = (split + 1) * nkb / splits;
-      for (int kb = kb0; kb < kb1; ++kb, ++it) {
-        const int s = it % S;
-        const uint32_t ph = (it / S) & 1;
-        mbar_wait(empty_bar(s), ph ^ 1);
-        if (elect_one_sync()) {
-          mbar_expect_tx(full_bar(s), Cfg::kStageBytes);
-          const uint32_t a_dst = base + s * Cfg::kStageBytes;
-          tma_load_2d(a_dst, &tmA, kb * KE, m0, full_bar(s));
-          tma_load_2d(a_dst + Cfg::kABytes, &tmB, kb * KE, n0, full_bar(s));
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
+    if (warp == 0) {
+      // TMA producer: warp-uniform loop, only the instruction issue is guarded by elect.sync
+      const int cm = crank % CM, cn = crank / CM;
+      uint16_t a_mask = 0, b_mask = 0;              // peers sharing this CTA's A rows / Bw rows
+      for (int j = 0; j < CN; ++j) a_mask |= (uint16_t)(1u << (cm + CM * j));
+      for (int i = 0; i < CM; ++i) b_mask |= (uint16_t)(1u << (i + CM * cn));
+      int it = 0;                                   // running k-block counter across tiles
+      for (int item = cluster_id; item < total_items; item += clusters) {
+        const TcWork w = tc_work_item(item, crank, tiles_m, tiles_n, CM, CN);
+        const int m0 = w.tm * TC_BM, n0 = w.tn * BN;
+        const int kb0 = w.split * nkb / splits, kb1 = (w.split + 1) * nkb / splits;
+        for (int kb = kb0; kb < kb1; ++kb, ++it) {
+          const int s = it % S;
+          const uint32_t ph = (it / S) & 1;
+          mbar_wait(empty_bar(s), ph ^ 1);
+          if (elect_one_sync()) {
+            mbar_expect_tx(full_bar(s), Cfg::kStageBytes);   // own slices + the peers' multicast slices
+            const uint32_t a_dst = base + s * Cfg::kStageBytes;
+            if constexpr (CN == 1) tma_load_2d(a_dst, &tmA, kb * KE, m0, full_bar(s));
+            else tma_load_2d_mc(a_dst + cn * (TC_BM / CN) * 128, &tmA, kb * KE, m0 + cn * (TC_BM / CN), full_bar(s), a_mask);
+            if constexpr (CM == 1) tma_load_2d(a_dst + Cfg::kABytes, &tmB, kb * KE, n0, full_bar(s));
+            else tma_load_2d_mc(a_dst + Cfg::kABytes + cm * (BN / CM) * 128, &tmB, kb * KE, n0 + cm * (BN / CM),
+                                full_bar(s), b_mask);
+          }
         }
       }
     }
-  } else if (warp >= 4) {
+  } else {
+    setmaxnreg_inc<232>();
     const int wg = (warp - 4) >> 2;              // consumer warpgroup: accumulator rows [64 wg, 64 wg + 64)
     const int e = warp - 4;                      // epilogue warp 0..7
     const int q = e & 3;                         // 32-row slab of the tile this warp drains
     const int chalf = e >> 2;                    // which half of the tile's columns this warp drains
-    uint8_t* stg = stg_base + e * STG_WARP;
+    constexpr int RB = LD * 4;                               // accumulator row stride in bytes
+    // transpose buffer of a chunk: the warp's own accumulator rows, from the chunk's first column (epilogue.cuh)
+    auto stg_at = [&](int c) { return reinterpret_cast<uint8_t*>(s_acc + (q * 32) * LD + c); };
     const int cb = chalf * (BN / 2), ce = cb + BN / 2;      // this warp's columns of the tile
     const int pr = lane >> 3;                                // row (of 4) this lane emits per read iteration
     const int pc = lane & 7;                                 // 16-byte piece of the 128-byte row segment
@@ -195,11 +216,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    // a stage is released to the producer of every CTA of the cluster (lane r -> CTA r)
+    auto release = [&](int s) {
+      if constexpr (CS == 1) { if (lane == 0) mbar_arrive(empty_bar(s)); }
+      else { if (lane < CS) mbar_arrive_cluster(empty_bar(s), (uint32_t)lane); }
+    };
     int it = 0;
 #pragma unroll 1
-    for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-    const int tile = item % total_tiles, split = item / total_tiles;
-    const int m0 = (tile / tiles_n) * TC_BM, n0 = (tile % tiles_n) * BN;
+    for (int item = cluster_id; item < total_items; item += clusters) {
+    const TcWork w = tc_work_item(item, crank, tiles_m, tiles_n, CM, CN);
+    const int split = w.split, tile = w.tm * tiles_n + w.tn;
+    const int m0 = w.tm * TC_BM, n0 = w.tn * BN;
     const int kb0 = split * nkb / splits, kb1 = (split + 1) * nkb / splits;
     // ---- main loop: one wgmma group in flight; a stage is released once the group that read it has retired
     for (int kb = kb0; kb < kb1; ++kb, ++it) {
@@ -215,11 +242,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       wgmma_commit();
       wgmma_wait<1>();
       wgmma_fence_regs<BN / 2>(acc);
-      if (kb != kb0 && lane == 0) mbar_arrive(empty_bar((it - 1) % S));
+      if (kb != kb0) release((it - 1) % S);
     }
     wgmma_wait<0>();
     wgmma_fence_regs<BN / 2>(acc);
-    if (lane == 0) mbar_arrive(empty_bar((it - 1) % S));
+    release((it - 1) % S);
+    if (!w.valid) continue;                        // past the matrix edge: took part in the loads, stores nothing
     // ---- accumulator -> shared memory (fp32 rows), the tile's per-column vectors next to it
     asm volatile("bar.sync 1, 256;" ::: "memory");   // previous tile's readers of s_acc / s_vec are done
     {
@@ -254,22 +282,24 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll 1
         for (int g = 0; g < BN; g += 128) {
           const int c = g + chalf * 32;
+          uint8_t* stg = stg_at(c);
           float val[32], gate[32];
           acc_ld32(c, val);
           acc_ld32(c + 64, gate);
           const float* sb = s_vec + c;
 #pragma unroll
           for (int j = 0; j < 32; ++j) val[j] = (val[j] + sb[j]) * sigmoidf_fast(gate[j] + sb[64 + j]);
-          stage_write_f32(stg, lane, val, false);
+          stage_write_f32(stg, RB, lane, val, false);
           __syncwarp();
 #pragma unroll
-          for (int it8 = 0; it8 < 8; ++it8) emit_glu(ep, mw + it8 * 4 + pr, n0 + c + pc * 4, stage_read(stg, it8, lane));
+          for (int it8 = 0; it8 < 8; ++it8) emit_glu(ep, mw + it8 * 4 + pr, n0 + c + pc * 4, stage_read(stg, RB, it8, lane));
           __syncwarp();
         }
       } else if constexpr (MODE == EPI_LINEAR) {
         if (!ep.round_out) {                                 // fp32 destination (+ residual)
 #pragma unroll 1
           for (int c = cb; c < ce; c += 32) {
+            uint8_t* stg = stg_at(c);
             float v[32];
             acc_ld32(c, v);
             const float* sb = s_vec + c;
@@ -277,7 +307,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
               for (int j = 0; j < 32; ++j) { v[j] += sb[j]; if (ep.relu) v[j] = fmaxf(v[j], 0.f); }
             }
-            stage_write_f32(stg, lane, v, false);
+            stage_write_f32(stg, RB, lane, v, false);
             __syncwarp();
             const int n = n0 + c + pc * 4;
             if (splits > 1) {
@@ -287,7 +317,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
               for (int it8 = 0; it8 < 8; ++it8) {
                 const int m = mw + it8 * 4 + pr;
-                const uint4 pay = stage_read(stg, it8, lane);
+                const uint4 pay = stage_read(stg, RB, it8, lane);
                 if (m < ep.M && n < ep.N) *reinterpret_cast<uint4*>(part + (long)m * ep.ldo + n) = pay;
               }
             } else {
@@ -305,7 +335,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
             for (int it8 = 0; it8 < 8; ++it8) {
               const int m = mw + it8 * 4 + pr;
-              const uint4 pay = stage_read(stg, it8, lane);
+              const uint4 pay = stage_read(stg, RB, it8, lane);
               float4 o = *reinterpret_cast<const float4*>(&pay);
               if (ep.resid) {
                 o.x = r[it8].x + ep.alpha * o.x; o.y = r[it8].y + ep.alpha * o.y;
@@ -320,17 +350,18 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         } else {                                             // operand-typed destination (FFN hidden)
 #pragma unroll 1
           for (int c = cb; c < ce; c += OC) {
+            uint8_t* stg = stg_at(c);
             float v[OC];
 #pragma unroll
             for (int k = 0; k < OC; k += 32) acc_ld32(c + k, v + k);
             const float* sb = s_vec + c;
 #pragma unroll
             for (int j = 0; j < OC; ++j) { v[j] += sb[j]; if (ep.relu) v[j] = fmaxf(v[j], 0.f); }
-            StageOp<TOp>::write(stg, lane, v);
+            StageOp<TOp>::write(stg, RB, lane, v);
             __syncwarp();
 #pragma unroll
             for (int it8 = 0; it8 < 8; ++it8)
-              emit_linear_op<TOp>(ep, mw + it8 * 4 + pr, n0 + c + pc * ONE, stage_read(stg, it8, lane));
+              emit_linear_op<TOp>(ep, mw + it8 * 4 + pr, n0 + c + pc * ONE, stage_read(stg, RB, it8, lane));
             __syncwarp();
           }
         }
@@ -340,6 +371,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int D = ep.H * kHeadDim;
 #pragma unroll 1
         for (int c = cb; c < ce; c += OC) {
+          uint8_t* stg = stg_at(c);
           float v[OC];
 #pragma unroll
           for (int k = 0; k < OC; k += 32) acc_ld32(c + k, v + k);
@@ -365,34 +397,39 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               }
             }
             if (n < D) {                                     // q: two outputs, q + pos_bias_u and q + pos_bias_v
+              // the first output's transpose overwrites the chunk's first 128 bytes: keep those accumulators
+              float keep[32];
+              acc_ld32(c, keep);
               const float* su = s_vec + BN + c;
 #pragma unroll
               for (int j = 0; j < OC; ++j) v[j] += su[j];
-              StageOp<TOp>::write(stg, lane, v);
+              StageOp<TOp>::write(stg, RB, lane, v);
               __syncwarp();
 #pragma unroll
               for (int it8 = 0; it8 < 8; ++it8)
-                emit_heads<TOp>(ep, ep.qu, rok[it8], rb[it8], rt[it8], hh, d0, stage_read(stg, it8, lane));
+                emit_heads<TOp>(ep, ep.qu, rok[it8], rb[it8], rt[it8], hh, d0, stage_read(stg, RB, it8, lane));
               __syncwarp();
-              // second output: re-read the accumulator chunk (cheaper than keeping two register copies)
+              // second output: the accumulator chunk again (kept registers + the part still in shared memory)
 #pragma unroll
-              for (int k = 0; k < OC; k += 32) acc_ld32(c + k, v + k);
+              for (int j = 0; j < 32; ++j) v[j] = keep[j];
+#pragma unroll
+              for (int k = 32; k < OC; k += 32) acc_ld32(c + k, v + k);
               const float* sv = s_vec + 2 * BN + c;
 #pragma unroll
               for (int j = 0; j < OC; ++j) v[j] += sb[j] + sv[j];
-              StageOp<TOp>::write(stg, lane, v);
+              StageOp<TOp>::write(stg, RB, lane, v);
               __syncwarp();
 #pragma unroll
               for (int it8 = 0; it8 < 8; ++it8)
-                emit_heads<TOp>(ep, ep.qv, rok[it8], rb[it8], rt[it8], hh, d0, stage_read(stg, it8, lane));
+                emit_heads<TOp>(ep, ep.qv, rok[it8], rb[it8], rt[it8], hh, d0, stage_read(stg, RB, it8, lane));
               __syncwarp();
             } else {
-              StageOp<TOp>::write(stg, lane, v);
+              StageOp<TOp>::write(stg, RB, lane, v);
               __syncwarp();
               void* dst = n < 2 * D ? ep.kk : ep.vt;
 #pragma unroll
               for (int it8 = 0; it8 < 8; ++it8)
-                emit_heads<TOp>(ep, dst, rok[it8], rb[it8], rt[it8], hh, d0, stage_read(stg, it8, lane));
+                emit_heads<TOp>(ep, dst, rok[it8], rb[it8], rt[it8], hh, d0, stage_read(stg, RB, it8, lane));
               __syncwarp();
             }
           } else {
@@ -400,11 +437,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
               for (int j = 0; j < OC; ++j) v[j] += row_bias;
             }
-            StageOp<TOp>::write(stg, lane, v);
+            StageOp<TOp>::write(stg, RB, lane, v);
             __syncwarp();
 #pragma unroll
             for (int it8 = 0; it8 < 8; ++it8) {
-              const uint4 pay = stage_read(stg, it8, lane);
+              const uint4 pay = stage_read(stg, RB, it8, lane);
               if constexpr (MODE == EPI_VT) emit_vt<TOp>(ep, mw + it8 * 4 + pr, n + pc * ONE, pay);
               else emit_pos<TOp>(ep, mw + it8 * 4 + pr, n + pc * ONE, pay);
             }
@@ -466,6 +503,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }  // tile loop
   }
   __syncthreads();
+  if constexpr (CS > 1) cluster_sync();   // no CTA leaves while a peer may still arrive on or load into its memory
   AVSR_TSPAN_CLOSE();
 }
 
@@ -481,19 +519,44 @@ static int num_sms() {
   return n;
 }
 
-template <int MODE, int BN, typename TOp>
+// Most clusters of this kernel that can be resident at once (GPCs need not hold a multiple of the cluster size).
+template <typename Kernel>
+static int max_active_clusters(Kernel kernel, int cs, int smem) {
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(cs); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = smem;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = cs; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+  cfg.attrs = &attr; cfg.numAttrs = 1;
+  int n = 0;
+  if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess) return 0;
+  return n;
+}
+
+template <int MODE, int BN, typename TOp, int CM, int CN>
 static int launch_tc(const void* A, const void* Bw, int M, int N, int K, int splits, const EpiParams& ep,
                      cudaStream_t st) {
   using Cfg = TcCfg<BN>;
+  constexpr int CS = CM * CN;
+  auto kernel = gemm_tc_kernel<MODE, BN, TOp, CM, CN>;
   CUtensorMap tmA, tmB;
-  AVSR_TRY(make_tmap_2d(&tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)K, TC_BM, (int)sizeof(TOp)));
-  AVSR_TRY(make_tmap_2d(&tmB, Bw, (uint64_t)N, (uint64_t)K, (uint64_t)K, BN, (int)sizeof(TOp)));
-  AVSR_SET_MAX_SMEM((gemm_tc_kernel<MODE, BN, TOp>), Cfg::kSmem);
+  AVSR_TRY(make_tmap_2d(&tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)K, TC_BM / CN, (int)sizeof(TOp)));
+  AVSR_TRY(make_tmap_2d(&tmB, Bw, (uint64_t)N, (uint64_t)K, (uint64_t)K, BN / CM, (int)sizeof(TOp)));
+  AVSR_SET_MAX_SMEM(kernel, Cfg::kSmem);
   const int tiles_m = cdiv(M, TC_BM), tiles_n = cdiv(N, BN);
-  if (splits > kMaxSplits || tiles_m * tiles_n > kSplitCounters) splits = 1;   // caller's workspace contract
-  const int total = tiles_m * tiles_n * splits;
-  const int grid = total < num_sms() ? total : num_sms();
-  AVSR_LAUNCH((gemm_tc_kernel<MODE, BN, TOp>), grid, TC_THREADS, Cfg::kSmem, st, tmA, tmB, K, tiles_m, tiles_n, splits, ep);
+  if (CS > 1 || splits > kMaxSplits || tiles_m * tiles_n > kSplitCounters) splits = 1;   // caller's workspace contract
+  const int total = tc_cluster_items(tiles_m, tiles_n, splits, CM, CN);
+  int slots = num_sms();
+  if constexpr (CS > 1) {
+    static int dev_done = -1, active = 0;
+    int dev = 0;
+    AVSR_CUDA_TRY(cudaGetDevice(&dev));
+    if (dev_done != dev) { active = max_active_clusters(kernel, CS, Cfg::kSmem); dev_done = dev; }
+    AVSR_REQUIRE(active > 0, "gemm_tc: no %dx%d cluster of this kernel fits on the device", CM, CN);
+    slots = active;
+  }
+  const int grid = (total < slots ? total : slots) * CS;
+  AVSR_LAUNCH_CLUSTER(kernel, grid, TC_THREADS, Cfg::kSmem, st, CS, tmA, tmB, K, tiles_m, tiles_n, splits, ep);
   return AVSR_OK;
 }
 
@@ -503,7 +566,11 @@ static int launch_tc(const void* A, const void* Bw, int M, int N, int K, int spl
 // the last item (it does not overlap the main loop of a following item: the accumulator lives in the registers of the
 // warpgroups that also run the epilogue).  Split-K (only for GEMMs that accumulate into the fp32 residual stream)
 // spreads a long K over more SMs.
-struct TileChoice { int bn, splits; };
+// It picks 1 x 1 clusters only.  Multicast clusters cut the modelled L2 -> SM bytes by 25 % (2x1, 1x2) or 50 % (2x2)
+// but measured about 1.8x slower at the S2 shapes on an H100 80GB HBM3 at 400 W (FFN w_1 1600x3072x768: 22.7 us at
+// 1x1, 42.6 us at 2x1): the main loop waits on load latency, not L2 bandwidth (DESIGN.md section 4); clusters stay
+// reachable through AVSR_B200_TILE for sweeps.
+struct TileChoice { int bn, splits, cm, cn; };
 static const int kTileWidths[] = {64, 128};
 
 static TileChoice choose_tile(int mode, int M, int N, int K, int esz, bool operand_dest, bool can_split) {
@@ -512,7 +579,7 @@ static TileChoice choose_tile(int mode, int M, int N, int K, int esz, bool opera
   const int nkb = K / (128 / esz);
   const int sms = num_sms();
   double best = 1e30;
-  TileChoice pick{128, 1};
+  TileChoice pick{128, 1, 1, 1};
   for (const int bn : kTileWidths) {
     if (mode == EPI_GLU && bn % 128 != 0) continue;
     if (bn == 64 && esz == 2 && (mode != EPI_LINEAR || operand_dest)) continue;   // needs 64-column row segments
@@ -529,19 +596,30 @@ static TileChoice choose_tile(int mode, int M, int N, int K, int esz, bool opera
       // fix-up: the last arriver re-reads `splits` fp32 partial tiles through the same port
       const double t_red = splits > 1 ? (double)splits * 128.0 * bn * 4.0 / ingest : 0.0;
       const double est = (t_mma > t_in ? t_mma : t_in) + t_epi + t_red + 4000.0;
-      if (est < best) { best = est; pick = TileChoice{bn, splits}; }
+      if (est < best) { best = est; pick = TileChoice{bn, splits, 1, 1}; }
     }
   }
   return pick;
+}
+
+template <int MODE, int BN, typename TOp>
+static int dispatch_cluster(TileChoice t, const void* A, const void* Bw, int M, int N, int K, const EpiParams& ep,
+                            cudaStream_t st) {
+  if (t.cm == 1 && t.cn == 1) return launch_tc<MODE, BN, TOp, 1, 1>(A, Bw, M, N, K, t.splits, ep, st);
+  if (t.cm == 2 && t.cn == 1) return launch_tc<MODE, BN, TOp, 2, 1>(A, Bw, M, N, K, 1, ep, st);
+  if (t.cm == 1 && t.cn == 2) return launch_tc<MODE, BN, TOp, 1, 2>(A, Bw, M, N, K, 1, ep, st);
+  if (t.cm == 2 && t.cn == 2) return launch_tc<MODE, BN, TOp, 2, 2>(A, Bw, M, N, K, 1, ep, st);
+  set_error("gemm_tc: no kernel for cluster %dx%d", t.cm, t.cn);
+  return AVSR_E_INVALID;
 }
 
 template <int MODE, typename TOp>
 static int dispatch_tile(TileChoice t, const void* A, const void* Bw, int M, int N, int K, const EpiParams& ep,
                          cudaStream_t st) {
   if (t.bn == 64) {
-    if constexpr (MODE != EPI_GLU) return launch_tc<MODE, 64, TOp>(A, Bw, M, N, K, t.splits, ep, st);
+    if constexpr (MODE != EPI_GLU) return dispatch_cluster<MODE, 64, TOp>(t, A, Bw, M, N, K, ep, st);
   }
-  if (t.bn == 128) return launch_tc<MODE, 128, TOp>(A, Bw, M, N, K, t.splits, ep, st);
+  if (t.bn == 128) return dispatch_cluster<MODE, 128, TOp>(t, A, Bw, M, N, K, ep, st);
   set_error("gemm_tc: no kernel for tile 128x%d", t.bn);
   return AVSR_E_INVALID;
 }
@@ -558,14 +636,15 @@ static int dispatch_mode(int mode, const void* A, const void* Bw, int M, int N, 
   const bool can_split = allow_split && mode == EPI_LINEAR && !ep.round_out && !ep.relu && ep.resid != nullptr &&
                          ep.partial != nullptr && ep.counters != nullptr;
   TileChoice t = choose_tile(mode, M, N, K, (int)sizeof(TOp), operand_dest, can_split);
-  if (const char* force = getenv("AVSR_B200_TILE")) {        // "BN[,SPLITS]" -- tuning / profiling aid
-    int bn = 0, sp = 1;
-    const int got = sscanf(force, "%d,%d", &bn, &sp);
+  if (const char* force = getenv("AVSR_B200_TILE")) {        // "BN[,SPLITS[,CMxCN]]" -- tuning / profiling aid
+    int bn = 0, sp = 1, cm = 1, cn = 1;
+    const int got = sscanf(force, "%d,%d,%dx%d", &bn, &sp, &cm, &cn);
     if (got >= 1 && (bn == 64 || bn == 128) && (mode != EPI_GLU || bn % 128 == 0) &&
         !(bn == 64 && sizeof(TOp) == 2 && operand_dest)) {
-      if (got < 2 || !can_split || sp < 1) sp = 1;
+      if (got < 4 || cm < 1 || cm > 2 || cn < 1 || cn > 2) cm = cn = 1;
+      if (got < 2 || !can_split || sp < 1 || cm * cn > 1) sp = 1;
       const int nkb = K / (128 / (int)sizeof(TOp));
-      t = TileChoice{bn, sp > nkb ? nkb : sp};
+      t = TileChoice{bn, sp > nkb ? nkb : sp, cm, cn};
     }
   }
   AVSR_REQUIRE(mode == EPI_VT || N % 8 == 0, "gemm_tc: N=%d must be a multiple of 8", N);

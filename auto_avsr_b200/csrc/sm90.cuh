@@ -76,6 +76,44 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, 
       : "memory");
 }
 
+// 2-D tiled load multicast to the CTAs of the cluster in `cta_mask`: the box lands at the same shared offset `dst` in
+// each of them, and its bytes are credited to the mbarrier at offset `bar` in each of them.
+__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* m, int c0, int c1, uint32_t bar,
+                                               uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;"
+      :
+      : "r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask)
+      : "memory");
+}
+
+// ---------------------------------------------------------------- clusters
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster; orders shared-memory writes (barrier init) before peers' accesses
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// arrive on the mbarrier at shared offset `bar` of cluster CTA `cta` (this CTA included)
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(bar),
+      "r"(cta)
+      : "memory");
+}
+
+// per-warpgroup register budget (all 128 threads of the warpgroup execute it)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // ---------------------------------------------------------------- wgmma
 // The accumulator of an m64nN wgmma lives in the registers of the 128 threads of a warpgroup: thread (warp w, lane l)
 // holds, for every 8-column block j, d[4j + e] = D[16w + l/4 + 8*(e/2)][8j + 2*(l%4) + e%2].
