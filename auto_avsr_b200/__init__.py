@@ -10,7 +10,7 @@ __version__ = "0.1.0"
 
 _LAZY = {"ConformerEncoder", "Encoder", "EncoderLayer", "ConvolutionModule", "RelPositionMultiHeadedAttention",
          "PositionwiseFeedForward", "LayerNorm", "RelPositionalEncoding", "CTC", "ProjEncoder", "TransformerDecoder",
-         "CTCPrefixScorer"}
+         "CTCPrefixScorer", "LabelSmoothingLoss"}
 
 
 def install():
@@ -25,8 +25,9 @@ def install_head(model):
 
 
 def install_decoder(model):
-    """Swap an already-built reference ``E2E``'s attention decoder for the CUDA scoring drop-in and make
-    ``model.scorers()`` return the CUDA CTC prefix scorer (inference / beam search only)."""
+    """Swap an already-built reference ``E2E``'s attention decoder (and ``criterion``) for the CUDA drop-ins and make
+    ``model.scorers()`` return the CUDA CTC prefix scorer: the decoder then trains (teacher-forced forward + backward,
+    LabelSmoothingLoss), validates and decodes in libavsr_b200."""
     from .install import install_decoder as _install_decoder
     return _install_decoder(model)
 

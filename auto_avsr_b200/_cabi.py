@@ -126,6 +126,15 @@ SIGNATURES = {
     "avsr_ctc_loss_state_bytes": (_Z, [_I, _I, _I]),
     "avsr_ctc_loss_fwd": (_I, [_P, C.c_long, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _Z, _P]),
     "avsr_ctc_loss_bwd": (_I, [_P, C.c_long, _P, _P, _I, _I, _I, _I, _P, _P, _Z, _P, C.c_long, _P]),
+    "avsr_mha_core_fwd": (_I, [_P, C.c_long, _P, C.c_long, _P, C.c_long, _I, _I, _I, _I, _I, _P, _P, _F, _P, _P, _P]),
+    "avsr_mha_core_bwd_workspace_bytes": (_Z, [_I, _I, _I]),
+    "avsr_mha_core_bwd": (_I, [_P, C.c_long, _P, C.c_long, _P, C.c_long, _I, _I, _I, _I, _I, _P, _P, _F, _P, _P, _P,
+                               C.c_long, _P, _P, C.c_long, _P, _Z, _P]),
+    "avsr_label_smoothing_fwd": (_I, [_P, C.c_long, _P, _I, _I, _I, _F, _P, _P, _P]),
+    "avsr_label_smoothing_bwd": (_I, [_P, C.c_long, _P, _I, _I, _I, _F, _P, _P, _P, C.c_long, _P]),
+    "avsr_embed_fwd": (_I, [_P, _P, _I, _I, _I, _I, _P, _P]),
+    "avsr_embed_bwd_workspace_bytes": (_Z, [_I, _I]),
+    "avsr_embed_bwd": (_I, [_P, _P, _I, _I, _I, _P, _P, _Z, _P]),
     "avsr_pack_padded": (_I, [_P, _P, _P, _P, _I, _I, _I, _F, _P]),
     "avsr_unpack_padded": (_I, [_P, _P, _P, _I, _I, _I, _P]),
     "avsr_head_prepared_bytes": (_Z, [_CFG, _I, _I]),

@@ -130,8 +130,15 @@ AVSR_HD float logaddexp_f(float a, float b) {
   return m + log1pf(expf(-fabsf(a - b)));
 }
 
-// embed: Embedding row * sqrt(d) + PositionalEncoding row `pos` (transformer_decoder.py:163-167, embedding.py:60-90);
-// the table entry is evaluated the way extend_pe does: fp32 exp of (2i * -(ln 1e4 / d)), fp32 product with the position
+// PositionalEncoding table entry (pos, c) (embedding.py:60-90), evaluated the way extend_pe does: fp32 exp of
+// (2i * kf), kf = -(ln 1e4 / d), fp32 product with the position.  Shared by the scoring step (EmbedElem) and the
+// teacher-forced training pass (decoder_train_body.cuh).
+AVSR_HD float pe_value(int pos, int c, float kf) {
+  const float ang = (float)pos * expf((float)(c & ~1) * kf);
+  return (c & 1) ? cosf(ang) : sinf(ang);
+}
+
+// embed: Embedding row * sqrt(d) + PositionalEncoding row `pos` (transformer_decoder.py:163-167, embedding.py:60-90)
 struct EmbedElem {
   const int32_t* tokens; const float* emb; float* x;
   int D, odim, pos;
@@ -140,9 +147,7 @@ struct EmbedElem {
     const int i = (int)(idx / D), c = (int)(idx - (long)i * D);
     int tok = tokens[i];
     tok = tok < 0 ? 0 : (tok >= odim ? odim - 1 : tok);
-    const float ang = (float)pos * expf((float)(c & ~1) * kf);
-    const float pe = (c & 1) ? cosf(ang) : sinf(ang);
-    x[idx] = emb[(long)tok * D + c] * xscale + pe;
+    x[idx] = emb[(long)tok * D + c] * xscale + pe_value(pos, c, kf);
   }
 };
 

@@ -3,6 +3,7 @@ from .attention import RelPositionMultiHeadedAttention
 from .conformer_encoder import ConformerEncoder, ConvolutionModule, EncoderLayer
 from .ctc import CTC, ProjEncoder
 from .embedding import RelPositionalEncoding
+from .label_smoothing_loss import LabelSmoothingLoss
 from .layer_norm import LayerNorm
 from .positionwise_feed_forward import PositionwiseFeedForward
 from .repeat import MultiSequential, repeat
@@ -14,4 +15,4 @@ Encoder = ConformerEncoder
 
 __all__ = ["ConformerEncoder", "Encoder", "EncoderLayer", "ConvolutionModule", "RelPositionMultiHeadedAttention",
            "PositionwiseFeedForward", "LayerNorm", "RelPositionalEncoding", "MultiSequential", "repeat", "CTC",
-           "ProjEncoder", "TransformerDecoder", "CTCPrefixScorer"]
+           "ProjEncoder", "TransformerDecoder", "CTCPrefixScorer", "LabelSmoothingLoss"]

@@ -11,7 +11,11 @@ Scorer state: the reference hands the beam search, per hypothesis, the list of e
 and re-projects K/V of the whole prefix -- and of the whole encoder memory -- at every step.  Here the K/V live in the
 library's per-utterance session (``auto_avsr_b200.decoder.DecoderEngine``); the state of a hypothesis is just the tuple
 (utterance serial, beam slot of prefix position 0, 1, ...), which the beam search's ``select_state`` (``state[i]``)
-shuffles for free.  One utterance at a time per decoder module (as the reference's CTCPrefixScorer.impl)."""
+shuffles for free.  One utterance at a time per decoder module (as the reference's CTCPrefixScorer.impl).
+
+``forward`` -- the teacher-forced pass of the training loss (transformer_decoder.py:229-258) -- runs in libavsr_b200 as
+well, forward and backward, in train and eval mode (auto_avsr_b200/decoder_train.py), on the same parameters."""
+import os
 from typing import Any, List, Optional, Tuple
 
 import torch
@@ -109,6 +113,8 @@ class TransformerDecoder(_si.BatchScorerInterface, torch.nn.Module):
         self.odim = odim
         self._cfg = (odim, attention_dim, attention_heads, linear_units, num_blocks)
         self.precision: Optional[str] = None
+        #: verify that forward's tgt_mask / memory_mask have the form passed on as lengths (one host sync each)
+        self.check_mask = os.environ.get("AVSR_B200_CHECK_MASK", "0") == "1"
         #: beam slots per position the per-utterance session is sized for (>= the beam size of the search)
         self.beam_slots = 64
         #: positions per session; None = memory length + 1 (BeamSearch.forward's maxlen with maxlenratio 0, + the <eos> step)
@@ -126,8 +132,20 @@ class TransformerDecoder(_si.BatchScorerInterface, torch.nn.Module):
 
     # ---------------------------------------------------------------- reference surface
     def forward(self, tgt, tgt_mask, memory, memory_mask):
-        raise NotImplementedError("TransformerDecoder.forward (the teacher-forced training pass, transformer_decoder.py:231-258)"
-                                  " is not on the CUDA scoring path")
+        """Teacher-forced pass (transformer_decoder.py:229-258) -> (pred_pad (B, L, odim), tgt_mask), in train and eval
+        mode, forward and backward in libavsr_b200 (auto_avsr_b200/decoder_train.py).  tgt (B, L) int64 token ids;
+        tgt_mask (B, L, L) = target_mask(tgt, ignore_id) (key prefix AND causal: passed on as key lengths + a causal
+        flag); memory (B, T, d) fp32; memory_mask (B, 1, T) prefix mask or None.  GEMMs run in ``precision`` (backward
+        GEMMs TF32 unless fp32); pred_pad is a column view of the output-layer GEMM padded to a multiple of 8 columns."""
+        if not (tgt.is_cuda and memory.is_cuda):
+            raise NotImplementedError("TransformerDecoder.forward runs on CUDA tensors only (no CPU fallback)")
+        from ..decoder_train import decoder_forward, target_lengths
+        from .attention import mask_to_lengths
+        B, L = tgt.shape
+        tgt_lengths = target_lengths(tgt_mask, B, L, self.check_mask)
+        mem_lengths = None if memory_mask is None else mask_to_lengths(memory_mask, B, memory.size(1), check=self.check_mask)
+        pred = decoder_forward(self, tgt, tgt_lengths, memory, mem_lengths, self.precision or default_precision())
+        return pred, tgt_mask
 
     def forward_one_step(self, tgt, tgt_mask, memory, memory_mask=None, cache=None):
         raise NotImplementedError("forward_one_step exposes the reference's per-layer output cache, which this path does not "

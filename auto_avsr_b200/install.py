@@ -68,16 +68,22 @@ def install_decoder(model):
     this re-homes the decoder of an existing ``E2E`` instance onto the drop-in (the very same ``Parameter`` objects) and
     re-points the two names in the already-imported E2E module, so ``model.scorers()`` -- what
     ``get_beam_search_decoder`` feeds to ``BatchBeamSearch`` (lightning.py:126-157) -- returns the CUDA scorers.
-    Inference only: the teacher-forced ``decoder.forward`` of the training loss stays with the reference module, so call
-    this on a model that is used for decoding."""
+    The drop-in also trains: ``decoder(ys_in_pad, ys_mask, x, padding_mask)``, the teacher-forced pass of the training
+    and validation steps (e2e_asr_conformer.py:79), runs forward and backward in libavsr_b200 with the old module's
+    dropout rates, and ``model.criterion`` (when the model has one) is re-homed onto the library's LabelSmoothingLoss.
+    So one ``E2E`` with install() + install_head() + install_decoder() trains, validates and decodes."""
     from .espnet_dropin import scorer_interface, scorers_ctc
     from .espnet_dropin import transformer_decoder as td
+    from .espnet_dropin.label_smoothing_loss import LabelSmoothingLoss
 
     scorer_interface.rebind()
     old = model.decoder
     emb, first = old.embed[0], old.decoders[0]
     new = td.TransformerDecoder(odim=emb.num_embeddings, attention_dim=emb.embedding_dim, attention_heads=first.self_attn.h,
-                                linear_units=first.feed_forward.w_1.out_features, num_blocks=len(old.decoders))
+                                linear_units=first.feed_forward.w_1.out_features, num_blocks=len(old.decoders),
+                                dropout_rate=first.dropout.p, positional_dropout_rate=old.embed[1].dropout.p,
+                                self_attention_dropout_rate=first.self_attn.dropout.p,
+                                src_attention_dropout_rate=first.src_attn.dropout.p)
     for name, p in old.named_parameters():
         mod = new
         *path, leaf = name.split(".")
@@ -86,6 +92,11 @@ def install_decoder(model):
         setattr(mod, leaf, p)
     new.train(old.training)
     model.decoder = new
+    oc = getattr(model, "criterion", None)
+    if oc is not None:
+        nc = LabelSmoothingLoss(oc.size, oc.padding_idx, oc.smoothing, oc.normalize_length, oc.criterion)
+        nc.train(oc.training)
+        model.criterion = nc
     e2e = sys.modules.get(E2E_MODULE)
     if e2e is not None:
         e2e.TransformerDecoder = td.TransformerDecoder

@@ -300,6 +300,43 @@ int avsr_ctc_loss_bwd(const float *logits, long ld, const int32_t *hlens, const 
                       int Lmax, int odim, const float *dnll, const void *state, size_t state_bytes, float *dlogits,
                       long ldd, void *stream);
 
+/* ---- teacher-forced training pass of the attention decoder (transformer_decoder.py:229-258) ------------------------
+ * Masked multi-head attention core (transformer/attention.py:59-88), d_k = 64, fp32:
+ *   q (B, Lq, H*64) row stride ldq, k / v (B, Lk, H*64) row strides ldk / ldv (multiples of 4, 16-byte aligned bases:
+ *   the fused self q|k|v and source k|v GEMM outputs are read in place).  Query row i of utterance b sees keys
+ *   j < min(key_lengths[b], Lk) (key_lengths NULL = all) and, when causal != 0, j <= i.  keep (B, H, Lq, Lk) uint8 or
+ *   NULL: dropout on the probabilities, kept entries scaled by keep_scale = 1 / (1 - p).
+ *   fwd: ctx (B, Lq, H*64) contiguous; probs (B, H, Lq, Lk) fp32 post-softmax, pre-dropout (0 on masked keys), or NULL
+ *        when no backward follows.  A row that sees no key gives ctx 0.
+ *   bwd: from probs, keep and dctx (B, Lq, H*64) contiguous -> dq (row stride lddq), dk and dv (row stride lddkv):
+ *        dS = P o (dP - rowsum(dP o P)) / 8.  workspace >= avsr_mha_core_bwd_workspace_bytes.
+ * Label smoothing (transformer/label_smoothing_loss.py:41-63, KLDivLoss against the smoothed target, per row):
+ *   logits (rows, ld) fp32, the first odim columns the vocabulary; target (rows) int64, ignore_id rows give 0, a target
+ *   outside [0, odim) that is not ignore_id gives NaN.  fwd -> row_loss (rows) and lse (rows, kept for the backward);
+ *   bwd -> dlogits (rows, ldd) = *dscale * (softmax - smoothed target), 0 on ignored rows and on columns [odim, ldd).
+ *   dscale is a DEVICE scalar.
+ * Embedding + positional encoding (embedding.py:60-90): x (rows, D) = embed[tokens] * sqrt(D) + pe(row mod L); a token
+ *   outside [0, odim) gives a NaN row.  bwd: dembed (odim, D) dense, positions grouped by token on the device and summed
+ *   in position order (rows of unused tokens 0).
+ * Every output element has one writer and a fixed summation order: repeated calls give identical bits. */
+int avsr_mha_core_fwd(const float *q, long ldq, const float *k, long ldk, const float *v, long ldv, int B, int H, int Lq,
+                      int Lk, int causal, const int32_t *key_lengths, const uint8_t *keep, float keep_scale, float *ctx,
+                      float *probs, void *stream);
+size_t avsr_mha_core_bwd_workspace_bytes(int B, int H, int Lq);
+int avsr_mha_core_bwd(const float *q, long ldq, const float *k, long ldk, const float *v, long ldv, int B, int H, int Lq,
+                      int Lk, int causal, const int32_t *key_lengths, const uint8_t *keep, float keep_scale,
+                      const float *probs, const float *dctx, float *dq, long lddq, float *dk, float *dv, long lddkv,
+                      void *workspace, size_t workspace_bytes, void *stream);
+int avsr_label_smoothing_fwd(const float *logits, long ld, const int64_t *target, int rows, int odim, int ignore_id,
+                             float smoothing, float *row_loss, float *lse, void *stream);
+int avsr_label_smoothing_bwd(const float *logits, long ld, const int64_t *target, int rows, int odim, int ignore_id,
+                             float smoothing, const float *lse, const float *dscale, float *dlogits, long ldd,
+                             void *stream);
+int avsr_embed_fwd(const int64_t *tokens, const float *embed, int rows, int L, int D, int odim, float *x, void *stream);
+size_t avsr_embed_bwd_workspace_bytes(int rows, int odim);
+int avsr_embed_bwd(const int64_t *tokens, const float *dx, int rows, int D, int odim, float *dembed, void *workspace,
+                   size_t workspace_bytes, void *stream);
+
 /* ---- on-device collate (SURVEY.md 8f #4) ------------------------------------------------------------------------
  * datamodule/data_module.py:10-41 (`pad` / `collate_pad`) on the GPU: the utterances of a max-frames bucket lie back to
  * back in `flat` (sum of lengths rows x d; offsets[B+1] int64 DEVICE prefix sums), the zero-padded (B, Tmax, d) batch and
