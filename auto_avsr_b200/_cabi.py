@@ -156,6 +156,12 @@ SIGNATURES = {
     "avsr_ctc_prefix_init": (_I, [_P, _I, _I, _I, _P, _P]),
     "avsr_ctc_prefix_score": (_I, [_P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P]),
     "avsr_ctc_prefix_select": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P]),
+    "avsr_decoder_batch_session_bytes": (_Z, [_DCFG, _I, _P, _I, _I]),
+    "avsr_decoder_batch_step_workspace_bytes": (_Z, [_DCFG, _I, _I, _I]),
+    "avsr_decoder_batch_begin": (_I, [_DCFG, _P, _P, _P, _I, _I, _I, _I, _P, _Z, _I, _P]),
+    "avsr_decoder_batch_step": (_I, [_DCFG, _P, _P, _Z, _P, _I, _I, _I, _I, _P, _P, _P, _I, _I, _P, _P, _Z, _I, _P]),
+    "avsr_ctc_prefix_batch_init": (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P]),
+    "avsr_ctc_prefix_batch_score": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P]),
 }
 
 if not os.path.exists(LIB_PATH):

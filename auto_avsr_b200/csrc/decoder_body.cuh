@@ -96,6 +96,47 @@ static inline DecSession layout_dec_session(const AvsrDecoderConfig& c, int T, i
   return S;
 }
 
+// U utterances decoded in lock-step: their source K/V packed frame after frame (no padding), the self-attention slots
+// as in DecSession with max_hyps = U x beam slots (hypothesis row i of any utterance takes slot i of a position)
+struct DecBatchSession {
+  float* mem_kv;       // (L, sum_T, 2d) fp32: utterance u's frames are rows [utt_off[u], utt_off[u] + utt_len[u])
+  float* self_qkv;     // (L, max_steps, max_hyps, 3d) fp32
+  float* mem_op;       // (T_max, d) operand copy of one utterance's memory (begin only)
+  int32_t* utt_off;    // (U) first packed frame of each utterance
+  int32_t* utt_len;    // (U) frames of each utterance
+  size_t bytes;
+};
+static inline DecBatchSession layout_dec_batch_session(const AvsrDecoderConfig& c, int U, long sum_T, int T_max,
+                                                       int max_steps, int max_hyps, void* base) {
+  DecBatchSession S{};
+  Carve cv{reinterpret_cast<char*>(base)};
+  const size_t D = c.d_model, L = c.num_blocks;
+  S.mem_kv = cv.take(L * (size_t)sum_T * 2 * D);
+  S.self_qkv = cv.take(L * (size_t)max_steps * max_hyps * 3 * D);
+  S.mem_op = cv.take((size_t)T_max * D);
+  S.utt_off = reinterpret_cast<int32_t*>(cv.take((size_t)U));
+  S.utt_len = reinterpret_cast<int32_t*>(cv.take((size_t)U));
+  S.bytes = cv.off;
+  return S;
+}
+
+// lengths: HOST array of U utterance lengths, each in 1..T_max (T_max <= 0: no upper bound) -> total and longest
+static inline int check_batch_lengths(const int32_t* lengths, int U, int T_max, long* sum_T, int* max_len) {
+  AVSR_REQUIRE(U >= 1, "decoder batch: U=%d utterances", U);
+  AVSR_REQUIRE(lengths != nullptr, "NULL lengths");
+  long s = 0;
+  int m = 0;
+  for (int u = 0; u < U; ++u) {
+    AVSR_REQUIRE(lengths[u] >= 1 && (T_max <= 0 || lengths[u] <= T_max),
+                 "decoder batch: utterance %d has %d frames (must be 1..T_max = %d)", u, lengths[u], T_max);
+    s += lengths[u];
+    m = lengths[u] > m ? lengths[u] : m;
+  }
+  *sum_T = s;
+  *max_len = m;
+  return AVSR_OK;
+}
+
 struct DecWork {
   float *x, *xn, *q2, *scores, *ctx, *hid, *logits;
   size_t bytes;
@@ -206,6 +247,57 @@ struct PvElem {
   }
 };
 
+// Source attention of a batched step, row i over its own utterance's frames: the per-output operations and their order
+// are ScoresElem's / PvElem's with S = utt_len[row_utt[i]] and the key rows offset by utt_off[row_utt[i]].  scores rows
+// are strided by T_max; entries past the utterance's length are neither written nor read.  The host replay runs these;
+// the device runs the grouped kernel of decoder.cu, which must give the same bits.
+struct ScoresBatchElem {
+  const float* q; const float* kv; const int32_t* row_utt; const int32_t* utt_off; const int32_t* utt_len;
+  int H, dk, D, T_max;
+  float sqrt_dk;
+  float* out;
+  AVSR_HD void operator()(long idx) const {
+    const int s = (int)(idx % T_max);
+    const long ih = idx / T_max;
+    const int h = (int)(ih % H), i = (int)(ih / H);
+    const int u = row_utt[i];
+    if (s >= utt_len[u]) return;
+    const float* qp = q + (long)i * D + h * dk;
+    const float* kp = kv + (long)(utt_off[u] + s) * 2 * D + h * dk;
+    float acc = 0.f;
+    for (int e = 0; e < dk; ++e) acc = fmaf(qp[e], kp[e], acc);
+    out[idx] = acc / sqrt_dk;
+  }
+};
+struct PvBatchElem {
+  const float* scores; const float* kv; const int32_t* row_utt; const int32_t* utt_off; const int32_t* utt_len;
+  int H, dk, D, T_max, kind;
+  void* ctx;
+  AVSR_HD void operator()(long idx) const {
+    const int i = (int)(idx / D), c = (int)(idx - (long)i * D);
+    const int h = c / dk, u = row_utt[i], S = utt_len[u];
+    const float* sc = scores + ((long)i * H + h) * T_max;
+    const float* vp = kv + (long)utt_off[u] * 2 * D + D + c;
+    float m = sc[0];
+    for (int s = 1; s < S; ++s) m = fmaxf(m, sc[s]);
+    float l = 0.f, acc = 0.f;
+    for (int s = 0; s < S; ++s) {
+      const float p = expf(sc[s] - m);
+      l += p;
+      acc = fmaf(p, vp[(long)s * 2 * D], acc);
+    }
+    store_operand(ctx, idx, kind, acc / l);
+  }
+};
+// utt_off = exclusive prefix sum of utt_len (one thread: U is the number of utterances in a batch)
+struct UttOffsetsElem {
+  const int32_t* len; int32_t* off; int U;
+  AVSR_HD void operator()(long) const {
+    int32_t acc = 0;
+    for (int u = 0; u < U; ++u) { off[u] = acc; acc += len[u]; }
+  }
+};
+
 // generic copy with conversion into an operand storage kind (weights at preparation, the memory at begin)
 struct ConvertElem {
   const float* src; void* dst; int kind;
@@ -299,6 +391,73 @@ struct CtcSelectScoreElem {
   AVSR_HD void operator()(long j) const { s_next[j] = log_psi[(long)parent[j] * O + token[j]]; }
 };
 
+// ---- CTC prefix scorer over U utterances of lengths len[u] <= T_max (CTCPrefixScoreTH with xlens,
+//      ctc_prefix_score.py:21-54, :180-181): logp (U, T_max, O); row i belongs to utterance row_utt[i].  Per row, the
+//      operations and their order are those of the one-utterance functors above with T = len[row_utt[i]]; state entries
+//      at frames t >= T are logzero (CtcSelectElem copies all T_max frames) ---------------------------------------------
+struct CtcInitBatchElem {   // r0 (T_max, 2, U)
+  const float* logp; const int32_t* len; float* r0; int U, T_max, O, blank;
+  AVSR_HD void operator()(long u) const {
+    const int T = len[u];
+    const float* lp = logp + u * (long)T_max * O;
+    float acc = 0.f;
+    for (int t = 0; t < T_max; ++t) {
+      if (t < T) acc += lp[(long)t * O + blank];
+      r0[(long)(2 * t) * U + u] = kLogZero;
+      r0[(long)(2 * t + 1) * U + u] = t < T ? acc : kLogZero;
+    }
+  }
+};
+struct CtcFillBatchElem {
+  const float* r_prev; const float* s_prev; const int32_t* row_utt; const int32_t* len; float* local; float* log_psi;
+  int O, n, blank, eos;
+  AVSR_HD void operator()(long idx) const {
+    const int i = (int)(idx / O), o = (int)(idx - (long)i * O);
+    const int T = len[row_utt[i]];
+    float v = kLogZero;
+    if (o == eos) v = logaddexp_f(r_prev[((long)(T - 1) * 2 + 0) * n + i], r_prev[((long)(T - 1) * 2 + 1) * n + i]);
+    if (o == blank) v = kLogZero;
+    log_psi[idx] = v;
+    local[idx] = v - s_prev[i];
+  }
+};
+struct CtcCandBatchElem {
+  const float* logp; const float* r_prev; const float* s_prev; const int32_t* last_ids; const int32_t* cand;
+  const int32_t* row_utt; const int32_t* len;
+  float* r; float* local; float* log_psi;
+  int T_max, O, n, S, blank, eos, out_len;
+  AVSR_HD void operator()(long idx) const {
+    const int i = (int)(idx / S), c = (int)(idx - (long)i * S);
+    const int u = row_utt[i], T = len[u];
+    const float* lp = logp + (long)u * T_max * O;
+    const int tok = cand[idx];
+    const bool same = tok == last_ids[i];
+    const int start = out_len > 1 ? out_len : 1;
+    const long plane = (long)n * S;
+    float* rp = r + (long)i * S + c;
+    for (int t = 0; t < start && t < T; ++t) { rp[(long)(2 * t) * plane] = kLogZero; rp[(long)(2 * t + 1) * plane] = kLogZero; }
+    float rn = kLogZero, rb = kLogZero;
+    if (out_len == 0) { rn = lp[tok]; rp[0] = rn; }
+    float psi = rn;
+    for (int t = start; t < T; ++t) {
+      const float pn = r_prev[((long)(t - 1) * 2 + 0) * n + i], pb = r_prev[((long)(t - 1) * 2 + 1) * n + i];
+      const float phi = same ? pb : logaddexp_f(pn, pb);
+      const float xt = lp[(long)t * O + tok], xb = lp[(long)t * O + blank];
+      const float rn_new = logaddexp_f(rn, phi) + xt;
+      const float rb_new = logaddexp_f(rn, rb) + xb;
+      psi = logaddexp_f(psi, phi + xt);
+      rp[(long)(2 * t) * plane] = rn_new;
+      rp[(long)(2 * t + 1) * plane] = rb_new;
+      rn = rn_new; rb = rb_new;
+    }
+    for (int t = T; t < T_max; ++t) { rp[(long)(2 * t) * plane] = kLogZero; rp[(long)(2 * t + 1) * plane] = kLogZero; }
+    if (tok != eos && tok != blank) {
+      log_psi[(long)i * O + tok] = psi;
+      local[(long)i * O + tok] = psi - s_prev[i];
+    }
+  }
+};
+
 // ------------------------------------------------------------------ schedules
 // Backend BK provides: gemm(prec, A_op, W_op, M, N, K, bias, out, resid, alpha, relu, out_is_operand),
 //   layernorm(x, g, b, y, rows, d, out_kind), log_softmax(x, ldx, y, ldy, rows, n), for_each(count, functor).
@@ -350,14 +509,15 @@ int prepare_body(BK& bk, const AvsrDecoderConfig& c, const AvsrDecoderLayerParam
 
 // utterance start: source-attention K | V of every layer, once (the reference recomputes them at every step inside
 // src_attn, transformer_decoder.py:119-127)
+// source K|V of one utterance's T frames into rows [row0, row0 + T) of every layer's (rows_per_layer, 2d) block
 template <class BK>
-int begin_body(BK& bk, const AvsrDecoderConfig& c, const DecPrep& P, const DecSession& S, const float* memory, int T,
-               int prec) {
+int project_memory_kv(BK& bk, const AvsrDecoderConfig& c, const DecPrep& P, const float* memory, int T, void* mem_op,
+                      float* mem_kv, long rows_per_layer, long row0, int prec) {
   const int D = c.d_model;
   const void* a = memory;
   if (prec != AVSR_PREC_FP32) {
-    AVSR_TRY(bk.for_each((long)T * D, ConvertElem{memory, S.mem_op, dec_operand_kind(prec)}));
-    a = S.mem_op;
+    AVSR_TRY(bk.for_each((long)T * D, ConvertElem{memory, mem_op, dec_operand_kind(prec)}));
+    a = mem_op;
   }
   // Row chunks of <= 192 frames: every launch stays in the M < 256 regime of the persistent one-CTA GEMM -- the same
   // kernel variant (fp32 output + bias) every step GEMM of this path uses; once per utterance, so the extra launches
@@ -369,27 +529,49 @@ int begin_body(BK& bk, const AvsrDecoderConfig& c, const DecPrep& P, const DecSe
       const int rows = T - r0 < kChunk ? T - r0 : kChunk;
       const void* a_rows = reinterpret_cast<const char*>(a) + (size_t)r0 * D * esz;
       AVSR_TRY(bk.gemm(prec, a_rows, P.L[l].src_kv_w, rows, 2 * D, D, P.L[l].src_kv_b,
-                       S.mem_kv + ((size_t)l * T + r0) * 2 * D, nullptr, 0.f, 0, 0));
+                       mem_kv + ((size_t)l * rows_per_layer + row0 + r0) * 2 * D, nullptr, 0.f, 0, 0));
     }
   return AVSR_OK;
 }
 
-// one decoding step for n hypotheses of equal length `step + 1` (their last tokens in `tokens`, their earlier
-// positions' slots in `anc` (step, n)): next-token log-probabilities (n, odim)
 template <class BK>
-int step_body(BK& bk, const AvsrDecoderConfig& c, const DecPrep& P, const DecSession& S, const DecWork& W,
-              const int32_t* tokens, const int32_t* anc, int step, int n, int T, int max_steps, int max_hyps, float* logp,
-              int prec) {
+int begin_body(BK& bk, const AvsrDecoderConfig& c, const DecPrep& P, const DecSession& S, const float* memory, int T,
+               int prec) {
+  return project_memory_kv(bk, c, P, memory, T, S.mem_op, S.mem_kv, T, 0, prec);
+}
+
+// U utterances: memory (U, T_max, d) fp32, lengths a HOST array.  Each utterance's K|V is projected with the chunks of
+// begin_body, so it has the bits a one-utterance session would hold.
+template <class BK>
+int begin_batch_body(BK& bk, const AvsrDecoderConfig& c, const DecPrep& P, const DecBatchSession& S,
+                     const float* memory, const int32_t* lengths, int U, int T_max, long sum_T, int prec) {
+  AVSR_TRY(bk.upload_i32(S.utt_len, lengths, U));
+  AVSR_TRY(bk.for_each(1, UttOffsetsElem{S.utt_len, S.utt_off, U}));
+  long off = 0;
+  for (int u = 0; u < U; ++u) {
+    AVSR_TRY(project_memory_kv(bk, c, P, memory + (size_t)u * T_max * c.d_model, lengths[u], S.mem_op, S.mem_kv, sum_T,
+                               off, prec));
+    off += lengths[u];
+  }
+  return AVSR_OK;
+}
+
+// one decoding step for n hypotheses of equal length `step + 1` (their last tokens in `tokens`, their earlier
+// positions' slots in `anc` (step, n)): next-token log-probabilities (n, odim).  `src_attn(l)` computes the source
+// attention of layer l from W.q2 into W.ctx.
+template <class BK, class SrcAttn>
+int step_layers(BK& bk, const AvsrDecoderConfig& c, const DecPrep& P, float* self_qkv, const DecWork& W,
+                const int32_t* tokens, const int32_t* anc, int step, int n, int max_steps, int max_hyps, float* logp,
+                int prec, const SrcAttn& src_attn) {
   const int D = c.d_model, H = c.n_heads, F = c.linear_units, dk = D / H;
   const int kind = dec_operand_kind(prec);
   const float sqrt_dk = (float)sqrt((double)dk);
   AVSR_TRY(bk.for_each((long)n * D, EmbedElem{tokens, P.embed, W.x, D, c.odim, step, (float)sqrt((double)D),
                                                (float)(-(log(10000.0) / D))}));
   const KvIndex self_ix{anc, n, step, max_hyps, 1};
-  const KvIndex src_ix{nullptr, n, 0, 0, 0};
   for (int l = 0; l < c.num_blocks; ++l) {
     const DecLayerPrep& q = P.L[l];
-    float* qkv_l = S.self_qkv + (size_t)l * max_steps * max_hyps * 3 * D;        // row (position, slot)
+    float* qkv_l = self_qkv + (size_t)l * max_steps * max_hyps * 3 * D;          // row (position, slot)
     float* qkv_t = qkv_l + (size_t)step * max_hyps * 3 * D;                      // this step's rows: slot = hypothesis index
     // (1) x += self_attn(norm1(x)) over the prefix
     AVSR_TRY(bk.layernorm(W.x, q.n1w, q.n1b, W.xn, n, D, kind));
@@ -401,9 +583,7 @@ int step_body(BK& bk, const AvsrDecoderConfig& c, const DecPrep& P, const DecSes
     // (2) x += src_attn(norm2(x), memory)
     AVSR_TRY(bk.layernorm(W.x, q.n2w, q.n2b, W.xn, n, D, kind));
     AVSR_TRY(bk.gemm(prec, W.xn, q.src_q_w, n, D, D, q.src_q_b, W.q2, nullptr, 0.f, 0, 0));
-    const float* mkv = S.mem_kv + (size_t)l * T * 2 * D;
-    AVSR_TRY(bk.for_each((long)n * H * T, ScoresElem{W.q2, (long)D, mkv, 2L * D, 0, src_ix, H, dk, T, sqrt_dk, W.scores}));
-    AVSR_TRY(bk.for_each((long)n * D, PvElem{W.scores, mkv, 2L * D, D, src_ix, H, dk, T, D, kind, W.ctx}));
+    AVSR_TRY(src_attn(l));
     AVSR_TRY(bk.gemm(prec, W.ctx, q.src_out_w, n, D, D, q.src_out_b, W.x, W.x, 1.f, 0, 0));
     // (3) x += w_2(relu(w_1(norm3(x))))
     AVSR_TRY(bk.layernorm(W.x, q.n3w, q.n3b, W.xn, n, D, kind));
@@ -417,12 +597,56 @@ int step_body(BK& bk, const AvsrDecoderConfig& c, const DecPrep& P, const DecSes
 }
 
 template <class BK>
+int step_body(BK& bk, const AvsrDecoderConfig& c, const DecPrep& P, const DecSession& S, const DecWork& W,
+              const int32_t* tokens, const int32_t* anc, int step, int n, int T, int max_steps, int max_hyps, float* logp,
+              int prec) {
+  const int D = c.d_model, H = c.n_heads, dk = D / H;
+  const int kind = dec_operand_kind(prec);
+  const float sqrt_dk = (float)sqrt((double)dk);
+  const KvIndex src_ix{nullptr, n, 0, 0, 0};
+  auto src_attn = [&](int l) {
+    const float* mkv = S.mem_kv + (size_t)l * T * 2 * D;
+    AVSR_TRY(bk.for_each((long)n * H * T, ScoresElem{W.q2, (long)D, mkv, 2L * D, 0, src_ix, H, dk, T, sqrt_dk, W.scores}));
+    return bk.for_each((long)n * D, PvElem{W.scores, mkv, 2L * D, D, src_ix, H, dk, T, D, kind, W.ctx});
+  };
+  return step_layers(bk, c, P, S.self_qkv, W, tokens, anc, step, n, max_steps, max_hyps, logp, prec, src_attn);
+}
+
+// one step of U utterances in lock-step: rows in any order, row i of utterance row_utt[i] (DEVICE int32, not checked);
+// everything but the source attention is step_body's code at M = n.  BK::src_attention_batch runs the source attention
+// of every row over its own utterance's frames (the batched functors on the host, the grouped kernel on the device).
+template <class BK>
+int step_batch_body(BK& bk, const AvsrDecoderConfig& c, const DecPrep& P, const DecBatchSession& S, const DecWork& W,
+                    const int32_t* tokens, const int32_t* anc, const int32_t* row_utt, int step, int n, int U, int T_max,
+                    long sum_T, int max_steps, int max_hyps, float* logp, int prec) {
+  const int D = c.d_model, H = c.n_heads, dk = D / H;
+  const int kind = dec_operand_kind(prec);
+  const float sqrt_dk = (float)sqrt((double)dk);
+  auto src_attn = [&](int l) {
+    const float* mkv = S.mem_kv + (size_t)l * sum_T * 2 * D;
+    return bk.src_attention_batch(W.q2, mkv, row_utt, S.utt_off, S.utt_len, U, sum_T, n, H, dk, T_max, sqrt_dk, W.scores,
+                                  kind, W.ctx);
+  };
+  return step_layers(bk, c, P, S.self_qkv, W, tokens, anc, step, n, max_steps, max_hyps, logp, prec, src_attn);
+}
+
+template <class BK>
 int ctc_prefix_body(BK& bk, const float* logp, int T, int O, int blank, int eos, int out_len, const int32_t* last_ids,
                     const float* r_prev, const float* s_prev, const int32_t* cand, int n, int S, float* local, float* r,
                     float* log_psi) {
   AVSR_TRY(bk.for_each((long)n * O, CtcFillElem{r_prev, s_prev, local, log_psi, T, O, n, blank, eos}));
   return bk.for_each((long)n * S, CtcCandElem{logp, r_prev, s_prev, last_ids, cand, r, local, log_psi, T, O, n, S, blank,
                                               eos, out_len});
+}
+
+template <class BK>
+int ctc_prefix_batch_body(BK& bk, const float* logp, const int32_t* len, int T_max, int O, int blank, int eos,
+                          int out_len, const int32_t* last_ids, const float* r_prev, const float* s_prev,
+                          const int32_t* cand, const int32_t* row_utt, int n, int S, float* local, float* r,
+                          float* log_psi) {
+  AVSR_TRY(bk.for_each((long)n * O, CtcFillBatchElem{r_prev, s_prev, row_utt, len, local, log_psi, O, n, blank, eos}));
+  return bk.for_each((long)n * S, CtcCandBatchElem{logp, r_prev, s_prev, last_ids, cand, row_utt, len, r, local, log_psi,
+                                                   T_max, O, n, S, blank, eos, out_len});
 }
 
 template <class BK>

@@ -414,6 +414,39 @@ int avsr_ctc_prefix_select(const float *r, const float *log_psi, const int32_t *
                            const int32_t *token, int T, int O, int n, int S, int m, float *r_next, float *s_next,
                            void *stream);
 
+/* ---- U utterances decoded in lock-step (one beam search over a batch) ----------------------------------------------
+ * A batch session holds the source K|V of U utterances packed frame after frame, (L, sum T_u, 2d), with their frame
+ * offsets and lengths, and the self-attention slots as above with max_hyps = U x beam slots.  Row i of a step belongs
+ * to utterance row_utt[i]; rows may come in any order and take beam slot i of the position being decoded.  A row's
+ * log-probabilities have the bits of the same hypothesis scored in a one-utterance session.
+ *   lengths (U) int32 HOST      frames of each utterance, 1 <= T_u <= T_max; pass the same array to begin and every step
+ *   memory (U, T_max, d) fp32   encoder output, utterance u's first T_u frames read
+ *   row_utt (n) int32 DEVICE    utterance of each row, in 0..U-1 (not checked per call)
+ * The workspace is the one-utterance step's at T = T_max. */
+size_t avsr_decoder_batch_session_bytes(const AvsrDecoderConfig *cfg, int U, const int32_t *lengths, int max_steps,
+                                        int max_hyps);
+size_t avsr_decoder_batch_step_workspace_bytes(const AvsrDecoderConfig *cfg, int T_max, int max_steps, int max_hyps);
+int avsr_decoder_batch_begin(const AvsrDecoderConfig *cfg, const void *prepared, const float *memory,
+                             const int32_t *lengths, int U, int T_max, int max_steps, int max_hyps, void *session,
+                             size_t session_bytes, int precision, void *stream);
+int avsr_decoder_batch_step(const AvsrDecoderConfig *cfg, const void *prepared, void *session, size_t session_bytes,
+                            const int32_t *lengths, int U, int T_max, int max_steps, int max_hyps, const int32_t *tokens,
+                            const int32_t *anc, const int32_t *row_utt, int step, int n, float *logp, void *workspace,
+                            size_t workspace_bytes, int precision, void *stream);
+
+/* CTCPrefixScoreTH over U utterances with xlens (ctc_prefix_score.py:21-54): logp (U, T_max, O) fp32, row_utt (n) int32
+ * DEVICE.  r0 (T_max, 2, U); r_prev (T_max, 2, n); r (T_max, 2, n, S).  A row's recursion stops at its utterance's T_u,
+ * <eos> reads frame T_u - 1, and state entries at frames >= T_u are logzero.  avsr_ctc_prefix_select carries the states
+ * over with T = T_max.
+ *   avsr_ctc_prefix_batch_init   lengths (U) int32 HOST, checked (1..T_max); writes their device copy to lengths_dev (U)
+ *   avsr_ctc_prefix_batch_score  lengths_dev = the device copy batch_init wrote for the same logp */
+int avsr_ctc_prefix_batch_init(const float *logp, const int32_t *lengths, int U, int T_max, int O, int blank,
+                               int32_t *lengths_dev, float *r0, void *stream);
+int avsr_ctc_prefix_batch_score(const float *logp, const int32_t *lengths_dev, int U, int T_max, int O, int blank, int eos,
+                                int out_len, const int32_t *last_ids, const float *r_prev, const float *s_prev,
+                                const int32_t *cand, const int32_t *row_utt, int n, int S, float *local, float *r,
+                                float *log_psi, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
