@@ -4,15 +4,20 @@
 // (transformer/attention.py:174-189 + :59-82 of the reference).  The reference materialises the (T x 2T-1) product
 // (q+v) P^T in HBM and re-lays it out with the pad/view "rel_shift" copy; here nothing of size T^2 ever leaves the SM.
 //
-// One CTA = one warpgroup = one (head h, utterance b, 64-query tile).  Per 64-key tile:
+// One CTA = one warpgroup = 64 consecutive queries of one (head h, utterance b).  Per 64-key tile:
 //   wgmma  S [64 x  64] = Qu . K_tile^T          (registers)
-//   wgmma  G [64 x 128] = Qv . Pband^T           (registers, then shared memory)
-//          Pband = the 127 table rows m = j-i+T-1 this (query tile, key tile) pair can touch -- a BAND of the rel-pos
-//          table fetched by one TMA box; score (r, c) needs G[r][c + 63 - r]: the rel_shift is a per-row skew, read
-//          from the fp32 copy of G in shared memory at the positions of this thread's S fragment.
+//   wgmma  G [64 x 128] = Qv . Pband^T           (registers)
+//          Pband = the 127 table rows m = j-i+T-1 this (query tile, key tile) pair can touch, one TMA box.  Score
+//          (r, c) needs G[r][c + 63 - r]: each thread stores only the G elements its rows use, pre-skewed, to Gsk[r][c]
+//          (rows are private to a warp's quads, so a __syncwarp orders the exchange), and reads them back at its
+//          S-fragment positions.
 //   softmax in the accumulator layout (the 4 threads of a quad share a row): scale, key mask, online max / sum
 //          (exp2), rescale of the O accumulator, P -> shared memory in the K-major SWIZZLE_128B layout
-//   wgmma  O [64 x 64] += P . V_tile             (registers)
+//   wgmma  O [64 x 64] += P . V_tile             (registers; left in flight while the next tile's S and G are issued)
+// Loads overlap the math without a producer warp: once S and G of tile j (and P.V of tile j-1) have retired, thread 0
+// issues the K tile and band of tile j+1 (`kb_full`) and the V tile of tile j (`v_full`, awaited just before P.V), so
+// the next tile's K and band arrive during this tile's softmax and P.V.  fp16 needs 74 KB of shared memory, so three
+// CTAs (warpgroups) share an SM: at S2 the 336 (h, b, query tile) CTAs fit one wave of 3 x 132.
 // TF32: V arrives as v^T (B,H,64,Tp), K-major.  fp16: V keeps its natural (B,H,T,64) layout (MN-major B operand).
 // Padded QUERY rows are computed like any other row (the reference masks keys only).
 #include "common.cuh"
@@ -26,7 +31,7 @@ constexpr int AT_BQ = 64;     // queries per CTA (= wgmma M)
 constexpr int AT_BKV = 64;    // keys per tile
 constexpr int AT_BAND = 128;  // rel-pos rows per tile (>= BQ + BKV - 1)
 constexpr int AT_THREADS = 128;
-constexpr int AT_GS = AT_BAND + 8;   // fp32 row stride of the G copy (8-byte aligned rows, skewed reads spread banks)
+constexpr int AT_GLD = 64 + 4;   // fp32 row stride of the pre-skewed G tile (spreads the quads' rows over the banks)
 
 template <typename TOp>
 struct AtCfg {
@@ -35,24 +40,26 @@ struct AtCfg {
   static constexpr int kQu = 0;
   static constexpr int kQv = kQu + AT_BQ * 128 * kAtoms;
   static constexpr int kK = kQv + AT_BQ * 128 * kAtoms;
-  static constexpr int kV = kK + AT_BKV * 128 * kAtoms;        // tf32: [64 d][64 keys]; f16: [64 keys][64 d]
-  static constexpr int kPb = kV + 64 * 128 * kAtoms;
-  static constexpr int kP = kPb + AT_BAND * 128 * kAtoms;
+  static constexpr int kPb = kK + AT_BKV * 128 * kAtoms;
+  static constexpr int kV = kPb + AT_BAND * 128 * kAtoms;      // tf32: [64 d][64 keys]; f16: [64 keys][64 d]
+  static constexpr int kP = kV + 64 * 128 * kAtoms;
   static constexpr int kG = kP + AT_BQ * 128 * kAtoms;
-  static constexpr int kBars = kG + AT_BQ * AT_GS * 4;
+  static constexpr int kBars = kG + AT_BQ * AT_GLD * 4;        // q_full, kb_full, v_full
   static constexpr int kSmem = kBars + 64 + 1024;
-  static constexpr uint32_t kTileBytes = (AT_BKV + AT_BAND + 64) * 128 * kAtoms;
+  static constexpr uint32_t kKbBytes = (AT_BKV + AT_BAND) * 128 * kAtoms;
+  static constexpr uint32_t kVBytes = 64 * 128 * kAtoms;
+  // CTAs per SM the shared memory allows (228 KB per SM, 1 KB of it reserved per CTA): fp16 3, TF32 1
+  static constexpr int kCtasPerSm = (228 * 1024) / (kSmem + 1024);
 };
 
-// MMA-K step ks of a [ROWS][64 elements] K-major tile stored as kAtoms atoms of [ROWS][128 B]
-template <typename TOp>
+// MMA-K step ks of a [rows][64 elements] K-major tile stored as kAtoms atoms of [rows][128 B]
 __device__ __forceinline__ uint64_t at_desc(uint32_t tile, int rows, int ks) {
   const int bytes = ks * 32;
   return wgmma_desc_sw128(tile + (bytes >> 7) * (rows * 128) + (bytes & 127));
 }
 
 template <typename TOp>
-__global__ void __launch_bounds__(AT_THREADS, 1)
+__global__ void __launch_bounds__(AT_THREADS, AtCfg<TOp>::kCtasPerSm)
 attention_wg_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_constant__ CUtensorMap tmQv,
                     const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                     const __grid_constant__ CUtensorMap tmP, const int32_t* __restrict__ lengths, TOp* __restrict__ ctx,
@@ -63,8 +70,8 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_const
   const uint32_t raw = smem_u32(at_smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* gen = at_smem_raw + (base - raw);
-  const uint32_t q_full = base + Cfg::kBars, kv_full = q_full + 8;
-  float* gs = reinterpret_cast<float*>(gen + Cfg::kG);
+  const uint32_t q_full = base + Cfg::kBars, kb_full = q_full + 8, v_full = q_full + 16;
+  float* gsk = reinterpret_cast<float*>(gen + Cfg::kG);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // grid = (H, B, query tiles): the query tile is the SLOWEST block index, so the partially filled last tile of every
@@ -72,17 +79,37 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_const
   const int h = blockIdx.x, b = blockIdx.y, i0 = blockIdx.z * AT_BQ;
   const int bh = b * H + h;
   pdl_launch_dependents();
+  AVSR_TSPAN_OPEN(300, (unsigned)sizeof(TOp));
   int L = T;
   if (lengths) { L = lengths[b]; L = L < 0 ? 0 : (L > T ? T : L); }   // lengths: written before the graph, not by the predecessor
   const int nkt = (L + AT_BKV - 1) / AT_BKV;
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQu); tma_prefetch_desc(&tmQv); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
     tma_prefetch_desc(&tmP);
-    mbar_init(q_full, 1); mbar_init(kv_full, 1);
+    mbar_init(q_full, 1); mbar_init(kb_full, 1); mbar_init(v_full, 1);
     fence_barrier_init();
   }
   __syncthreads();
   pdl_wait();
+  AVSR_TSPAN_DEP();
+
+  auto load_kb = [&](int j0) {     // K tile and position band of the key tile starting at j0
+    const int m_lo = j0 - i0 - (AT_BQ - 1) + T - 1;   // first table row of the band (may be < 0: zero fill)
+    mbar_expect_tx(kb_full, Cfg::kKbBytes);
+#pragma unroll
+    for (int a = 0; a < Cfg::kAtoms; ++a) {
+      tma_load_2d(base + Cfg::kK + a * AT_BKV * 128, &tmK, a * 32, bh * T + j0, kb_full);
+      tma_load_3d(base + Cfg::kPb + a * AT_BAND * 128, &tmP, a * 32, m_lo, h, kb_full);
+    }
+  };
+  auto load_v = [&](int j0) {
+    mbar_expect_tx(v_full, Cfg::kVBytes);
+    if constexpr (kF16) tma_load_2d(base + Cfg::kV, &tmV, 0, bh * T + j0, v_full);
+    else {
+#pragma unroll
+      for (int a = 0; a < Cfg::kAtoms; ++a) tma_load_2d(base + Cfg::kV + a * 64 * 128, &tmV, j0 + a * 32, bh * 64, v_full);
+    }
+  };
 
   // this thread's accumulator rows r0, r0 + 8 and first column cq of every 8-column block
   const int r0 = 16 * warp + (lane >> 2), cq = 2 * (lane & 3);
@@ -99,57 +126,62 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_const
       tma_load_2d(base + Cfg::kQu + a * AT_BQ * 128, &tmQu, a * 32, bh * T + i0, q_full);
       tma_load_2d(base + Cfg::kQv + a * AT_BQ * 128, &tmQv, a * 32, bh * T + i0, q_full);
     }
+    load_kb(0);
+    load_v(0);
   }
+  if (nkt > 0) mbar_wait(q_full, 0);
+#pragma unroll 1
   for (int it = 0; it < nkt; ++it) {
     const int j0 = it * AT_BKV;
-    if (it > 0) __syncthreads();                 // every warp's P.V(it-1) retired: K, Pband, V, P are free
-    if (threadIdx.x == 0) {
-      mbar_expect_tx(kv_full, Cfg::kTileBytes);
-      const int m_lo = j0 - i0 - (AT_BQ - 1) + T - 1;   // first table row of the band (may be < 0: zero fill)
-#pragma unroll
-      for (int a = 0; a < Cfg::kAtoms; ++a) {
-        tma_load_2d(base + Cfg::kK + a * AT_BKV * 128, &tmK, a * 32, bh * T + j0, kv_full);
-        tma_load_3d(base + Cfg::kPb + a * AT_BAND * 128, &tmP, a * 32, m_lo, h, kv_full);
-        if constexpr (kF16) tma_load_2d(base + Cfg::kV, &tmV, 0, bh * T + j0, kv_full);
-        else tma_load_2d(base + Cfg::kV + a * 64 * 128, &tmV, j0 + a * 32, bh * 64, kv_full);
-      }
-    }
-    if (it == 0) mbar_wait(q_full, 0);
-    mbar_wait(kv_full, it & 1);
-
-    float s[32], g[64];
+    mbar_wait(kb_full, it & 1);
+    float sc[32], g[64];
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < Cfg::kSteps; ++ks) {
-      const uint64_t dq = at_desc<TOp>(base + Cfg::kQu, AT_BQ, ks), dk = at_desc<TOp>(base + Cfg::kK, AT_BKV, ks);
-      const uint64_t dv = at_desc<TOp>(base + Cfg::kQv, AT_BQ, ks), dp = at_desc<TOp>(base + Cfg::kPb, AT_BAND, ks);
-      if constexpr (kF16) { wgmma_f16_n64(s, dq, dk, ks != 0); wgmma_f16_n128(g, dv, dp, ks != 0); }
-      else { wgmma_tf32_n64(s, dq, dk, ks != 0); wgmma_tf32_n128(g, dv, dp, ks != 0); }
+      const uint64_t dq = at_desc(base + Cfg::kQu, AT_BQ, ks), dk = at_desc(base + Cfg::kK, AT_BKV, ks);
+      const uint64_t dv = at_desc(base + Cfg::kQv, AT_BQ, ks), dp = at_desc(base + Cfg::kPb, AT_BAND, ks);
+      if constexpr (kF16) { wgmma_f16_n64(sc, dq, dk, ks != 0); wgmma_f16_n128(g, dv, dp, ks != 0); }
+      else { wgmma_tf32_n64(sc, dq, dk, ks != 0); wgmma_tf32_n128(g, dv, dp, ks != 0); }
     }
     wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs<32>(s);
+    wgmma_wait<0>();                             // this tile's S and G, and the previous tile's P.V
+    wgmma_fence_regs<32>(sc);
     wgmma_fence_regs<64>(g);
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      *reinterpret_cast<float2*>(gs + r0 * AT_GS + 8 * j + cq) = make_float2(g[4 * j], g[4 * j + 1]);
-      *reinterpret_cast<float2*>(gs + (r0 + 8) * AT_GS + 8 * j + cq) = make_float2(g[4 * j + 2], g[4 * j + 3]);
+    wgmma_fence_regs<32>(o);
+    __syncthreads();                             // every warp is done with K, Pband, V and P: refill them
+    if (threadIdx.x == 0) {
+      if (it + 1 < nkt) load_kb(j0 + AT_BKV);
+      if (it > 0) load_v(j0);
     }
-    __syncthreads();
-    // scores in the S fragment: s[4j + 2rr + e] is (row r0 + 8rr, key j0 + 8j + cq + e)
+    // G column cb of row r feeds score column c = cb - 63 + r: keep the 64 of 128 that land in [0, 64)
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      const int r = r0 + 8 * rr;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int c = 8 * j + cq + e - (AT_BKV - 1) + r;
+          if (c >= 0 && c < AT_BKV) gsk[r * AT_GLD + c] = g[4 * j + 2 * rr + e];
+        }
+      }
+    }
+    __syncwarp();
+    // scores in the S fragment: sc[4j + 2rr + e] is (row r0 + 8rr, key j0 + 8j + cq + e)
     float mx[2] = {m_run[0], m_run[1]};
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr) {
       const int r = r0 + 8 * rr;
-      const float* grow = gs + r * AT_GS + (AT_BQ - 1) - r;
+      const float* grow = gsk + r * AT_GLD;
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
+        const float2 gg = *reinterpret_cast<const float2*>(grow + 8 * j + cq);
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int c = 8 * j + cq + e;
-          const float v = (s[4 * j + 2 * rr + e] + grow[c]) * kScale;
-          s[4 * j + 2 * rr + e] = (j0 + c < L) ? v : -INFINITY;
-          mx[rr] = fmaxf(mx[rr], s[4 * j + 2 * rr + e]);
+          const float v = (sc[4 * j + 2 * rr + e] + (e ? gg.y : gg.x)) * kScale;
+          sc[4 * j + 2 * rr + e] = (j0 + c < L) ? v : -INFINITY;
+          mx[rr] = fmaxf(mx[rr], sc[4 * j + 2 * rr + e]);
         }
       }
       mx[rr] = fmaxf(mx[rr], __shfl_xor_sync(0xffffffffu, mx[rr], 1));
@@ -173,8 +205,8 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_const
       const int r = r0 + 8 * rr;
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        const float p0 = exp2f(s[4 * j + 2 * rr] - mx[rr]);
-        const float p1 = exp2f(s[4 * j + 2 * rr + 1] - mx[rr]);
+        const float p0 = exp2f(sc[4 * j + 2 * rr] - mx[rr]);
+        const float p1 = exp2f(sc[4 * j + 2 * rr + 1] - mx[rr]);
         l_run[rr] += p0 + p1;
         if constexpr (kF16) {
           *reinterpret_cast<uint32_t*>(gen + Cfg::kP + r * 128 + ((j ^ (r & 7)) << 4) + cq * 2) = pack_half2_sat(p0, p1);
@@ -186,18 +218,19 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_const
       }
     }
     fence_proxy_async();      // generic-proxy smem writes -> visible to the tensor core (async proxy)
-    __syncthreads();
+    __syncthreads();          // P complete; every warp's Gsk reads of this tile are done
+    mbar_wait(v_full, it & 1);
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < Cfg::kSteps; ++ks) {
-      const uint64_t dp = at_desc<TOp>(base + Cfg::kP, AT_BQ, ks);
+      const uint64_t dp = at_desc(base + Cfg::kP, AT_BQ, ks);
       if constexpr (kF16) wgmma_f16_n64_bmn(o, dp, wgmma_desc_sw128(base + Cfg::kV + ks * 16 * 128), 1);
-      else wgmma_tf32_n64(o, dp, at_desc<TOp>(base + Cfg::kV, 64, ks), 1);
+      else wgmma_tf32_n64(o, dp, at_desc(base + Cfg::kV, 64, ks), 1);
     }
     wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs<32>(o);
   }
+  wgmma_wait<0>();                               // the last P.V (unconditional: no divergent path around o)
+  wgmma_fence_regs<32>(o);
   // O / l -> ctx (B*T, H*64); rows beyond T are not stored
 #pragma unroll
   for (int rr = 0; rr < 2; ++rr) {
@@ -220,7 +253,10 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_const
       }
     }
   }
+  AVSR_TSPAN_CLOSE();
 }
+
+AVSR_TRACE_DEFINE_BIND(trace_bind_attention_tc)
 
 template <typename TOp>
 static int attention_wg(const TOp* qu, const TOp* qv, const TOp* kk, const TOp* v, const TOp* pos,

@@ -503,8 +503,9 @@ struct AvsrPlan {
 namespace avsr {
 int trace_bind_elementwise(unsigned long long*);
 int trace_bind_gemm_tc(unsigned long long*);
+int trace_bind_attention_tc(unsigned long long*);
 static int trace_bind_all(unsigned long long* p) {
-  return trace_bind_elementwise(p) | trace_bind_gemm_tc(p);
+  return trace_bind_elementwise(p) | trace_bind_gemm_tc(p) | trace_bind_attention_tc(p);
 }
 }
 // diagnostic build only (scripts/build_trace.py): device buffer of `words` 64-bit words, see common.cuh "phase trace"
