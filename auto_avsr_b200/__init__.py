@@ -10,7 +10,7 @@ __version__ = "0.1.0"
 
 _LAZY = {"ConformerEncoder", "Encoder", "EncoderLayer", "ConvolutionModule", "RelPositionMultiHeadedAttention",
          "PositionwiseFeedForward", "LayerNorm", "RelPositionalEncoding", "CTC", "ProjEncoder", "TransformerDecoder",
-         "CTCPrefixScorer", "LabelSmoothingLoss"}
+         "CTCPrefixScorer", "LabelSmoothingLoss", "Conv3dResNet", "Conv1dResNet"}
 
 
 def install():
@@ -30,6 +30,13 @@ def install_decoder(model):
     LabelSmoothingLoss), validates and decodes in libavsr_b200."""
     from .install import install_decoder as _install_decoder
     return _install_decoder(model)
+
+
+def install_frontend(model):
+    """Swap an already-built reference ``E2E``'s ResNet front-end for the CUDA drop-in (same parameters and buffers):
+    in eval the front-end then runs in libavsr_b200 from the raw clip or waveform."""
+    from .install import install_frontend as _install_frontend
+    return _install_frontend(model)
 
 
 def __getattr__(name):

@@ -81,6 +81,15 @@ class DecoderLayerParams(C.Structure):
     _fields_ = [(name, C.c_void_p) for name, _ in DECODER_LAYER_FIELDS]
 
 
+FRONTEND_VIDEO, FRONTEND_AUDIO = 0, 1
+FRONTEND_CONVS = 20
+
+
+class ConvBnParams(C.Structure):
+    _fields_ = [("conv_w", C.c_void_p), ("bn_w", C.c_void_p), ("bn_b", C.c_void_p), ("bn_mean", C.c_void_p),
+                ("bn_var", C.c_void_p), ("eps", C.c_double)]
+
+
 #: every symbol include/avsr_b200.h declares: name -> (restype, argtypes)
 _P, _I, _Z, _F = C.c_void_p, C.c_int, C.c_size_t, C.c_float
 _CFG = C.POINTER(EncoderConfig)
@@ -162,6 +171,12 @@ SIGNATURES = {
     "avsr_decoder_batch_step": (_I, [_DCFG, _P, _P, _Z, _P, _I, _I, _I, _I, _P, _P, _P, _I, _I, _P, _P, _Z, _I, _P]),
     "avsr_ctc_prefix_batch_init": (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P]),
     "avsr_ctc_prefix_batch_score": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P]),
+    "avsr_frontend_prepared_bytes": (_Z, [_I, _I]),
+    "avsr_prepare_frontend": (_I, [_I, C.POINTER(ConvBnParams), _P, _Z, _I, _P]),
+    "avsr_frontend_workspace_bytes": (_Z, [_I, _I, _I, _I, _I, _I]),
+    "avsr_frontend_forward": (_I, [_I, _P, _P, _I, _I, _I, _I, _P, _P, _Z, _I, _P]),
+    "avsr_conv_bn_act_workspace_bytes": (_Z, [_I] * 9),
+    "avsr_conv_bn_act": (_I, [_P, _P, _P, _P, _P, _I, _P] + [_I] * 8 + [_P, _Z, _I, _P]),
 }
 
 if not os.path.exists(LIB_PATH):

@@ -7,6 +7,7 @@ from .label_smoothing_loss import LabelSmoothingLoss
 from .layer_norm import LayerNorm
 from .positionwise_feed_forward import PositionwiseFeedForward
 from .repeat import MultiSequential, repeat
+from .resnet import Conv1dResNet, Conv3dResNet
 from .scorers_ctc import CTCPrefixScorer
 from .transformer_decoder import TransformerDecoder
 
@@ -15,4 +16,4 @@ Encoder = ConformerEncoder
 
 __all__ = ["ConformerEncoder", "Encoder", "EncoderLayer", "ConvolutionModule", "RelPositionMultiHeadedAttention",
            "PositionwiseFeedForward", "LayerNorm", "RelPositionalEncoding", "MultiSequential", "repeat", "CTC",
-           "ProjEncoder", "TransformerDecoder", "CTCPrefixScorer", "LabelSmoothingLoss"]
+           "ProjEncoder", "TransformerDecoder", "CTCPrefixScorer", "LabelSmoothingLoss", "Conv3dResNet", "Conv1dResNet"]

@@ -9,6 +9,8 @@ already-imported E2E modules get their ``ConformerEncoder`` symbol re-pointed).
 import sys
 import types
 
+import torch
+
 REF_ENCODER_MODULE = "espnet.nets.pytorch_backend.encoder.conformer_encoder"
 ALIAS_PACKAGE = "espnet.nets.pytorch_backend.conformer"          # north_star spelling (SURVEY.md D1)
 E2E_MODULE = "espnet.nets.pytorch_backend.e2e_asr_conformer"
@@ -101,6 +103,30 @@ def install_decoder(model):
     if e2e is not None:
         e2e.TransformerDecoder = td.TransformerDecoder
         e2e.CTCPrefixScorer = scorers_ctc.CTCPrefixScorer
+    return model
+
+
+def install_frontend(model):
+    """The ResNet front-end.  ``E2E`` builds it through ``video_resnet()`` / ``audio_resnet()`` (e2e_asr_conformer.py:26-29),
+    so this re-homes ``model.frontend`` of an existing ``E2E`` onto the drop-in ``Conv3dResNet`` / ``Conv1dResNet``: the
+    very same ``Parameter`` and buffer objects, each sub-module's train / eval mode and BatchNorm settings, and therefore
+    an unchanged ``model.state_dict()``.  In eval the front-end then runs in libavsr_b200 from the raw clip or waveform;
+    in train it stays torch autograd."""
+    from .espnet_dropin.resnet import Conv1dResNet, Conv3dResNet
+
+    old = model.frontend
+    new = Conv3dResNet() if hasattr(old, "frontend3D") else Conv1dResNet()
+    old_mods = dict(old.named_modules())
+    for name, mod in new.named_modules():
+        src = old_mods[name]
+        for leaf, p in src.named_parameters(recurse=False):
+            setattr(mod, leaf, p)
+        for leaf, b in src.named_buffers(recurse=False):
+            setattr(mod, leaf, b)
+        if isinstance(mod, torch.nn.modules.batchnorm._BatchNorm):
+            mod.eps, mod.momentum = src.eps, src.momentum
+        mod.training = src.training
+    model.frontend = new
     return model
 
 

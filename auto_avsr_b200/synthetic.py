@@ -150,6 +150,68 @@ def decoder_state_dict(seed: int = 0, odim: int = 5049, d_model: int = 768, n_he
     return sd
 
 
+def _frontend_shapes(modality: str):
+    """(key, shape) of every tensor of the reference front-end's state dict, in its order: Conv3dResNet registers
+    ``trunk`` before ``frontend3D``; Conv1dResNet's stem is ``trunk.conv1`` / ``trunk.bn1``."""
+    video = modality == "video"
+    if modality not in ("video", "audio"):
+        raise ValueError(f"modality must be 'video' or 'audio', got {modality!r}")
+    k = (3, 3) if video else (3,)
+    one = (1, 1) if video else (1,)
+    out = []
+
+    def conv_bn(conv, bn, shape):
+        out.append((conv + ".weight", shape))
+        for leaf in ("weight", "bias", "running_mean", "running_var", "num_batches_tracked"):
+            out.append((f"{bn}.{leaf}", (shape[0],) if leaf != "num_batches_tracked" else ()))
+
+    if not video:
+        conv_bn("trunk.conv1", "trunk.bn1", (64, 1, 80))
+    cin = 64
+    for i, planes in enumerate((64, 128, 256, 512)):
+        for b in range(2):
+            p = f"trunk.layer{i + 1}.{b}."
+            conv_bn(p + "conv1", p + "bn1", (planes, cin) + k)
+            conv_bn(p + "conv2", p + "bn2", (planes, planes) + k)
+            if i > 0 and b == 0:
+                conv_bn(p + "downsample.0", p + "downsample.1", (planes, cin) + one)
+            cin = planes
+    if video:
+        conv_bn("frontend3D.0", "frontend3D.1", (64, 1, 5, 7, 7))
+    return out
+
+
+def frontend_state_dict(seed: int = 0, modality: str = "video",
+                        dtype: torch.dtype = torch.float32) -> "OrderedDict[str, torch.Tensor]":
+    """Synthetic ``Conv3dResNet`` / ``Conv1dResNet`` state dict under the reference's keys: He-scaled conv weights
+    (std sqrt(2 / fan_in)), BatchNorm weight in [0.5, 1.5], bias and running_mean N(0, 0.1), running_var in [0.5, 1.5],
+    and a non-zero ``num_batches_tracked``."""
+    sd: "OrderedDict[str, torch.Tensor]" = OrderedDict()
+    for key, shape in _frontend_shapes(modality):
+        g = _gen(seed, key)
+        leaf = key.rsplit(".", 1)[1]
+        if leaf == "num_batches_tracked":
+            sd[key] = torch.tensor(1000 + len(sd), dtype=torch.long)
+        elif len(shape) > 1:
+            fan_in = math.prod(shape[1:])
+            sd[key] = (torch.randn(shape, generator=g, dtype=torch.float64) * math.sqrt(2.0 / fan_in)).to(dtype)
+        elif leaf in ("weight", "running_var"):
+            sd[key] = (torch.rand(shape, generator=g, dtype=torch.float64) + 0.5).to(dtype)
+        else:
+            sd[key] = (torch.randn(shape, generator=g, dtype=torch.float64) * 0.1).to(dtype)
+    return sd
+
+
+def frontend_input(modality: str, B: int, T: int, H: int = 88, W: int = 88, seed: int = 777,
+                   dtype: torch.dtype = torch.float32) -> torch.Tensor:
+    """Seeded N(0, 1) input of the front-end: video (B, T, 1, H, W) clips, audio (B, T, 1) waveforms of T samples.
+    Every frame / sample is drawn, so the padded tail of a shorter utterance holds non-zero data, as it may in a batch."""
+    g = torch.Generator(device="cpu")
+    g.manual_seed(seed)
+    shape = (B, T, 1, H, W) if modality == "video" else (B, T, 1)
+    return torch.randn(shape, generator=g, dtype=torch.float64).to(dtype)
+
+
 #: Canonical length sets of SURVEY.md §8 (25 Hz frames).
 SHAPES: Dict[str, Sequence[int]] = {
     "S1": [100],

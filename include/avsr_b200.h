@@ -447,6 +447,48 @@ int avsr_ctc_prefix_batch_score(const float *logp, const int32_t *lengths_dev, i
                                 const int32_t *cand, const int32_t *row_utt, int n, int S, float *local, float *r,
                                 float *log_psi, void *stream);
 
+/* ---- ResNet front-ends, inference (eval-mode BatchNorm): Conv3dResNet (frontend/resnet.py:176-233) and
+ * Conv1dResNet (frontend/resnet1d.py:204-234) with relu_type "swish".  Activations are channels-last in the precision's
+ * operand storage: (frames, H, W, C) for video, (utterances, L, C) for audio.  AVSR_PREC_TF32 and AVSR_PREC_F16 run the
+ * trunk convolutions and both stems as implicit GEMMs on wgmma; AVSR_PREC_FP32 runs a CUDA-core direct convolution
+ * (the exact reference path). */
+enum { AVSR_FRONTEND_VIDEO = 0, AVSR_FRONTEND_AUDIO = 1 };
+#define AVSR_FRONTEND_CONVS 20
+
+/* One convolution and the BatchNorm after it, as the module holds them (DEVICE fp32, contiguous): conv_w is
+ * (C_out, C_in, [KT,] [KH,] KW); the BatchNorm's weight, bias, running_mean, running_var are (C_out); eps is the module's. */
+typedef struct AvsrConvBnParams {
+  const float *conv_w;
+  const float *bn_w;
+  const float *bn_b;
+  const float *bn_mean;
+  const float *bn_var;
+  double eps;
+} AvsrConvBnParams;
+
+/* params: HOST array of AVSR_FRONTEND_CONVS entries in the reference's state-dict order (the stem, then per
+ * BasicBlock conv1, conv2 and, in the first block of layer2..4, downsample).  Weights are reordered to
+ * (C_out, taps * C_in) in operand storage; BatchNorm becomes an fp32 scale and shift.  Re-run whenever a parameter or
+ * running statistic changes. */
+size_t avsr_frontend_prepared_bytes(int modality, int precision);
+int avsr_prepare_frontend(int modality, const AvsrConvBnParams *params, void *prepared, size_t prepared_bytes,
+                          int precision, void *stream);
+/* video x: (B, T_in, 1, H, W) fp32 -> out (B, T_in, 512) fp32.
+ * audio x: (B, T_in, 1) fp32 samples (H, W ignored) -> out (B, T_in / 640, 512) fp32.
+ * Padded frames are data: the front-end takes no lengths.  Temporal taps stay inside each utterance's row. */
+size_t avsr_frontend_workspace_bytes(int modality, int B, int T_in, int H, int W, int precision);
+int avsr_frontend_forward(int modality, const void *prepared, const float *x, int B, int T_in, int H, int W,
+                          float *out, void *workspace, size_t workspace_bytes, int precision, void *stream);
+
+/* One trunk convolution + BatchNorm (as scale, shift) [+ residual] [+ SiLU] on channels-last fp32 tensors, computed in
+ * `precision` (inputs converted to operand storage in the workspace): x (N, H, W, C_in), w (C_out, C_in, KH, KW) in
+ * torch layout, resid / y (N, Ho, Wo, C_out).  Padding is (KH - 1) / 2, (KW - 1) / 2; audio convs are KH = H = 1. */
+size_t avsr_conv_bn_act_workspace_bytes(int N, int H, int W, int C_in, int C_out, int KH, int KW, int stride,
+                                        int precision);
+int avsr_conv_bn_act(const float *x, const float *w, const float *scale, const float *shift, const float *resid,
+                     int act, float *y, int N, int H, int W, int C_in, int C_out, int KH, int KW, int stride,
+                     void *workspace, size_t workspace_bytes, int precision, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
