@@ -320,10 +320,7 @@ int avsr_relpos_attention_bwd(const float* q, const float* k, const float* v, co
   AVSR_REQUIRE(q && k && v && p && pos_bias_u && pos_bias_v && ctx && dctx && dq_k && dq_p && dk && dv && dp && workspace,
                "NULL argument");
   if (B <= 0 || T <= 0) return AVSR_OK;
-  if (avsr_relpos_attention_bwd_workspace_bytes(B, T, H) > workspace_bytes) {
-    set_error("attention backward workspace too small");
-    return AVSR_E_WORKSPACE;
-  }
+  AVSR_REQUIRE_BYTES(avsr_relpos_attention_bwd_workspace_bytes(B, T, H), workspace_bytes, "attention backward workspace");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   float* lse = reinterpret_cast<float*>(workspace);
   float* delta = lse + (size_t)B * H * T;

@@ -49,12 +49,35 @@ extern std::atomic<uint64_t> g_launches;
     if (_r != AVSR_OK) return _r; \
   } while (0)
 
+// a caller-provided buffer of `have` bytes must hold `need`: else "<what> too small: need N bytes, got M"
+#define AVSR_REQUIRE_BYTES(need, have, what)                                             \
+  do {                                                                                   \
+    const size_t _need = (need), _have = (have);                                         \
+    if (_need > _have) {                                                                 \
+      ::avsr::set_error("%s too small: need %zu bytes, got %zu", what, _need, _have);    \
+      return AVSR_E_WORKSPACE;                                                           \
+    }                                                                                    \
+  } while (0)
+
 constexpr int kSplitCounters = 4096;  // split-K tile counters a caller must provide (EpiParams::counters)
 constexpr int kMaxSplits = 8;         // split-K slices gemm_tc may choose; sizes EpiParams::partial
 constexpr int kHeadDim = 64;  // d_k of the reference encoder (768 / 12); the attention kernels are built for it
 
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
+
+// Lays caller-owned buffers out back to back, each in a 256-byte-aligned slot.  With a NULL base only the size is
+// computed: take() returns NULL and `off` ends as the bytes the layout needs.
+struct Carver {
+  char* base;
+  size_t off = 0;
+  template <typename T = float>
+  T* take(size_t n) {
+    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+    off += align_up(n * sizeof(T), 256);
+    return p;
+  }
+};
 
 // ---------------------------------------------------------------- programmatic dependent launch (PDL)
 // Every hot-path kernel is launched with cudaLaunchAttributeProgrammaticStreamSerialization: it may start (block
@@ -158,6 +181,13 @@ __device__ __forceinline__ float warp_max(float v) {
 //   OP_F16  : IEEE half (same 10-bit mantissa as TF32, 5-bit exponent, saturating) -> wgmma .f16;
 //             half the bytes through L2/shared memory and twice the MMA rate of .tf32
 enum OperandKind : int { OP_F32 = 0, OP_TF32 = 1, OP_F16 = 2 };
+
+static inline bool valid_precision(int p) { return p == AVSR_PREC_FP32 || p == AVSR_PREC_TF32 || p == AVSR_PREC_F16; }
+// AVSR_PREC_* -> how the operands of that precision's contractions are stored
+static inline int operand_kind(int precision) {
+  return precision == AVSR_PREC_F16 ? OP_F16 : (precision == AVSR_PREC_TF32 ? OP_TF32 : OP_F32);
+}
+static inline size_t operand_bytes(int kind) { return kind == OP_F16 ? 2 : 4; }
 
 __device__ __forceinline__ __half to_half_sat(float x) {
   unsigned short r;

@@ -179,11 +179,7 @@ static int ctc_check(const float* logits, long ld, const int32_t* hlens, const i
   AVSR_REQUIRE(B >= 0 && Tmax >= 0 && Lmax >= 0 && Lmax <= kMaxLabels && odim >= 1 && ld >= odim,
                "ctc_loss: bad B=%d Tmax=%d Lmax=%d (<= %d) odim=%d ld=%ld", B, Tmax, Lmax, kMaxLabels, odim, ld);
   AVSR_REQUIRE(B == 0 || (hlens && state && (Lmax == 0 || ys_pad) && (Tmax == 0 || logits)), "NULL argument");
-  if (layout_ctc_state(B, Tmax, Lmax, nullptr).bytes > state_bytes) {
-    set_error("ctc_loss: state too small: need %zu bytes, got %zu", layout_ctc_state(B, Tmax, Lmax, nullptr).bytes,
-              state_bytes);
-    return AVSR_E_WORKSPACE;
-  }
+  AVSR_REQUIRE_BYTES(layout_ctc_state(B, Tmax, Lmax, nullptr).bytes, state_bytes, "ctc_loss state");
   return AVSR_OK;
 }
 

@@ -41,22 +41,16 @@ struct CtcState {
 
 static inline CtcState layout_ctc_state(int B, int Tmax, int Lmax, void* base) {
   CtcState s{};
-  char* p = reinterpret_cast<char*>(base);
-  size_t off = 0;
-  auto take = [&](size_t n, size_t esz = 4) {
-    char* r = p + off;
-    off += align_up(n * esz, 256);
-    return p ? r : nullptr;
-  };
+  Carver cv{reinterpret_cast<char*>(base)};
   const size_t BT = (size_t)B * Tmax, Smax = 2 * (size_t)Lmax + 1;
-  s.labels = reinterpret_cast<int32_t*>(take((size_t)B * (Lmax > 0 ? Lmax : 1)));
-  s.nlab = reinterpret_cast<int32_t*>(take((size_t)B));
-  s.nll = reinterpret_cast<double*>(take((size_t)B, 8));
-  s.lse = reinterpret_cast<float*>(take(BT));
-  s.lp = reinterpret_cast<float*>(take(BT * (Lmax + 1)));
-  s.alpha = reinterpret_cast<double*>(take(BT * Smax, 8));
-  s.beta = reinterpret_cast<double*>(take(BT * Smax, 8));
-  s.bytes = off;
+  s.labels = cv.take<int32_t>((size_t)B * (Lmax > 0 ? Lmax : 1));
+  s.nlab = cv.take<int32_t>((size_t)B);
+  s.nll = cv.take<double>((size_t)B);
+  s.lse = cv.take<float>(BT);
+  s.lp = cv.take<float>(BT * (Lmax + 1));
+  s.alpha = cv.take<double>(BT * Smax);
+  s.beta = cv.take<double>(BT * Smax);
+  s.bytes = cv.off;
   return s;
 }
 

@@ -181,7 +181,7 @@ struct DeviceBackend {
     e.round_out = (out_is_operand && prec != AVSR_PREC_FP32) ? 1 : 0;
     if (prec == AVSR_PREC_FP32)
       return gemm_simt(EPI_LINEAR, reinterpret_cast<const float*>(A), reinterpret_cast<const float*>(W), M, N, K, e, st);
-    return gemm_tc(EPI_LINEAR, dec_operand_kind(prec), A, W, M, N, K, e, st);
+    return gemm_tc(EPI_LINEAR, operand_kind(prec), A, W, M, N, K, e, st);
   }
   int layernorm(const float* x, const float* g, const float* b, void* y, int rows, int d, int out_kind) {
     return launch_layernorm(x, g, b, y, rows, d, out_kind, st);
@@ -218,229 +218,98 @@ struct DeviceBackend {
   }
 };
 
-static int check_dec_cfg(const AvsrDecoderConfig* c) {
-  AVSR_REQUIRE(c != nullptr, "NULL decoder config");
-  AVSR_REQUIRE(c->d_model > 0 && c->n_heads > 0 && c->d_model % c->n_heads == 0 && c->d_model % 64 == 0,
-               "decoder: d_model=%d must be a multiple of 64 and of n_heads=%d", c->d_model, c->n_heads);
-  AVSR_REQUIRE(c->linear_units > 0 && c->linear_units % 64 == 0, "decoder: linear_units=%d must be a multiple of 64",
-               c->linear_units);
-  AVSR_REQUIRE(c->num_blocks > 0 && c->num_blocks <= kMaxDecLayers, "decoder: num_blocks=%d outside 1..%d", c->num_blocks,
-               kMaxDecLayers);
-  AVSR_REQUIRE(c->odim > 1, "decoder: odim=%d", c->odim);
-  return AVSR_OK;
-}
-static inline bool dec_valid_precision(int p) { return p == AVSR_PREC_FP32 || p == AVSR_PREC_TF32 || p == AVSR_PREC_F16; }
-
 }  // namespace dec
 }  // namespace avsr
 
 using namespace avsr;
 using namespace avsr::dec;
 
+static DeviceBackend device(void* stream) { return DeviceBackend{reinterpret_cast<cudaStream_t>(stream)}; }
+
 extern "C" {
 
-size_t avsr_decoder_prepared_bytes(const AvsrDecoderConfig* cfg) {
-  if (check_dec_cfg(cfg) != AVSR_OK) return 0;
-  return layout_dec_prepared(*cfg, nullptr).bytes;
-}
+size_t avsr_decoder_prepared_bytes(const AvsrDecoderConfig* cfg) { return decoder_prepared_bytes_entry(cfg); }
 
 int avsr_prepare_decoder(const AvsrDecoderConfig* cfg, const AvsrDecoderLayerParams* layers, const float* embed_w,
                          const float* after_norm_w, const float* after_norm_b, const float* out_w, const float* out_b,
                          void* prepared, size_t prepared_bytes, int precision, void* stream) {
-  AVSR_TRY(check_dec_cfg(cfg));
-  AVSR_REQUIRE(layers && embed_w && after_norm_w && after_norm_b && out_w && out_b && prepared, "NULL argument");
-  AVSR_REQUIRE(dec_valid_precision(precision), "bad precision %d", precision);
-  for (int l = 0; l < cfg->num_blocks; ++l) {
-    const void* const* p = reinterpret_cast<const void* const*>(&layers[l]);
-    for (size_t k = 0; k < sizeof(AvsrDecoderLayerParams) / sizeof(void*); ++k)
-      AVSR_REQUIRE(p[k] != nullptr, "decoder layer %d: parameter %zu is NULL", l, k);
-  }
-  const DecPrep P = layout_dec_prepared(*cfg, prepared);
-  if (P.bytes > prepared_bytes) {
-    set_error("decoder prepared buffer too small: need %zu bytes, got %zu", P.bytes, prepared_bytes);
-    return AVSR_E_WORKSPACE;
-  }
-  DeviceBackend bk{reinterpret_cast<cudaStream_t>(stream)};
-  return prepare_body(bk, *cfg, layers, embed_w, after_norm_w, after_norm_b, out_w, out_b, P, precision);
+  return prepare_decoder_entry(device(stream), cfg, layers, embed_w, after_norm_w, after_norm_b, out_w, out_b, prepared,
+                               prepared_bytes, precision);
 }
 
 size_t avsr_decoder_session_bytes(const AvsrDecoderConfig* cfg, int T, int max_steps, int max_hyps) {
-  if (check_dec_cfg(cfg) != AVSR_OK || T <= 0 || max_steps <= 0 || max_hyps <= 0) return 0;
-  return layout_dec_session(*cfg, T, max_steps, max_hyps, nullptr).bytes;
+  return decoder_session_bytes_entry(cfg, T, max_steps, max_hyps);
 }
 
 int avsr_decoder_begin(const AvsrDecoderConfig* cfg, const void* prepared, const float* memory, int T, int max_steps,
                        int max_hyps, void* session, size_t session_bytes, int precision, void* stream) {
-  AVSR_TRY(check_dec_cfg(cfg));
-  AVSR_REQUIRE(prepared && memory && session, "NULL argument");
-  AVSR_REQUIRE(T > 0 && max_steps > 0 && max_hyps > 0, "decoder_begin: bad T=%d max_steps=%d max_hyps=%d", T, max_steps, max_hyps);
-  AVSR_REQUIRE(dec_valid_precision(precision), "bad precision %d", precision);
-  const DecSession S = layout_dec_session(*cfg, T, max_steps, max_hyps, session);
-  if (S.bytes > session_bytes) {
-    set_error("decoder session too small: need %zu bytes, got %zu", S.bytes, session_bytes);
-    return AVSR_E_WORKSPACE;
-  }
-  const DecPrep P = layout_dec_prepared(*cfg, const_cast<void*>(prepared));
-  DeviceBackend bk{reinterpret_cast<cudaStream_t>(stream)};
-  return begin_body(bk, *cfg, P, S, memory, T, precision);
+  return decoder_begin_entry(device(stream), cfg, prepared, memory, T, max_steps, max_hyps, session, session_bytes,
+                             precision);
 }
 
 size_t avsr_decoder_step_workspace_bytes(const AvsrDecoderConfig* cfg, int T, int max_steps, int max_hyps) {
-  if (check_dec_cfg(cfg) != AVSR_OK || T <= 0 || max_steps <= 0 || max_hyps <= 0) return 0;
-  return layout_dec_work(*cfg, T, max_steps, max_hyps, nullptr).bytes;
+  return decoder_step_workspace_bytes_entry(cfg, T, max_steps, max_hyps);
 }
 
 int avsr_decoder_step(const AvsrDecoderConfig* cfg, const void* prepared, void* session, size_t session_bytes, int T,
                       int max_steps, int max_hyps, const int32_t* tokens, const int32_t* anc, int step, int n, float* logp,
                       void* workspace, size_t workspace_bytes, int precision, void* stream) {
-  AVSR_TRY(check_dec_cfg(cfg));
-  AVSR_REQUIRE(prepared && session && tokens && logp && workspace, "NULL argument");
-  AVSR_REQUIRE(T > 0 && max_steps > 0 && max_hyps > 0, "decoder_step: bad T=%d max_steps=%d max_hyps=%d", T, max_steps, max_hyps);
-  AVSR_REQUIRE(step >= 0 && step < max_steps, "decoder_step: step %d outside the session's %d positions", step, max_steps);
-  AVSR_REQUIRE(n >= 0 && n <= max_hyps, "decoder_step: n=%d hypotheses exceed the session's %d beam slots", n, max_hyps);
-  AVSR_REQUIRE(step == 0 || anc != nullptr, "decoder_step: step %d needs the ancestor table", step);
-  AVSR_REQUIRE(dec_valid_precision(precision), "bad precision %d", precision);
-  if (n == 0) return AVSR_OK;
-  const DecSession S = layout_dec_session(*cfg, T, max_steps, max_hyps, session);
-  const DecWork W = layout_dec_work(*cfg, T, max_steps, max_hyps, workspace);
-  if (S.bytes > session_bytes) {
-    set_error("decoder session too small: need %zu bytes, got %zu", S.bytes, session_bytes);
-    return AVSR_E_WORKSPACE;
-  }
-  if (W.bytes > workspace_bytes) {
-    set_error("decoder step workspace too small: need %zu bytes, got %zu", W.bytes, workspace_bytes);
-    return AVSR_E_WORKSPACE;
-  }
-  const DecPrep P = layout_dec_prepared(*cfg, const_cast<void*>(prepared));
-  DeviceBackend bk{reinterpret_cast<cudaStream_t>(stream)};
-  return step_body(bk, *cfg, P, S, W, tokens, anc, step, n, T, max_steps, max_hyps, logp, precision);
+  return decoder_step_entry(device(stream), cfg, prepared, session, session_bytes, T, max_steps, max_hyps, tokens, anc,
+                            step, n, logp, workspace, workspace_bytes, precision);
 }
 
 int avsr_ctc_prefix_init(const float* logp, int T, int O, int blank, float* r0, void* stream) {
-  AVSR_REQUIRE(logp && r0, "NULL argument");
-  AVSR_REQUIRE(T > 0 && O > 1 && blank >= 0 && blank < O, "ctc_prefix_init: bad T=%d O=%d blank=%d", T, O, blank);
-  DeviceBackend bk{reinterpret_cast<cudaStream_t>(stream)};
-  return bk.for_each(1, CtcInitElem{logp, r0, T, O, blank});
+  return ctc_prefix_init_entry(device(stream), logp, T, O, blank, r0);
 }
 
 int avsr_ctc_prefix_score(const float* logp, int T, int O, int blank, int eos, int out_len, const int32_t* last_ids,
                           const float* r_prev, const float* s_prev, const int32_t* cand, int n, int S, float* local,
                           float* r, float* log_psi, void* stream) {
-  AVSR_REQUIRE(logp && last_ids && r_prev && s_prev && cand && local && r && log_psi, "NULL argument");
-  AVSR_REQUIRE(T > 0 && O > 1 && blank >= 0 && blank < O && eos >= 0 && eos < O && blank != eos,
-               "ctc_prefix_score: bad T=%d O=%d blank=%d eos=%d", T, O, blank, eos);
-  AVSR_REQUIRE(out_len >= 0 && n >= 0 && S > 0 && S <= O, "ctc_prefix_score: bad out_len=%d n=%d S=%d", out_len, n, S);
-  if (n == 0) return AVSR_OK;
-  DeviceBackend bk{reinterpret_cast<cudaStream_t>(stream)};
-  return ctc_prefix_body(bk, logp, T, O, blank, eos, out_len, last_ids, r_prev, s_prev, cand, n, S, local, r, log_psi);
+  return ctc_prefix_score_entry(device(stream), logp, T, O, blank, eos, out_len, last_ids, r_prev, s_prev, cand, n, S,
+                                local, r, log_psi);
 }
 
 size_t avsr_decoder_batch_session_bytes(const AvsrDecoderConfig* cfg, int U, const int32_t* lengths, int max_steps,
                                         int max_hyps) {
-  long sum_T;
-  int max_len;
-  if (check_dec_cfg(cfg) != AVSR_OK || check_batch_lengths(lengths, U, 0, &sum_T, &max_len) != AVSR_OK ||
-      max_steps <= 0 || max_hyps <= 0)
-    return 0;
-  return layout_dec_batch_session(*cfg, U, sum_T, max_len, max_steps, max_hyps, nullptr).bytes;
+  return decoder_batch_session_bytes_entry(cfg, U, lengths, max_steps, max_hyps);
 }
 
 size_t avsr_decoder_batch_step_workspace_bytes(const AvsrDecoderConfig* cfg, int T_max, int max_steps, int max_hyps) {
-  return avsr_decoder_step_workspace_bytes(cfg, T_max, max_steps, max_hyps);
+  return decoder_step_workspace_bytes_entry(cfg, T_max, max_steps, max_hyps);
 }
 
 int avsr_decoder_batch_begin(const AvsrDecoderConfig* cfg, const void* prepared, const float* memory,
                              const int32_t* lengths, int U, int T_max, int max_steps, int max_hyps, void* session,
                              size_t session_bytes, int precision, void* stream) {
-  AVSR_TRY(check_dec_cfg(cfg));
-  AVSR_REQUIRE(prepared && memory && session, "NULL argument");
-  AVSR_REQUIRE(T_max > 0 && max_steps > 0 && max_hyps > 0, "decoder_batch_begin: bad T_max=%d max_steps=%d max_hyps=%d",
-               T_max, max_steps, max_hyps);
-  AVSR_REQUIRE(dec_valid_precision(precision), "bad precision %d", precision);
-  long sum_T;
-  int max_len;
-  AVSR_TRY(check_batch_lengths(lengths, U, T_max, &sum_T, &max_len));
-  const DecBatchSession S = layout_dec_batch_session(*cfg, U, sum_T, max_len, max_steps, max_hyps, session);
-  if (S.bytes > session_bytes) {
-    set_error("decoder batch session too small: need %zu bytes, got %zu", S.bytes, session_bytes);
-    return AVSR_E_WORKSPACE;
-  }
-  const DecPrep P = layout_dec_prepared(*cfg, const_cast<void*>(prepared));
-  DeviceBackend bk{reinterpret_cast<cudaStream_t>(stream)};
-  return begin_batch_body(bk, *cfg, P, S, memory, lengths, U, T_max, sum_T, precision);
+  return decoder_batch_begin_entry(device(stream), cfg, prepared, memory, lengths, U, T_max, max_steps, max_hyps, session,
+                                   session_bytes, precision);
 }
 
 int avsr_decoder_batch_step(const AvsrDecoderConfig* cfg, const void* prepared, void* session, size_t session_bytes,
                             const int32_t* lengths, int U, int T_max, int max_steps, int max_hyps, const int32_t* tokens,
                             const int32_t* anc, const int32_t* row_utt, int step, int n, float* logp, void* workspace,
                             size_t workspace_bytes, int precision, void* stream) {
-  AVSR_TRY(check_dec_cfg(cfg));
-  AVSR_REQUIRE(prepared && session && tokens && row_utt && logp && workspace, "NULL argument");
-  AVSR_REQUIRE(T_max > 0 && max_steps > 0 && max_hyps > 0, "decoder_batch_step: bad T_max=%d max_steps=%d max_hyps=%d",
-               T_max, max_steps, max_hyps);
-  AVSR_REQUIRE(step >= 0 && step < max_steps, "decoder_batch_step: step %d outside the session's %d positions", step,
-               max_steps);
-  AVSR_REQUIRE(n >= 0 && n <= max_hyps, "decoder_batch_step: n=%d hypotheses exceed the session's %d beam slots", n,
-               max_hyps);
-  AVSR_REQUIRE(step == 0 || anc != nullptr, "decoder_batch_step: step %d needs the ancestor table", step);
-  AVSR_REQUIRE(dec_valid_precision(precision), "bad precision %d", precision);
-  long sum_T;
-  int max_len;
-  AVSR_TRY(check_batch_lengths(lengths, U, T_max, &sum_T, &max_len));
-  if (n == 0) return AVSR_OK;
-  const DecBatchSession S = layout_dec_batch_session(*cfg, U, sum_T, max_len, max_steps, max_hyps, session);
-  const DecWork W = layout_dec_work(*cfg, T_max, max_steps, max_hyps, workspace);
-  if (S.bytes > session_bytes) {
-    set_error("decoder batch session too small: need %zu bytes, got %zu", S.bytes, session_bytes);
-    return AVSR_E_WORKSPACE;
-  }
-  if (W.bytes > workspace_bytes) {
-    set_error("decoder batch step workspace too small: need %zu bytes, got %zu", W.bytes, workspace_bytes);
-    return AVSR_E_WORKSPACE;
-  }
-  const DecPrep P = layout_dec_prepared(*cfg, const_cast<void*>(prepared));
-  DeviceBackend bk{reinterpret_cast<cudaStream_t>(stream)};
-  return step_batch_body(bk, *cfg, P, S, W, tokens, anc, row_utt, step, n, U, T_max, sum_T, max_steps, max_hyps, logp,
-                         precision);
+  return decoder_batch_step_entry(device(stream), cfg, prepared, session, session_bytes, lengths, U, T_max, max_steps,
+                                  max_hyps, tokens, anc, row_utt, step, n, logp, workspace, workspace_bytes, precision);
 }
 
 int avsr_ctc_prefix_batch_init(const float* logp, const int32_t* lengths, int U, int T_max, int O, int blank,
                                int32_t* lengths_dev, float* r0, void* stream) {
-  AVSR_REQUIRE(logp && lengths_dev && r0, "NULL argument");
-  AVSR_REQUIRE(T_max > 0 && O > 1 && blank >= 0 && blank < O, "ctc_prefix_batch_init: bad T_max=%d O=%d blank=%d", T_max,
-               O, blank);
-  long sum_T;
-  int max_len;
-  AVSR_TRY(check_batch_lengths(lengths, U, T_max, &sum_T, &max_len));
-  DeviceBackend bk{reinterpret_cast<cudaStream_t>(stream)};
-  AVSR_TRY(bk.upload_i32(lengths_dev, lengths, U));
-  return bk.for_each(U, CtcInitBatchElem{logp, lengths_dev, r0, U, T_max, O, blank});
+  return ctc_prefix_batch_init_entry(device(stream), logp, lengths, U, T_max, O, blank, lengths_dev, r0);
 }
 
 int avsr_ctc_prefix_batch_score(const float* logp, const int32_t* lengths, int U, int T_max, int O, int blank, int eos,
                                 int out_len, const int32_t* last_ids, const float* r_prev, const float* s_prev,
                                 const int32_t* cand, const int32_t* row_utt, int n, int S, float* local, float* r,
                                 float* log_psi, void* stream) {
-  AVSR_REQUIRE(logp && lengths && last_ids && r_prev && s_prev && cand && row_utt && local && r && log_psi,
-               "NULL argument");
-  AVSR_REQUIRE(U >= 1 && T_max > 0 && O > 1 && blank >= 0 && blank < O && eos >= 0 && eos < O && blank != eos,
-               "ctc_prefix_batch_score: bad U=%d T_max=%d O=%d blank=%d eos=%d", U, T_max, O, blank, eos);
-  AVSR_REQUIRE(out_len >= 0 && n >= 0 && S > 0 && S <= O, "ctc_prefix_batch_score: bad out_len=%d n=%d S=%d", out_len, n,
-               S);
-  if (n == 0) return AVSR_OK;
-  DeviceBackend bk{reinterpret_cast<cudaStream_t>(stream)};
-  return ctc_prefix_batch_body(bk, logp, lengths, T_max, O, blank, eos, out_len, last_ids, r_prev, s_prev, cand, row_utt,
-                               n, S, local, r, log_psi);
+  return ctc_prefix_batch_score_entry(device(stream), logp, lengths, U, T_max, O, blank, eos, out_len, last_ids, r_prev,
+                                      s_prev, cand, row_utt, n, S, local, r, log_psi);
 }
 
 int avsr_ctc_prefix_select(const float* r, const float* log_psi, const int32_t* cand, const int32_t* parent,
                            const int32_t* token, int T, int O, int n, int S, int m, float* r_next, float* s_next,
                            void* stream) {
-  AVSR_REQUIRE(r && log_psi && cand && parent && token && r_next && s_next, "NULL argument");
-  AVSR_REQUIRE(T > 0 && O > 1 && n > 0 && S > 0 && m >= 0, "ctc_prefix_select: bad T=%d O=%d n=%d S=%d m=%d", T, O, n, S, m);
-  if (m == 0) return AVSR_OK;
-  DeviceBackend bk{reinterpret_cast<cudaStream_t>(stream)};
-  return ctc_select_body(bk, r, log_psi, cand, parent, token, T, O, n, S, m, r_next, s_next);
+  return ctc_prefix_select_entry(device(stream), r, log_psi, cand, parent, token, T, O, n, S, m, r_next, s_next);
 }
 
 }  // extern "C"

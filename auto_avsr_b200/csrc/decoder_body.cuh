@@ -28,20 +28,7 @@ namespace dec {
 constexpr int kMaxDecLayers = 16;
 constexpr float kLogZero = -10000000000.0f;   // ctc_prefix_score.py:31
 
-static inline int dec_operand_kind(int precision) {
-  return precision == AVSR_PREC_F16 ? OP_F16 : (precision == AVSR_PREC_TF32 ? OP_TF32 : OP_F32);
-}
-
 // ------------------------------------------------------------------ layouts (all slots 256-byte aligned, 4 B / element)
-struct Carve {
-  char* base;
-  size_t off = 0;
-  float* take(size_t n) {
-    float* p = reinterpret_cast<float*>(base + off);
-    off += align_up(n * sizeof(float), 256);
-    return base ? p : nullptr;
-  }
-};
 
 struct DecLayerPrep {
   float *self_qkv_w, *self_qkv_b, *self_out_w, *self_out_b;   // q|k|v rows concatenated: (3d, d)
@@ -57,7 +44,7 @@ struct DecPrep {
 };
 static inline DecPrep layout_dec_prepared(const AvsrDecoderConfig& c, void* base) {
   DecPrep P{};
-  Carve cv{reinterpret_cast<char*>(base)};
+  Carver cv{reinterpret_cast<char*>(base)};
   const size_t D = c.d_model, F = c.linear_units;
   for (int l = 0; l < c.num_blocks && l < kMaxDecLayers; ++l) {
     DecLayerPrep& q = P.L[l];
@@ -87,7 +74,7 @@ struct DecSession {
 };
 static inline DecSession layout_dec_session(const AvsrDecoderConfig& c, int T, int max_steps, int max_hyps, void* base) {
   DecSession S{};
-  Carve cv{reinterpret_cast<char*>(base)};
+  Carver cv{reinterpret_cast<char*>(base)};
   const size_t D = c.d_model, L = c.num_blocks;
   S.mem_kv = cv.take(L * (size_t)T * 2 * D);
   S.self_qkv = cv.take(L * (size_t)max_steps * max_hyps * 3 * D);
@@ -109,7 +96,7 @@ struct DecBatchSession {
 static inline DecBatchSession layout_dec_batch_session(const AvsrDecoderConfig& c, int U, long sum_T, int T_max,
                                                        int max_steps, int max_hyps, void* base) {
   DecBatchSession S{};
-  Carve cv{reinterpret_cast<char*>(base)};
+  Carver cv{reinterpret_cast<char*>(base)};
   const size_t D = c.d_model, L = c.num_blocks;
   S.mem_kv = cv.take(L * (size_t)sum_T * 2 * D);
   S.self_qkv = cv.take(L * (size_t)max_steps * max_hyps * 3 * D);
@@ -143,7 +130,7 @@ struct DecWork {
 };
 static inline DecWork layout_dec_work(const AvsrDecoderConfig& c, int T, int max_steps, int max_hyps, void* base) {
   DecWork W{};
-  Carve cv{reinterpret_cast<char*>(base)};
+  Carver cv{reinterpret_cast<char*>(base)};
   const size_t D = c.d_model, n = max_hyps;
   const size_t smax = (size_t)(T > max_steps ? T : max_steps);
   W.x = cv.take(n * D); W.xn = cv.take(n * D); W.q2 = cv.take(n * D);
@@ -466,7 +453,7 @@ int prepare_body(BK& bk, const AvsrDecoderConfig& c, const AvsrDecoderLayerParam
                  const float* after_w, const float* after_b, const float* out_w, const float* out_b, const DecPrep& P,
                  int prec) {
   const long D = c.d_model, F = c.linear_units;
-  const int kind = dec_operand_kind(prec);
+  const int kind = operand_kind(prec);
   for (int l = 0; l < c.num_blocks; ++l) {
     const AvsrDecoderLayerParams& s = layers[l];
     const DecLayerPrep& q = P.L[l];
@@ -516,7 +503,7 @@ int project_memory_kv(BK& bk, const AvsrDecoderConfig& c, const DecPrep& P, cons
   const int D = c.d_model;
   const void* a = memory;
   if (prec != AVSR_PREC_FP32) {
-    AVSR_TRY(bk.for_each((long)T * D, ConvertElem{memory, mem_op, dec_operand_kind(prec)}));
+    AVSR_TRY(bk.for_each((long)T * D, ConvertElem{memory, mem_op, operand_kind(prec)}));
     a = mem_op;
   }
   // Row chunks of <= 192 frames: every launch stays in the M < 256 regime of the persistent one-CTA GEMM -- the same
@@ -564,7 +551,7 @@ int step_layers(BK& bk, const AvsrDecoderConfig& c, const DecPrep& P, float* sel
                 const int32_t* tokens, const int32_t* anc, int step, int n, int max_steps, int max_hyps, float* logp,
                 int prec, const SrcAttn& src_attn) {
   const int D = c.d_model, H = c.n_heads, F = c.linear_units, dk = D / H;
-  const int kind = dec_operand_kind(prec);
+  const int kind = operand_kind(prec);
   const float sqrt_dk = (float)sqrt((double)dk);
   AVSR_TRY(bk.for_each((long)n * D, EmbedElem{tokens, P.embed, W.x, D, c.odim, step, (float)sqrt((double)D),
                                                (float)(-(log(10000.0) / D))}));
@@ -601,7 +588,7 @@ int step_body(BK& bk, const AvsrDecoderConfig& c, const DecPrep& P, const DecSes
               const int32_t* tokens, const int32_t* anc, int step, int n, int T, int max_steps, int max_hyps, float* logp,
               int prec) {
   const int D = c.d_model, H = c.n_heads, dk = D / H;
-  const int kind = dec_operand_kind(prec);
+  const int kind = operand_kind(prec);
   const float sqrt_dk = (float)sqrt((double)dk);
   const KvIndex src_ix{nullptr, n, 0, 0, 0};
   auto src_attn = [&](int l) {
@@ -620,7 +607,7 @@ int step_batch_body(BK& bk, const AvsrDecoderConfig& c, const DecPrep& P, const 
                     const int32_t* tokens, const int32_t* anc, const int32_t* row_utt, int step, int n, int U, int T_max,
                     long sum_T, int max_steps, int max_hyps, float* logp, int prec) {
   const int D = c.d_model, H = c.n_heads, dk = D / H;
-  const int kind = dec_operand_kind(prec);
+  const int kind = operand_kind(prec);
   const float sqrt_dk = (float)sqrt((double)dk);
   auto src_attn = [&](int l) {
     const float* mkv = S.mem_kv + (size_t)l * sum_T * 2 * D;
@@ -654,6 +641,200 @@ int ctc_select_body(BK& bk, const float* r, const float* log_psi, const int32_t*
                     const int32_t* token, int T, int O, int n, int S, int m, float* r_next, float* s_next) {
   AVSR_TRY(bk.for_each((long)T * 2 * m, CtcSelectElem{r, cand, parent, token, r_next, n, S, m}));
   return bk.for_each((long)m, CtcSelectScoreElem{log_psi, parent, token, s_next, O});
+}
+
+// ------------------------------------------------------------------ C-ABI entry bodies (include/avsr_b200.h)
+// The argument contract of every decoder / CTC-prefix entry, written once: decoder.cu forwards the extern "C" names to
+// these with its DeviceBackend, the host replay with its host backend.  What only one backend refuses stays in it.
+static inline int check_dec_cfg(const AvsrDecoderConfig* c) {
+  AVSR_REQUIRE(c != nullptr, "NULL decoder config");
+  AVSR_REQUIRE(c->d_model > 0 && c->n_heads > 0 && c->d_model % c->n_heads == 0 && c->d_model % 64 == 0,
+               "decoder: d_model=%d must be a multiple of 64 and of n_heads=%d", c->d_model, c->n_heads);
+  AVSR_REQUIRE(c->linear_units > 0 && c->linear_units % 64 == 0, "decoder: linear_units=%d must be a multiple of 64",
+               c->linear_units);
+  AVSR_REQUIRE(c->num_blocks > 0 && c->num_blocks <= kMaxDecLayers, "decoder: num_blocks=%d outside 1..%d", c->num_blocks,
+               kMaxDecLayers);
+  AVSR_REQUIRE(c->odim > 1, "decoder: odim=%d", c->odim);
+  return AVSR_OK;
+}
+
+static inline size_t decoder_prepared_bytes_entry(const AvsrDecoderConfig* cfg) {
+  if (check_dec_cfg(cfg) != AVSR_OK) return 0;
+  return layout_dec_prepared(*cfg, nullptr).bytes;
+}
+
+template <class BK>
+int prepare_decoder_entry(BK bk, const AvsrDecoderConfig* cfg, const AvsrDecoderLayerParams* layers,
+                          const float* embed_w, const float* after_norm_w, const float* after_norm_b, const float* out_w,
+                          const float* out_b, void* prepared, size_t prepared_bytes, int precision) {
+  AVSR_TRY(check_dec_cfg(cfg));
+  AVSR_REQUIRE(layers && embed_w && after_norm_w && after_norm_b && out_w && out_b && prepared, "NULL argument");
+  AVSR_REQUIRE(valid_precision(precision), "bad precision %d", precision);
+  for (int l = 0; l < cfg->num_blocks; ++l) {
+    const void* const* p = reinterpret_cast<const void* const*>(&layers[l]);
+    for (size_t k = 0; k < sizeof(AvsrDecoderLayerParams) / sizeof(void*); ++k)
+      AVSR_REQUIRE(p[k] != nullptr, "decoder layer %d: parameter %zu is NULL", l, k);
+  }
+  const DecPrep P = layout_dec_prepared(*cfg, prepared);
+  AVSR_REQUIRE_BYTES(P.bytes, prepared_bytes, "decoder prepared buffer");
+  return prepare_body(bk, *cfg, layers, embed_w, after_norm_w, after_norm_b, out_w, out_b, P, precision);
+}
+
+static inline size_t decoder_session_bytes_entry(const AvsrDecoderConfig* cfg, int T, int max_steps, int max_hyps) {
+  if (check_dec_cfg(cfg) != AVSR_OK || T <= 0 || max_steps <= 0 || max_hyps <= 0) return 0;
+  return layout_dec_session(*cfg, T, max_steps, max_hyps, nullptr).bytes;
+}
+
+template <class BK>
+int decoder_begin_entry(BK bk, const AvsrDecoderConfig* cfg, const void* prepared, const float* memory, int T,
+                        int max_steps, int max_hyps, void* session, size_t session_bytes, int precision) {
+  AVSR_TRY(check_dec_cfg(cfg));
+  AVSR_REQUIRE(prepared && memory && session, "NULL argument");
+  AVSR_REQUIRE(T > 0 && max_steps > 0 && max_hyps > 0, "decoder_begin: bad T=%d max_steps=%d max_hyps=%d", T, max_steps, max_hyps);
+  AVSR_REQUIRE(valid_precision(precision), "bad precision %d", precision);
+  const DecSession S = layout_dec_session(*cfg, T, max_steps, max_hyps, session);
+  AVSR_REQUIRE_BYTES(S.bytes, session_bytes, "decoder session");
+  const DecPrep P = layout_dec_prepared(*cfg, const_cast<void*>(prepared));
+  return begin_body(bk, *cfg, P, S, memory, T, precision);
+}
+
+static inline size_t decoder_step_workspace_bytes_entry(const AvsrDecoderConfig* cfg, int T, int max_steps,
+                                                        int max_hyps) {
+  if (check_dec_cfg(cfg) != AVSR_OK || T <= 0 || max_steps <= 0 || max_hyps <= 0) return 0;
+  return layout_dec_work(*cfg, T, max_steps, max_hyps, nullptr).bytes;
+}
+
+template <class BK>
+int decoder_step_entry(BK bk, const AvsrDecoderConfig* cfg, const void* prepared, void* session, size_t session_bytes,
+                       int T, int max_steps, int max_hyps, const int32_t* tokens, const int32_t* anc, int step, int n,
+                       float* logp, void* workspace, size_t workspace_bytes, int precision) {
+  AVSR_TRY(check_dec_cfg(cfg));
+  AVSR_REQUIRE(prepared && session && tokens && logp && workspace, "NULL argument");
+  AVSR_REQUIRE(T > 0 && max_steps > 0 && max_hyps > 0, "decoder_step: bad T=%d max_steps=%d max_hyps=%d", T, max_steps, max_hyps);
+  AVSR_REQUIRE(step >= 0 && step < max_steps, "decoder_step: step %d outside the session's %d positions", step, max_steps);
+  AVSR_REQUIRE(n >= 0 && n <= max_hyps, "decoder_step: n=%d hypotheses exceed the session's %d beam slots", n, max_hyps);
+  AVSR_REQUIRE(step == 0 || anc != nullptr, "decoder_step: step %d needs the ancestor table", step);
+  AVSR_REQUIRE(valid_precision(precision), "bad precision %d", precision);
+  if (n == 0) return AVSR_OK;
+  const DecSession S = layout_dec_session(*cfg, T, max_steps, max_hyps, session);
+  const DecWork W = layout_dec_work(*cfg, T, max_steps, max_hyps, workspace);
+  AVSR_REQUIRE_BYTES(S.bytes, session_bytes, "decoder session");
+  AVSR_REQUIRE_BYTES(W.bytes, workspace_bytes, "decoder step workspace");
+  const DecPrep P = layout_dec_prepared(*cfg, const_cast<void*>(prepared));
+  return step_body(bk, *cfg, P, S, W, tokens, anc, step, n, T, max_steps, max_hyps, logp, precision);
+}
+
+template <class BK>
+int ctc_prefix_init_entry(BK bk, const float* logp, int T, int O, int blank, float* r0) {
+  AVSR_REQUIRE(logp && r0, "NULL argument");
+  AVSR_REQUIRE(T > 0 && O > 1 && blank >= 0 && blank < O, "ctc_prefix_init: bad T=%d O=%d blank=%d", T, O, blank);
+  return bk.for_each(1, CtcInitElem{logp, r0, T, O, blank});
+}
+
+template <class BK>
+int ctc_prefix_score_entry(BK bk, const float* logp, int T, int O, int blank, int eos, int out_len,
+                           const int32_t* last_ids, const float* r_prev, const float* s_prev, const int32_t* cand, int n,
+                           int S, float* local, float* r, float* log_psi) {
+  AVSR_REQUIRE(logp && last_ids && r_prev && s_prev && cand && local && r && log_psi, "NULL argument");
+  AVSR_REQUIRE(T > 0 && O > 1 && blank >= 0 && blank < O && eos >= 0 && eos < O && blank != eos,
+               "ctc_prefix_score: bad T=%d O=%d blank=%d eos=%d", T, O, blank, eos);
+  AVSR_REQUIRE(out_len >= 0 && n >= 0 && S > 0 && S <= O, "ctc_prefix_score: bad out_len=%d n=%d S=%d", out_len, n, S);
+  if (n == 0) return AVSR_OK;
+  return ctc_prefix_body(bk, logp, T, O, blank, eos, out_len, last_ids, r_prev, s_prev, cand, n, S, local, r, log_psi);
+}
+
+template <class BK>
+int ctc_prefix_select_entry(BK bk, const float* r, const float* log_psi, const int32_t* cand, const int32_t* parent,
+                            const int32_t* token, int T, int O, int n, int S, int m, float* r_next, float* s_next) {
+  AVSR_REQUIRE(r && log_psi && cand && parent && token && r_next && s_next, "NULL argument");
+  AVSR_REQUIRE(T > 0 && O > 1 && n > 0 && S > 0 && m >= 0, "ctc_prefix_select: bad T=%d O=%d n=%d S=%d m=%d", T, O, n, S, m);
+  if (m == 0) return AVSR_OK;
+  return ctc_select_body(bk, r, log_psi, cand, parent, token, T, O, n, S, m, r_next, s_next);
+}
+
+static inline size_t decoder_batch_session_bytes_entry(const AvsrDecoderConfig* cfg, int U, const int32_t* lengths,
+                                                       int max_steps, int max_hyps) {
+  long sum_T;
+  int max_len;
+  if (check_dec_cfg(cfg) != AVSR_OK || check_batch_lengths(lengths, U, 0, &sum_T, &max_len) != AVSR_OK ||
+      max_steps <= 0 || max_hyps <= 0)
+    return 0;
+  return layout_dec_batch_session(*cfg, U, sum_T, max_len, max_steps, max_hyps, nullptr).bytes;
+}
+
+template <class BK>
+int decoder_batch_begin_entry(BK bk, const AvsrDecoderConfig* cfg, const void* prepared, const float* memory,
+                              const int32_t* lengths, int U, int T_max, int max_steps, int max_hyps, void* session,
+                              size_t session_bytes, int precision) {
+  AVSR_TRY(check_dec_cfg(cfg));
+  AVSR_REQUIRE(prepared && memory && session, "NULL argument");
+  AVSR_REQUIRE(T_max > 0 && max_steps > 0 && max_hyps > 0, "decoder_batch_begin: bad T_max=%d max_steps=%d max_hyps=%d",
+               T_max, max_steps, max_hyps);
+  AVSR_REQUIRE(valid_precision(precision), "bad precision %d", precision);
+  long sum_T;
+  int max_len;
+  AVSR_TRY(check_batch_lengths(lengths, U, T_max, &sum_T, &max_len));
+  const DecBatchSession S = layout_dec_batch_session(*cfg, U, sum_T, max_len, max_steps, max_hyps, session);
+  AVSR_REQUIRE_BYTES(S.bytes, session_bytes, "decoder batch session");
+  const DecPrep P = layout_dec_prepared(*cfg, const_cast<void*>(prepared));
+  return begin_batch_body(bk, *cfg, P, S, memory, lengths, U, T_max, sum_T, precision);
+}
+
+template <class BK>
+int decoder_batch_step_entry(BK bk, const AvsrDecoderConfig* cfg, const void* prepared, void* session,
+                             size_t session_bytes, const int32_t* lengths, int U, int T_max, int max_steps, int max_hyps,
+                             const int32_t* tokens, const int32_t* anc, const int32_t* row_utt, int step, int n,
+                             float* logp, void* workspace, size_t workspace_bytes, int precision) {
+  AVSR_TRY(check_dec_cfg(cfg));
+  AVSR_REQUIRE(prepared && session && tokens && row_utt && logp && workspace, "NULL argument");
+  AVSR_REQUIRE(T_max > 0 && max_steps > 0 && max_hyps > 0, "decoder_batch_step: bad T_max=%d max_steps=%d max_hyps=%d",
+               T_max, max_steps, max_hyps);
+  AVSR_REQUIRE(step >= 0 && step < max_steps, "decoder_batch_step: step %d outside the session's %d positions", step,
+               max_steps);
+  AVSR_REQUIRE(n >= 0 && n <= max_hyps, "decoder_batch_step: n=%d hypotheses exceed the session's %d beam slots", n,
+               max_hyps);
+  AVSR_REQUIRE(step == 0 || anc != nullptr, "decoder_batch_step: step %d needs the ancestor table", step);
+  AVSR_REQUIRE(valid_precision(precision), "bad precision %d", precision);
+  long sum_T;
+  int max_len;
+  AVSR_TRY(check_batch_lengths(lengths, U, T_max, &sum_T, &max_len));
+  if (n == 0) return AVSR_OK;
+  const DecBatchSession S = layout_dec_batch_session(*cfg, U, sum_T, max_len, max_steps, max_hyps, session);
+  const DecWork W = layout_dec_work(*cfg, T_max, max_steps, max_hyps, workspace);
+  AVSR_REQUIRE_BYTES(S.bytes, session_bytes, "decoder batch session");
+  AVSR_REQUIRE_BYTES(W.bytes, workspace_bytes, "decoder batch step workspace");
+  const DecPrep P = layout_dec_prepared(*cfg, const_cast<void*>(prepared));
+  return step_batch_body(bk, *cfg, P, S, W, tokens, anc, row_utt, step, n, U, T_max, sum_T, max_steps, max_hyps, logp,
+                         precision);
+}
+
+template <class BK>
+int ctc_prefix_batch_init_entry(BK bk, const float* logp, const int32_t* lengths, int U, int T_max, int O, int blank,
+                                int32_t* lengths_dev, float* r0) {
+  AVSR_REQUIRE(logp && lengths_dev && r0, "NULL argument");
+  AVSR_REQUIRE(T_max > 0 && O > 1 && blank >= 0 && blank < O, "ctc_prefix_batch_init: bad T_max=%d O=%d blank=%d", T_max,
+               O, blank);
+  long sum_T;
+  int max_len;
+  AVSR_TRY(check_batch_lengths(lengths, U, T_max, &sum_T, &max_len));
+  AVSR_TRY(bk.upload_i32(lengths_dev, lengths, U));
+  return bk.for_each(U, CtcInitBatchElem{logp, lengths_dev, r0, U, T_max, O, blank});
+}
+
+template <class BK>
+int ctc_prefix_batch_score_entry(BK bk, const float* logp, const int32_t* lengths, int U, int T_max, int O, int blank,
+                                 int eos, int out_len, const int32_t* last_ids, const float* r_prev, const float* s_prev,
+                                 const int32_t* cand, const int32_t* row_utt, int n, int S, float* local, float* r,
+                                 float* log_psi) {
+  AVSR_REQUIRE(logp && lengths && last_ids && r_prev && s_prev && cand && row_utt && local && r && log_psi,
+               "NULL argument");
+  AVSR_REQUIRE(U >= 1 && T_max > 0 && O > 1 && blank >= 0 && blank < O && eos >= 0 && eos < O && blank != eos,
+               "ctc_prefix_batch_score: bad U=%d T_max=%d O=%d blank=%d eos=%d", U, T_max, O, blank, eos);
+  AVSR_REQUIRE(out_len >= 0 && n >= 0 && S > 0 && S <= O, "ctc_prefix_batch_score: bad out_len=%d n=%d S=%d", out_len, n,
+               S);
+  if (n == 0) return AVSR_OK;
+  return ctc_prefix_batch_body(bk, logp, lengths, T_max, O, blank, eos, out_len, last_ids, r_prev, s_prev, cand, row_utt,
+                               n, S, local, r, log_psi);
 }
 
 }  // namespace dec

@@ -357,10 +357,7 @@ int avsr_mha_core_bwd(const float* q, long ldq, const float* k, long ldk, const 
   const long rows = (long)B * H * Lq, keys = (long)B * H * Lk;
   if (rows > 0) {
     AVSR_REQUIRE(dq && (Lk == 0 || (probs && dctx && aligned16(dctx))) && workspace, "NULL argument");
-    if (avsr_mha_core_bwd_workspace_bytes(B, H, Lq) > workspace_bytes) {
-      set_error("mha_core_bwd: workspace too small");
-      return AVSR_E_WORKSPACE;
-    }
+    AVSR_REQUIRE_BYTES(avsr_mha_core_bwd_workspace_bytes(B, H, Lq), workspace_bytes, "mha_core_bwd workspace");
     AVSR_LAUNCH(mha_bwd_rows_kernel, (unsigned)((rows + kMhaWarps - 1) / kMhaWarps), 32 * kMhaWarps, 0, st, k, ldk, v,
                 ldv, B, H, Lq, Lk, causal, key_lengths, keep, keep_scale, probs, dctx, dq, lddq,
                 reinterpret_cast<float*>(workspace));
@@ -419,10 +416,7 @@ int avsr_embed_bwd(const int64_t* tokens, const float* dx, int rows, int D, int 
                    size_t workspace_bytes, void* stream) {
   AVSR_REQUIRE(rows >= 0 && D >= 1 && odim >= 1, "embed_bwd: bad rows=%d D=%d odim=%d", rows, D, odim);
   AVSR_REQUIRE(dembed && workspace && (rows == 0 || (tokens && dx)), "NULL argument");
-  if (avsr_embed_bwd_workspace_bytes(rows, odim) > workspace_bytes) {
-    set_error("embed_bwd: workspace too small");
-    return AVSR_E_WORKSPACE;
-  }
+  AVSR_REQUIRE_BYTES(avsr_embed_bwd_workspace_bytes(rows, odim), workspace_bytes, "embed_bwd workspace");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   int32_t* start = reinterpret_cast<int32_t*>(workspace);
   int32_t* order = reinterpret_cast<int32_t*>(reinterpret_cast<char*>(workspace) + align_up((size_t)(odim + 1) * 4, 256));

@@ -4,6 +4,7 @@
 #include <stdarg.h>
 #include <string.h>
 
+#include <memory>
 #include <vector>
 
 #include "common.cuh"
@@ -35,16 +36,6 @@ struct Prepared {
   std::vector<LayerPrep> layers;
   float *pos_w_all, *after_w, *after_b;
   size_t bytes;
-};
-
-struct Carver {
-  char* base;
-  size_t off = 0;
-  float* take(size_t nfloats) {
-    float* p = reinterpret_cast<float*>(base + off);
-    off += align_up(nfloats * sizeof(float), 256);
-    return p;
-  }
 };
 
 static Prepared layout_prepared(const AvsrEncoderConfig& c, void* base) {
@@ -131,18 +122,9 @@ static int copy_round(const float* src, void* dst, long n, int kind, cudaStream_
   return AVSR_OK;
 }
 
-// ------------------------------------------------------------------ precision -> operand storage
-static inline bool valid_precision(int p) { return p == AVSR_PREC_FP32 || p == AVSR_PREC_TF32 || p == AVSR_PREC_F16; }
-static inline int operand_kind(int precision) {
-  return precision == AVSR_PREC_F16 ? OP_F16 : (precision == AVSR_PREC_TF32 ? OP_TF32 : OP_F32);
-}
-static inline size_t operand_size(int precision) { return precision == AVSR_PREC_F16 ? 2 : 4; }
-// element offset into an operand-typed buffer carved as floats
+// ------------------------------------------------------------------ element offset into an operand-typed buffer carved as floats
 static inline void* op_offset(void* base, size_t elems, int precision) {
-  return reinterpret_cast<char*>(base) + elems * operand_size(precision);
-}
-static inline const void* op_offset(const void* base, size_t elems, int precision) {
-  return reinterpret_cast<const char*>(base) + elems * operand_size(precision);
+  return reinterpret_cast<char*>(base) + elems * operand_bytes(operand_kind(precision));
 }
 
 // ------------------------------------------------------------------ workspace
@@ -389,10 +371,7 @@ static int forward_impl(const AvsrEncoderConfig* cfg, const void* prepared, cons
   AVSR_REQUIRE(prepared && xs && out && workspace, "NULL buffer");
   AVSR_REQUIRE((long)B * T < (1L << 24), "B*T=%ld too large", (long)B * T);
   Workspace W = layout_workspace(*cfg, B, T, workspace);
-  if (W.bytes > workspace_bytes) {
-    set_error("workspace too small: need %zu bytes, got %zu", W.bytes, workspace_bytes);
-    return AVSR_E_WORKSPACE;
-  }
+  AVSR_REQUIRE_BYTES(W.bytes, workspace_bytes, "workspace");
   Prepared P = layout_prepared(*cfg, const_cast<void*>(prepared));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   AVSR_TRY(launch_embed_scale(xs, W.x, (long)B * T * cfg->d_model, sqrtf((float)cfg->d_model), st));
@@ -497,7 +476,89 @@ struct AvsrPlan {
   int head_idim = 0;
   cudaGraph_t graph = nullptr;
   cudaGraphExec_t exec = nullptr;
+  uint64_t kernel_nodes = 0;       // kernels one replay launches (counted into avsr_launch_count)
 };
+
+namespace avsr {
+
+// The side streams and events a plan's capture forks onto: `aux` for the rel-pos branch and, for a batch-sliced plan,
+// one stream + completion event per extra branch (branch[0] is the caller's stream).  Released when the plan is built.
+struct PlanStreams {
+  AuxFork aux;
+  std::vector<cudaStream_t> branch;
+  std::vector<cudaEvent_t> done;
+
+  PlanStreams() = default;
+  PlanStreams(const PlanStreams&) = delete;
+  PlanStreams& operator=(const PlanStreams&) = delete;
+  ~PlanStreams() {
+    if (aux.fork) cudaEventDestroy(aux.fork);
+    if (aux.join) cudaEventDestroy(aux.join);
+    if (aux.stream) cudaStreamDestroy(aux.stream);
+    for (size_t h = 1; h < branch.size(); ++h) {
+      if (done[h]) cudaEventDestroy(done[h]);
+      if (branch[h]) cudaStreamDestroy(branch[h]);
+    }
+  }
+  int create(cudaStream_t st, int branches) {
+    if (cudaStreamCreateWithFlags(&aux.stream, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaEventCreateWithFlags(&aux.fork, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&aux.join, cudaEventDisableTiming) != cudaSuccess) {
+      set_error("plan: cannot create the auxiliary stream / events: %s", cudaGetErrorString(cudaGetLastError()));
+      return AVSR_E_CUDA;
+    }
+    branch.assign(branches, nullptr);
+    done.assign(branches, nullptr);
+    branch[0] = st;
+    for (int h = 1; h < branches; ++h)
+      if (cudaStreamCreateWithFlags(&branch[h], cudaStreamNonBlocking) != cudaSuccess ||
+          cudaEventCreateWithFlags(&done[h], cudaEventDisableTiming) != cudaSuccess) {
+        set_error("plan: cannot create the branch streams");
+        return AVSR_E_CUDA;
+      }
+    return AVSR_OK;
+  }
+};
+
+static uint64_t graph_kernel_nodes(cudaGraph_t g) {
+  size_t n = 0;
+  if (cudaGraphGetNodes(g, nullptr, &n) != cudaSuccess) return 0;
+  std::vector<cudaGraphNode_t> nodes(n);
+  if (n == 0 || cudaGraphGetNodes(g, nodes.data(), &n) != cudaSuccess) return 0;
+  uint64_t k = 0;
+  for (auto nd : nodes) {
+    cudaGraphNodeType t;
+    if (cudaGraphNodeGetType(nd, &t) == cudaSuccess && t == cudaGraphNodeTypeKernel) ++k;
+  }
+  return k;
+}
+
+// Runs `run_all` once outside capture (function attributes such as the dynamic shared-memory opt-in, and lazy module
+// loading, must not happen inside a capture), then captures it from `st` (the side streams join the capture) into
+// p->graph and instantiates it.
+template <class Run>
+static int capture_plan(AvsrPlan* p, cudaStream_t st, const Run& run_all, const PlanStreams& side) {
+  AVSR_TRY(run_all());
+  bool ok = cudaStreamSynchronize(st) == cudaSuccess && cudaStreamSynchronize(side.aux.stream) == cudaSuccess;
+  for (size_t h = 1; h < side.branch.size(); ++h) ok = ok && cudaStreamSynchronize(side.branch[h]) == cudaSuccess;
+  if (!ok) { set_error("plan warm-up failed: %s", cudaGetErrorString(cudaGetLastError())); return AVSR_E_CUDA; }
+  cudaError_t e = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal);
+  if (e != cudaSuccess) { set_error("cudaStreamBeginCapture: %s", cudaGetErrorString(e)); return AVSR_E_CUDA; }
+  const uint64_t before = g_launches.load();
+  const int rc = run_all();
+  g_launches.store(before);   // captured launches are counted when the graph is replayed
+  e = cudaStreamEndCapture(st, &p->graph);
+  AVSR_TRY(rc);
+  if (e != cudaSuccess) { set_error("cudaStreamEndCapture: %s", cudaGetErrorString(e)); return AVSR_E_CUDA; }
+  e = cudaGraphInstantiate(&p->exec, p->graph, 0);
+  if (e != cudaSuccess) { set_error("cudaGraphInstantiate: %s", cudaGetErrorString(e)); return AVSR_E_CUDA; }
+  p->kernel_nodes = graph_kernel_nodes(p->graph);
+  return AVSR_OK;
+}
+
+using PlanPtr = std::unique_ptr<AvsrPlan, decltype(&avsr_plan_destroy)>;   // released once the plan is built
+
+}  // namespace avsr
 
 #ifdef AVSR_TRACE
 namespace avsr {
@@ -543,10 +604,7 @@ int avsr_prepare_weights(const AvsrEncoderConfig* cfg, const AvsrLayerParams* la
   AVSR_REQUIRE(layers && after_norm_w && after_norm_b && prepared, "NULL argument");
   AVSR_REQUIRE(valid_precision(precision), "bad precision %d", precision);
   Prepared P = layout_prepared(*cfg, prepared);
-  if (P.bytes > prepared_bytes) {
-    set_error("prepared buffer too small: need %zu bytes, got %zu", P.bytes, prepared_bytes);
-    return AVSR_E_WORKSPACE;
-  }
+  AVSR_REQUIRE_BYTES(P.bytes, prepared_bytes, "prepared buffer");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int rnd = operand_kind(precision);   // storage kind of the GEMM weights
   const long D = cfg->d_model, F = cfg->linear_units, K = cfg->cnn_kernel;
@@ -617,43 +675,20 @@ int avsr_plan_create(const AvsrEncoderConfig* cfg, const void* prepared, int B, 
   AVSR_REQUIRE(B > 0 && T > 0, "plan needs B>0, T>0 (got %d, %d)", B, T);
   AVSR_REQUIRE(valid_precision(precision), "bad precision %d", precision);
   Workspace W = layout_workspace(*cfg, B, T, workspace);
-  if (W.bytes > workspace_bytes) {
-    set_error("workspace too small: need %zu bytes, got %zu", W.bytes, workspace_bytes);
-    return AVSR_E_WORKSPACE;
-  }
-  AvsrPlan* p = new AvsrPlan();
+  AVSR_REQUIRE_BYTES(W.bytes, workspace_bytes, "workspace");
+  PlanPtr p(new AvsrPlan(), avsr_plan_destroy);
   p->cfg = *cfg; p->B = B; p->T = T; p->precision = precision; p->W = W;
   p->P = layout_prepared(*cfg, const_cast<void*>(prepared));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  // warm-up outside capture: sets function attributes (dynamic smem opt-in) that capture must not do lazily
   fill_lengths_kernel<<<cdiv(B, 128), 128, 0, st>>>(W.lengths, nullptr, B, T);
   g_launches.fetch_add(1);
-  AuxFork aux;
-  if (cudaStreamCreateWithFlags(&aux.stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaEventCreateWithFlags(&aux.fork, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&aux.join, cudaEventDisableTiming) != cudaSuccess) {
-    set_error("plan: cannot create the auxiliary stream / events: %s", cudaGetErrorString(cudaGetLastError()));
-    delete p;
-    return AVSR_E_CUDA;
-  }
-  auto drop_aux0 = [&]() {
-    cudaEventDestroy(aux.fork); cudaEventDestroy(aux.join); cudaStreamDestroy(aux.stream);
-  };
   // Batch slices as concurrent branches (frames of different batch elements never interact in this path): the GEMMs
   // of one slice fill the SMs another slice's one-tile-per-cluster kernels leave idle and hide their un-overlapped
   // prologues / epilogues.  Slice h covers batch elements [b0_h, b0_h + B_h); slice 0 runs on the caller's stream.
   const int nbr = plan_branches(B, T, precision);
-  std::vector<cudaStream_t> bstream(nbr, st);
-  std::vector<cudaEvent_t> bdone(nbr, nullptr);
-  bool bok = true;
-  for (int h = 1; h < nbr; ++h)
-    bok = bok && cudaStreamCreateWithFlags(&bstream[h], cudaStreamNonBlocking) == cudaSuccess &&
-          cudaEventCreateWithFlags(&bdone[h], cudaEventDisableTiming) == cudaSuccess;
-  auto drop_aux = [&]() {
-    drop_aux0();
-    for (int h = 1; h < nbr; ++h) { if (bdone[h]) cudaEventDestroy(bdone[h]); if (bstream[h] != st) cudaStreamDestroy(bstream[h]); }
-  };
-  if (!bok) { set_error("plan: cannot create the branch streams"); drop_aux(); delete p; return AVSR_E_CUDA; }
+  PlanStreams side;
+  AVSR_TRY(side.create(st, nbr));
+  const AuxFork& aux = side.aux;
   auto run_all = [&]() -> int {
     if (nbr == 1) return forward_body(p->cfg, p->P, p->W, B, T, W.lengths, nullptr, precision, st, &aux);
     AVSR_CUDA_TRY(cudaEventRecord(aux.fork, st));
@@ -663,53 +698,20 @@ int avsr_plan_create(const AvsrEncoderConfig* cfg, const void* prepared, int B, 
     int b0 = 0;
     for (int h = 0; h < nbr; ++h) {
       const int Bh = B / nbr + (h < B % nbr ? 1 : 0);
-      if (h) AVSR_CUDA_TRY(cudaStreamWaitEvent(bstream[h], aux.fork, 0));
+      if (h) AVSR_CUDA_TRY(cudaStreamWaitEvent(side.branch[h], aux.fork, 0));
       const Workspace Wh = slice_workspace(p->W, p->cfg, b0, T, h);
-      AVSR_TRY(forward_body(p->cfg, p->P, Wh, Bh, T, Wh.lengths, nullptr, precision, bstream[h], &aux, true));
+      AVSR_TRY(forward_body(p->cfg, p->P, Wh, Bh, T, Wh.lengths, nullptr, precision, side.branch[h], &aux, true));
       if (h) {
-        AVSR_CUDA_TRY(cudaEventRecord(bdone[h], bstream[h]));
-        AVSR_CUDA_TRY(cudaStreamWaitEvent(st, bdone[h], 0));
+        AVSR_CUDA_TRY(cudaEventRecord(side.done[h], side.branch[h]));
+        AVSR_CUDA_TRY(cudaStreamWaitEvent(st, side.done[h], 0));
       }
       b0 += Bh;
     }
     return AVSR_OK;
   };
-  int rc = run_all();
-  if (rc == AVSR_OK) {
-    bool ok = cudaStreamSynchronize(st) == cudaSuccess && cudaStreamSynchronize(aux.stream) == cudaSuccess;
-    for (int h = 1; h < nbr; ++h) ok = ok && cudaStreamSynchronize(bstream[h]) == cudaSuccess;
-    if (!ok) { set_error("plan warm-up failed: %s", cudaGetErrorString(cudaGetLastError())); rc = AVSR_E_CUDA; }
-  }
-  if (rc != AVSR_OK) { drop_aux(); delete p; return rc; }
-  cudaError_t e = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal);
-  if (e != cudaSuccess) { set_error("cudaStreamBeginCapture: %s", cudaGetErrorString(e)); drop_aux(); delete p; return AVSR_E_CUDA; }
-  const uint64_t before = g_launches.load();
-  rc = run_all();   // aux and the branch streams join the capture
-  g_launches.store(before);  // captured launches are counted when the graph is replayed
-  e = cudaStreamEndCapture(st, &p->graph);
-  drop_aux();
-  if (rc != AVSR_OK) { if (p->graph) cudaGraphDestroy(p->graph); delete p; return rc; }
-  if (e != cudaSuccess) { set_error("cudaStreamEndCapture: %s", cudaGetErrorString(e)); delete p; return AVSR_E_CUDA; }
-  e = cudaGraphInstantiate(&p->exec, p->graph, 0);
-  if (e != cudaSuccess) {
-    set_error("cudaGraphInstantiate: %s", cudaGetErrorString(e));
-    cudaGraphDestroy(p->graph); delete p; return AVSR_E_CUDA;
-  }
-  *plan = p;
+  AVSR_TRY(capture_plan(p.get(), st, run_all, side));
+  *plan = p.release();
   return AVSR_OK;
-}
-
-static uint64_t graph_kernel_nodes(cudaGraph_t g) {
-  size_t n = 0;
-  if (cudaGraphGetNodes(g, nullptr, &n) != cudaSuccess) return 0;
-  std::vector<cudaGraphNode_t> nodes(n);
-  if (n == 0 || cudaGraphGetNodes(g, nodes.data(), &n) != cudaSuccess) return 0;
-  uint64_t k = 0;
-  for (auto nd : nodes) {
-    cudaGraphNodeType t;
-    if (cudaGraphNodeGetType(nd, &t) == cudaSuccess && t == cudaGraphNodeTypeKernel) ++k;
-  }
-  return k;
 }
 
 int avsr_plan_forward(AvsrPlan* p, const float* xs, const int32_t* lengths, float* out, void* stream) {
@@ -720,10 +722,7 @@ int avsr_plan_forward(AvsrPlan* p, const float* xs, const int32_t* lengths, floa
   AVSR_CHECK_LAUNCH();
   AVSR_TRY(launch_embed_scale(xs, p->W.x, (long)N * D, sqrtf((float)D), st));
   AVSR_CUDA_TRY(cudaGraphLaunch(p->exec, st));
-  static thread_local cudaGraph_t counted = nullptr;
-  static thread_local uint64_t nk = 0;
-  if (counted != p->graph) { nk = graph_kernel_nodes(p->graph); counted = p->graph; }
-  g_launches.fetch_add(nk);
+  g_launches.fetch_add(p->kernel_nodes);
   AVSR_TRY(launch_layernorm(p->W.x, p->P.after_w, p->P.after_b, out, N, D, 0, st));
   return AVSR_OK;
 }
@@ -754,11 +753,7 @@ int avsr_linear(const float* x, const float* w, const float* bias, const float* 
   const void *xa = x, *wa = w;
   if (precision == AVSR_PREC_F16 && rows > 0 && n > 0) {
     AVSR_REQUIRE(workspace != nullptr, "avsr_linear: AVSR_PREC_F16 needs a workspace");
-    if (avsr_linear_workspace_bytes(rows, n, k, precision) > workspace_bytes) {
-      set_error("linear workspace too small: need %zu bytes, got %zu", avsr_linear_workspace_bytes(rows, n, k, precision),
-                workspace_bytes);
-      return AVSR_E_WORKSPACE;
-    }
+    AVSR_REQUIRE_BYTES(avsr_linear_workspace_bytes(rows, n, k, precision), workspace_bytes, "linear workspace");
     char* xh = reinterpret_cast<char*>(workspace);
     char* wh = xh + align_up((size_t)rows * k * 2, 256);
     AVSR_TRY(copy_round(x, xh, (long)rows * k, OP_F16, st));
@@ -810,10 +805,7 @@ int avsr_relpos_attention(const float* q, const float* k, const float* v, const 
   AVSR_REQUIRE(q && k && v && p && pos_bias_u && pos_bias_v && ctx && workspace, "NULL argument");
   AVSR_REQUIRE(valid_precision(precision), "bad precision %d", precision);
   if (B <= 0 || T <= 0) return AVSR_OK;
-  if (avsr_attention_workspace_bytes(B, T, H) > workspace_bytes) {
-    set_error("attention workspace too small: need %zu, got %zu", avsr_attention_workspace_bytes(B, T, H), workspace_bytes);
-    return AVSR_E_WORKSPACE;
-  }
+  AVSR_REQUIRE_BYTES(avsr_attention_workspace_bytes(B, T, H), workspace_bytes, "attention workspace");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const size_t N = (size_t)B * T, D = (size_t)H * kHeadDim;
   const int Tp = (T + 7) & ~7, R = 2 * T - 1;
@@ -845,10 +837,7 @@ int avsr_dwconv_bn_silu(const float* x, const float* w, const float* b, const fl
                         void* workspace, size_t workspace_bytes, void* stream) {
   AVSR_REQUIRE(x && w && b && bn_w && bn_b && bn_mean && bn_var && y && workspace, "NULL argument");
   AVSR_REQUIRE(C > 0 && C % 4 == 0 && K >= 1 && K % 2 == 1, "dwconv: bad C=%d K=%d", C, K);
-  if ((size_t)(K + 2) * C * sizeof(float) > workspace_bytes) {
-    set_error("dwconv workspace too small: need %zu bytes, got %zu", (size_t)(K + 2) * C * sizeof(float), workspace_bytes);
-    return AVSR_E_WORKSPACE;
-  }
+  AVSR_REQUIRE_BYTES((size_t)(K + 2) * C * sizeof(float), workspace_bytes, "dwconv workspace");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   float *wt = reinterpret_cast<float*>(workspace), *scale = wt + (size_t)K * C, *shift = scale + C;
   dw_fold_kernel<<<cdiv(C, 128), 128, 0, st>>>(w, b, bn_w, bn_b, bn_mean, bn_var, wt, scale, shift, C, K);
@@ -866,11 +855,7 @@ int avsr_pointwise_glu(const float* x, const float* w, const float* b, float* y,
   AVSR_REQUIRE(x && w && b && y && workspace, "NULL argument");
   AVSR_REQUIRE(C > 0 && C % 64 == 0, "pointwise_glu: C=%d must be a multiple of 64", C);
   AVSR_REQUIRE(valid_precision(precision), "bad precision %d", precision);
-  if (avsr_pointwise_glu_workspace_bytes(rows, C) > workspace_bytes) {
-    set_error("pointwise_glu workspace too small: need %zu bytes, got %zu", avsr_pointwise_glu_workspace_bytes(rows, C),
-              workspace_bytes);
-    return AVSR_E_WORKSPACE;
-  }
+  AVSR_REQUIRE_BYTES(avsr_pointwise_glu_workspace_bytes(rows, C), workspace_bytes, "pointwise_glu workspace");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   float* wi = reinterpret_cast<float*>(workspace);
   float* bi = wi + (size_t)2 * C * C;
@@ -902,10 +887,7 @@ int avsr_prepare_head(const AvsrEncoderConfig* cfg, int idim, int odim, const fl
   AVSR_REQUIRE(valid_precision(precision), "bad precision %d", precision);
   AVSR_REQUIRE(idim > 0 && idim % 8 == 0 && odim > 0, "head: idim=%d must be a positive multiple of 8, odim=%d > 0", idim, odim);
   HeadPrep H = layout_head(*cfg, idim, odim, prepared_head);
-  if (H.bytes > prepared_bytes) {
-    set_error("prepared head buffer too small: need %zu bytes, got %zu", H.bytes, prepared_bytes);
-    return AVSR_E_WORKSPACE;
-  }
+  AVSR_REQUIRE_BYTES(H.bytes, prepared_bytes, "prepared head buffer");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int rnd = operand_kind(precision);
   const long D = cfg->d_model;
@@ -934,8 +916,7 @@ int avsr_proj_encoder(const AvsrEncoderConfig* cfg, const void* prepared_head, c
   AVSR_REQUIRE(valid_precision(precision), "bad precision %d", precision);
   if (rows <= 0) return AVSR_OK;
   HeadPrep H = layout_head(*cfg, idim, odim, const_cast<void*>(prepared_head));
-  const size_t need = align_up((size_t)rows * idim * sizeof(float), 256);
-  if (need > workspace_bytes) { set_error("proj_encoder workspace too small: need %zu, got %zu", need, workspace_bytes); return AVSR_E_WORKSPACE; }
+  AVSR_REQUIRE_BYTES(align_up((size_t)rows * idim * sizeof(float), 256), workspace_bytes, "proj_encoder workspace");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const void* fx = feats;
   if (precision != AVSR_PREC_FP32) { AVSR_TRY(copy_round(feats, workspace, (long)rows * idim, operand_kind(precision), st)); fx = workspace; }
@@ -956,10 +937,7 @@ int avsr_ctc_logprobs(const AvsrEncoderConfig* cfg, const void* prepared_head, c
   AVSR_REQUIRE(prepared_head && hs && (logp || argmax) && workspace, "NULL argument");
   AVSR_REQUIRE(valid_precision(precision), "bad precision %d", precision);
   if (rows <= 0) return AVSR_OK;
-  if (avsr_ctc_workspace_bytes(cfg, rows, odim) > workspace_bytes) {
-    set_error("ctc workspace too small: need %zu, got %zu", avsr_ctc_workspace_bytes(cfg, rows, odim), workspace_bytes);
-    return AVSR_E_WORKSPACE;
-  }
+  AVSR_REQUIRE_BYTES(avsr_ctc_workspace_bytes(cfg, rows, odim), workspace_bytes, "ctc workspace");
   HeadPrep H = layout_head(*cfg, idim, odim, const_cast<void*>(prepared_head));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   Carver cv{reinterpret_cast<char*>(workspace)};
@@ -981,10 +959,7 @@ int avsr_features_to_logprobs(const AvsrEncoderConfig* cfg, const void* prepared
   AVSR_REQUIRE(prepared && prepared_head && feats && (logp || argmax) && workspace, "NULL buffer");
   AVSR_REQUIRE((long)B * T < (1L << 24), "B*T=%ld too large", (long)B * T);
   HeadWorkspace HW = layout_head_workspace(*cfg, B, T, idim, odim, workspace);
-  if (HW.bytes > workspace_bytes) {
-    set_error("workspace too small: need %zu bytes, got %zu", HW.bytes, workspace_bytes);
-    return AVSR_E_WORKSPACE;
-  }
+  AVSR_REQUIRE_BYTES(HW.bytes, workspace_bytes, "workspace");
   Workspace W = layout_workspace(*cfg, B, T, HW.enc);
   Prepared P = layout_prepared(*cfg, const_cast<void*>(prepared));
   HeadPrep H = layout_head(*cfg, idim, odim, const_cast<void*>(prepared_head));
@@ -1007,13 +982,10 @@ int avsr_head_plan_create(const AvsrEncoderConfig* cfg, const void* prepared, co
   AVSR_REQUIRE(plan && prepared && prepared_head && workspace && (logp || argmax), "NULL argument");
   AVSR_REQUIRE(B > 0 && T > 0 && idim > 0 && odim > 0, "plan needs B>0, T>0 (got %d, %d)", B, T);
   AVSR_REQUIRE(valid_precision(precision), "bad precision %d", precision);
-  if (avsr_head_plan_workspace_bytes(cfg, B, T, idim, odim) > workspace_bytes) {
-    set_error("workspace too small: need %zu bytes, got %zu", avsr_head_plan_workspace_bytes(cfg, B, T, idim, odim), workspace_bytes);
-    return AVSR_E_WORKSPACE;
-  }
+  AVSR_REQUIRE_BYTES(avsr_head_plan_workspace_bytes(cfg, B, T, idim, odim), workspace_bytes, "workspace");
   HeadWorkspace HW = layout_head_workspace(*cfg, B, T, idim, odim, workspace);
   float* feats_static = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + align_up(HW.bytes, 256));
-  AvsrPlan* p = new AvsrPlan();
+  PlanPtr p(new AvsrPlan(), avsr_plan_destroy);
   p->cfg = *cfg; p->B = B; p->T = T; p->precision = precision;
   p->W = layout_workspace(*cfg, B, T, HW.enc);
   p->P = layout_prepared(*cfg, const_cast<void*>(prepared));
@@ -1023,40 +995,14 @@ int avsr_head_plan_create(const AvsrEncoderConfig* cfg, const void* prepared, co
   fill_lengths_kernel<<<cdiv(B, 128), 128, 0, st>>>(p->W.lengths, nullptr, B, T);
   g_launches.fetch_add(1);
   AVSR_CUDA_TRY(cudaMemsetAsync(feats_static, 0, (size_t)B * T * idim * sizeof(float), st));
-  AuxFork aux;
-  if (cudaStreamCreateWithFlags(&aux.stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaEventCreateWithFlags(&aux.fork, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&aux.join, cudaEventDisableTiming) != cudaSuccess) {
-    set_error("plan: cannot create the auxiliary stream / events: %s", cudaGetErrorString(cudaGetLastError()));
-    delete p;
-    return AVSR_E_CUDA;
-  }
-  auto drop_aux = [&]() { cudaEventDestroy(aux.fork); cudaEventDestroy(aux.join); cudaStreamDestroy(aux.stream); };
+  PlanStreams side;
+  AVSR_TRY(side.create(st, 1));
   auto run_all = [&]() -> int {
-    return head_forward_body(p->cfg, p->P, H, p->W, HW, feats_static, p->W.lengths, B, T, idim, odim, enc_out, logp, argmax,
-                             precision, st, &aux);
+    return head_forward_body(p->cfg, p->P, H, p->W, HW, feats_static, p->W.lengths, B, T, idim, odim, enc_out, logp,
+                             argmax, precision, st, &side.aux);
   };
-  int rc = run_all();     // warm-up outside capture (function attributes, lazy module loading)
-  if (rc == AVSR_OK && (cudaStreamSynchronize(st) != cudaSuccess || cudaStreamSynchronize(aux.stream) != cudaSuccess)) {
-    set_error("plan warm-up failed: %s", cudaGetErrorString(cudaGetLastError()));
-    rc = AVSR_E_CUDA;
-  }
-  if (rc != AVSR_OK) { drop_aux(); delete p; return rc; }
-  cudaError_t e = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal);
-  if (e != cudaSuccess) { set_error("cudaStreamBeginCapture: %s", cudaGetErrorString(e)); drop_aux(); delete p; return AVSR_E_CUDA; }
-  const uint64_t before = g_launches.load();
-  rc = run_all();
-  g_launches.store(before);
-  e = cudaStreamEndCapture(st, &p->graph);
-  drop_aux();
-  if (rc != AVSR_OK) { if (p->graph) cudaGraphDestroy(p->graph); delete p; return rc; }
-  if (e != cudaSuccess) { set_error("cudaStreamEndCapture: %s", cudaGetErrorString(e)); delete p; return AVSR_E_CUDA; }
-  e = cudaGraphInstantiate(&p->exec, p->graph, 0);
-  if (e != cudaSuccess) {
-    set_error("cudaGraphInstantiate: %s", cudaGetErrorString(e));
-    cudaGraphDestroy(p->graph); delete p; return AVSR_E_CUDA;
-  }
-  *plan = p;
+  AVSR_TRY(capture_plan(p.get(), st, run_all, side));
+  *plan = p.release();
   return AVSR_OK;
 }
 
@@ -1067,7 +1013,7 @@ int avsr_head_plan_forward(AvsrPlan* p, const float* feats, const int32_t* lengt
   AVSR_CHECK_LAUNCH();
   AVSR_CUDA_TRY(cudaMemcpyAsync(p->head_feats, feats, (size_t)p->B * p->T * p->head_idim * sizeof(float), cudaMemcpyDeviceToDevice, st));
   AVSR_CUDA_TRY(cudaGraphLaunch(p->exec, st));
-  g_launches.fetch_add(graph_kernel_nodes(p->graph));
+  g_launches.fetch_add(p->kernel_nodes);
   return AVSR_OK;
 }
 

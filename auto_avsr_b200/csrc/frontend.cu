@@ -437,11 +437,6 @@ static int run_conv(int kind, bool stem, const void* x, const void* w, const flo
               : launch_conv_tc_bn<float, false>(x, w, scale, shift, resid, y, g, act, st);
 }
 
-static int op_kind(int precision) {
-  return precision == AVSR_PREC_F16 ? OP_F16 : precision == AVSR_PREC_TF32 ? OP_TF32 : OP_F32;
-}
-static int op_esz(int kind) { return kind == OP_F16 ? 2 : 4; }
-
 // ---------------------------------------------------------------- the two trunks
 struct ConvSpec { int cin, cout, kt, kh, kw, stride, K, Kp; };
 struct FrontendLayout {
@@ -468,7 +463,7 @@ static void frontend_layout(int modality, int kind, FrontendLayout* L) {
     }
   }
   size_t off = 0;
-  const size_t esz = (size_t)op_esz(kind);
+  const size_t esz = operand_bytes(kind);
   for (int j = 0; j < AVSR_FRONTEND_CONVS; ++j) {
     L->w_off[j] = off;
     off = align_up(off + (size_t)L->conv[j].cout * L->conv[j].Kp * esz, 256);
@@ -477,8 +472,6 @@ static void frontend_layout(int modality, int kind, FrontendLayout* L) {
   }
   L->total = off;
 }
-
-static bool valid_precision(int p) { return p == AVSR_PREC_FP32 || p == AVSR_PREC_TF32 || p == AVSR_PREC_F16; }
 
 // trunk geometry with the reference's padding (k - 1) / 2; 1-D convs are H = KH = 1 (then Ho = 1 for any stride)
 static ConvGeom trunk_geom(int N, int H, int W, const ConvSpec& c) {
@@ -503,7 +496,7 @@ struct FrontendPlan {
 
 static void frontend_plan(int modality, int kind, int B, int T_in, int H, int W, const FrontendLayout& L,
                           FrontendPlan* p) {
-  const size_t esz = (size_t)op_esz(kind);
+  const size_t esz = operand_bytes(kind);
   ConvGeom& s = p->stem;
   s = ConvGeom{};
   s.Cin = 1; s.Cout = 64; s.K = L.conv[0].K; s.Kp = L.conv[0].Kp;
@@ -548,7 +541,7 @@ using namespace avsr;
 extern "C" size_t avsr_frontend_prepared_bytes(int modality, int precision) {
   if ((modality != AVSR_FRONTEND_VIDEO && modality != AVSR_FRONTEND_AUDIO) || !valid_precision(precision)) return 0;
   FrontendLayout L;
-  frontend_layout(modality, op_kind(precision), &L);
+  frontend_layout(modality, operand_kind(precision), &L);
   return L.total;
 }
 
@@ -557,13 +550,10 @@ extern "C" int avsr_prepare_frontend(int modality, const AvsrConvBnParams* param
   AVSR_REQUIRE(modality == AVSR_FRONTEND_VIDEO || modality == AVSR_FRONTEND_AUDIO, "frontend: bad modality %d", modality);
   AVSR_REQUIRE(valid_precision(precision), "frontend: bad precision %d", precision);
   AVSR_REQUIRE(params && prepared, "NULL argument");
-  const int kind = op_kind(precision);
+  const int kind = operand_kind(precision);
   FrontendLayout L;
   frontend_layout(modality, kind, &L);
-  if (prepared_bytes < L.total) {
-    set_error("frontend: prepared buffer %zu < %zu bytes", prepared_bytes, L.total);
-    return AVSR_E_WORKSPACE;
-  }
+  AVSR_REQUIRE_BYTES(L.total, prepared_bytes, "frontend prepared buffer");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   uint8_t* base = reinterpret_cast<uint8_t*>(prepared);
   for (int j = 0; j < AVSR_FRONTEND_CONVS; ++j) {
@@ -591,7 +581,7 @@ extern "C" size_t avsr_frontend_workspace_bytes(int modality, int B, int T_in, i
   if ((modality != AVSR_FRONTEND_VIDEO && modality != AVSR_FRONTEND_AUDIO) || !valid_precision(precision) ||
       !frontend_shape_ok(modality, B, T_in, H, W))
     return 0;
-  const int kind = op_kind(precision);
+  const int kind = operand_kind(precision);
   FrontendLayout L;
   frontend_layout(modality, kind, &L);
   FrontendPlan P;
@@ -604,17 +594,14 @@ extern "C" int avsr_frontend_forward(int modality, const void* prepared, const f
   AVSR_REQUIRE(modality == AVSR_FRONTEND_VIDEO || modality == AVSR_FRONTEND_AUDIO, "frontend: bad modality %d", modality);
   AVSR_REQUIRE(valid_precision(precision), "frontend: bad precision %d", precision);
   AVSR_REQUIRE(frontend_shape_ok(modality, B, T_in, H, W), "frontend: bad shape B=%d T=%d H=%d W=%d", B, T_in, H, W);
-  const int kind = op_kind(precision);
+  const int kind = operand_kind(precision);
   FrontendLayout L;
   frontend_layout(modality, kind, &L);
   FrontendPlan P;
   frontend_plan(modality, kind, B, T_in, H, W, L, &P);
   if (P.groups == 0) return AVSR_OK;
   AVSR_REQUIRE(prepared && x && out && workspace, "NULL argument");
-  if (workspace_bytes < P.total) {
-    set_error("frontend: workspace %zu < %zu bytes", workspace_bytes, P.total);
-    return AVSR_E_WORKSPACE;
-  }
+  AVSR_REQUIRE_BYTES(P.total, workspace_bytes, "frontend workspace");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const uint8_t* pb = reinterpret_cast<const uint8_t*>(prepared);
   auto wt = [&](int j) { return static_cast<const void*>(pb + L.w_off[j]); };
@@ -677,7 +664,7 @@ extern "C" size_t avsr_conv_bn_act_workspace_bytes(int N, int H, int W, int C_in
     return 0;
   const ConvSpec c{C_in, C_out, 1, KH, KW, stride, KH * KW * C_in, KH * KW * C_in};
   const ConvGeom g = trunk_geom(N, H, W, c);
-  const size_t esz = (size_t)op_esz(op_kind(precision));
+  const size_t esz = operand_bytes(operand_kind(precision));
   return align_up((size_t)N * H * W * C_in * esz, 256) + align_up((size_t)C_out * g.Kp * esz, 256) +
          2 * align_up((size_t)conv_rows(g) * C_out * esz, 256) + 256;
 }
@@ -695,12 +682,9 @@ extern "C" int avsr_conv_bn_act(const float* x, const float* w, const float* sca
   AVSR_REQUIRE(((reinterpret_cast<uintptr_t>(scale) | reinterpret_cast<uintptr_t>(shift)) & 15) == 0,
                "conv_bn_act: scale / shift must be 16-byte aligned");
   const size_t need = avsr_conv_bn_act_workspace_bytes(N, H, W, C_in, C_out, KH, KW, stride, precision);
-  if (workspace_bytes < need) {
-    set_error("conv_bn_act: workspace %zu < %zu bytes", workspace_bytes, need);
-    return AVSR_E_WORKSPACE;
-  }
-  const int kind = op_kind(precision);
-  const size_t esz = (size_t)op_esz(kind);
+  AVSR_REQUIRE_BYTES(need, workspace_bytes, "conv_bn_act workspace");
+  const int kind = operand_kind(precision);
+  const size_t esz = operand_bytes(kind);
   const ConvSpec c{C_in, C_out, 1, KH, KW, stride, KH * KW * C_in, KH * KW * C_in};
   const ConvGeom g = trunk_geom(N, H, W, c);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);

@@ -298,7 +298,7 @@ int avsr_layernorm_bwd(const float* x, const float* gamma, const float* dy, floa
   const int nblk = rows < kRedBlocks * 8 ? cdiv(rows, 8) : kRedBlocks;
   const int rpc = cdiv(rows, nblk);
   const int nb = cdiv(rows, rpc);
-  if ((size_t)nb * 2 * d * sizeof(float) > workspace_bytes) { set_error("layernorm_bwd workspace too small"); return AVSR_E_WORKSPACE; }
+  AVSR_REQUIRE_BYTES((size_t)nb * 2 * d * sizeof(float), workspace_bytes, "layernorm_bwd workspace");
   float* part = reinterpret_cast<float*>(workspace);
   const size_t smem = (size_t)8 * 2 * d * sizeof(float);
   if (smem > 48 * 1024)
@@ -307,7 +307,7 @@ int avsr_layernorm_bwd(const float* x, const float* gamma, const float* dy, floa
   AVSR_CHECK_LAUNCH();
   // part[b][0][:] -> dgamma, part[b][1][:] -> dbeta : reduce with width 2*d into a temporary, then split
   float* tmp = part + (size_t)nb * 2 * d;
-  if (((size_t)nb * 2 * d + 2 * d) * sizeof(float) > workspace_bytes) { set_error("layernorm_bwd workspace too small"); return AVSR_E_WORKSPACE; }
+  AVSR_REQUIRE_BYTES(((size_t)nb * 2 * d + 2 * d) * sizeof(float), workspace_bytes, "layernorm_bwd workspace");
   reduce_partials_kernel<<<cdiv(2 * d, 256), 256, 0, st>>>(part, tmp, nb, 2 * d);
   AVSR_CHECK_LAUNCH();
   AVSR_CUDA_TRY(cudaMemcpyAsync(dgamma, tmp, d * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -320,7 +320,7 @@ int avsr_colsum(const float* y, float* out, int rows, int cols, void* workspace,
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (rows <= 0) { AVSR_CUDA_TRY(cudaMemsetAsync(out, 0, cols * sizeof(float), st)); return AVSR_OK; }
   const int rpc = cdiv(rows, kRedBlocks), nb = cdiv(rows, rpc);
-  if ((size_t)nb * cols * sizeof(float) > workspace_bytes) { set_error("colsum workspace too small"); return AVSR_E_WORKSPACE; }
+  AVSR_REQUIRE_BYTES((size_t)nb * cols * sizeof(float), workspace_bytes, "colsum workspace");
   float* part = reinterpret_cast<float*>(workspace);
   colsum_partial_kernel<<<nb, 256, 0, st>>>(y, part, rows, cols, rpc);
   AVSR_CHECK_LAUNCH();
@@ -372,7 +372,7 @@ int avsr_dwconv_raw(const float* x, const float* w, const float* b, float* y, in
   AVSR_REQUIRE(x && w && y && workspace, "NULL argument");
   AVSR_REQUIRE(C > 0 && C % 4 == 0 && K >= 1 && K % 2 == 1, "dwconv: bad C=%d K=%d", C, K);
   if (B <= 0 || T <= 0) return AVSR_OK;
-  if ((size_t)(K + 2) * C * sizeof(float) > workspace_bytes) { set_error("dwconv_raw workspace too small"); return AVSR_E_WORKSPACE; }
+  AVSR_REQUIRE_BYTES((size_t)(K + 2) * C * sizeof(float), workspace_bytes, "dwconv_raw workspace");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   float* wt = reinterpret_cast<float*>(workspace);
   float *ones = wt + (size_t)K * C, *zeros = ones + C;
@@ -394,7 +394,7 @@ int avsr_chan_sums(const float* v, const float* dy, const float* mean, const flo
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (rows <= 0) { AVSR_CUDA_TRY(cudaMemsetAsync(sums, 0, 2 * C * sizeof(float), st)); return AVSR_OK; }
   const int rpc = cdiv(rows, kRedBlocks), nb = cdiv(rows, rpc);
-  if ((size_t)nb * 2 * C * sizeof(float) > workspace_bytes) { set_error("chan_sums workspace too small"); return AVSR_E_WORKSPACE; }
+  AVSR_REQUIRE_BYTES((size_t)nb * 2 * C * sizeof(float), workspace_bytes, "chan_sums workspace");
   float* part = reinterpret_cast<float*>(workspace);
   if (dy) bn_bwd_partial_kernel<<<nb, 256, 0, st>>>(v, dy, mean, invstd, gamma, beta, part, rows, C, rpc);
   else chan_stats_partial_kernel<<<nb, 256, 0, st>>>(v, mean, part, rows, C, rpc);
@@ -439,7 +439,7 @@ int avsr_dwconv_wgrad(const float* x, const float* dconv, float* dw, float* db, 
   const int fpc = cdiv(T, cpu_);
   cpu_ = cdiv(T, fpc);
   const int nbw = B * cpu_;
-  if ((size_t)nbw * (K + 1) * C * sizeof(float) > workspace_bytes) { set_error("dwconv_wgrad workspace too small"); return AVSR_E_WORKSPACE; }
+  AVSR_REQUIRE_BYTES((size_t)nbw * (K + 1) * C * sizeof(float), workspace_bytes, "dwconv_wgrad workspace");
   float* partw = reinterpret_cast<float*>(workspace);
   dwconv_wgrad_partial_kernel<<<nbw, 256, 0, st>>>(x, dconv, partw, B, T, C, K, fpc, cpu_);
   AVSR_CHECK_LAUNCH();

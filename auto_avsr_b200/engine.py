@@ -36,6 +36,59 @@ def require_cuda(t: torch.Tensor, what: str) -> None:
         raise TypeError(f"{what}: expected float32, got {t.dtype}")
 
 
+class PlanCache:
+    """Which shapes get a CUDA-graph plan.  A shape key runs on direct launches (``get`` returns None) until it has been
+    seen ``graph_after`` times (the caller's threshold); then ``build()`` makes its entry, a tuple whose first item is the plan handle.  At most
+    ``max_plans`` entries are kept, the least recently used evicted first; ``_seen`` remembers at most 64 * max_plans
+    keys, so a stream of one-off shapes (the B = 1 eval loop) does not grow it.  Evicted and cleared plans are destroyed
+    with avsr_plan_destroy."""
+
+    def __init__(self, max_plans: int):
+        self.max_plans = max_plans
+        self._plans: "OrderedDict[tuple, tuple]" = OrderedDict()
+        self._seen: "OrderedDict[tuple, int]" = OrderedDict()
+        self._capture_stream: Dict[int, torch.cuda.Stream] = {}
+
+    def __del__(self):
+        try:
+            self.clear()
+        except Exception:
+            pass
+
+    def get(self, key: tuple, graph_after: int, build) -> Optional[tuple]:
+        hit = self._plans.get(key)
+        if hit is not None:
+            self._plans.move_to_end(key)
+            return hit
+        seen = self._seen.get(key, 0) + 1
+        self._seen[key] = seen
+        self._seen.move_to_end(key)
+        while len(self._seen) > 64 * self.max_plans:
+            self._seen.popitem(last=False)
+        if seen < graph_after:
+            return None
+        entry = self._plans[key] = build()
+        while len(self._plans) > self.max_plans:
+            _, old = self._plans.popitem(last=False)
+            lib.avsr_plan_destroy(old[0])
+        return entry
+
+    def clear(self) -> None:
+        for entry in self._plans.values():
+            lib.avsr_plan_destroy(entry[0])
+        self._plans.clear()
+
+    def capture_stream(self, device: torch.device) -> torch.cuda.Stream:
+        """the stream plans of `device` are captured on (the legacy default stream cannot capture), ordered after the
+        current stream's work"""
+        idx = device.index or 0
+        if idx not in self._capture_stream:
+            self._capture_stream[idx] = torch.cuda.Stream(device=device)
+        cs = self._capture_stream[idx]
+        cs.wait_stream(torch.cuda.current_stream(device))
+        return cs
+
+
 class SaturationError(OverflowError):
     """The fp16 operand path left its range (+-65504) for these weights / inputs: use precision "tf32" or "fp32"."""
 
@@ -60,9 +113,7 @@ class EncoderEngine:
         self.prepared_bytes = need
         self._prepared: Dict[Tuple[int, int], torch.Tensor] = {}      # (device index, precision) -> buffer
         self._workspaces: "OrderedDict[tuple, torch.Tensor]" = OrderedDict()
-        self._plans: "OrderedDict[tuple, tuple]" = OrderedDict()
-        self._seen: "OrderedDict[tuple, int]" = OrderedDict()        # shape key -> times seen (bounded)
-        self._capture_stream: Dict[int, torch.cuda.Stream] = {}
+        self._plans = PlanCache(self.MAX_PLANS)
         self._sat: Dict[int, torch.Tensor] = {}
         self.graph_after = self.GRAPH_AFTER
         self.stats = {"direct": 0, "graph": 0, "plans_built": 0}
@@ -70,19 +121,8 @@ class EncoderEngine:
     # ---- weights -------------------------------------------------------------------------------
     def invalidate(self) -> None:
         """Forget prepared weights (and the plans that bake their addresses)."""
-        self._destroy_plans()
-        self._prepared.clear()
-
-    def _destroy_plans(self) -> None:
-        for plan, _ws in self._plans.values():
-            lib.avsr_plan_destroy(plan)
         self._plans.clear()
-
-    def __del__(self):
-        try:
-            self._destroy_plans()
-        except Exception:
-            pass
+        self._prepared.clear()
 
     def prepare(self, state, device: torch.device, precision: str) -> torch.Tensor:
         """state: reference-keyed tensors ('encoders.{l}.<suffix>', 'after_norm.*') living on `device`, or a
@@ -180,30 +220,16 @@ class EncoderEngine:
         """The plan for this shape, or None while the shape has been seen fewer than ``graph_after`` times.  A plan's
         workspace is private to it and to the stream it was built for (two streams never share one)."""
         key = (device.index or 0, B, T, prec, prepared.data_ptr(), stream)
-        hit = self._plans.get(key)
-        if hit is not None:
-            self._plans.move_to_end(key)
-            return hit[0]
-        seen = self._seen.get(key, 0) + 1
-        self._seen[key] = seen
-        self._seen.move_to_end(key)
-        while len(self._seen) > 64 * self.MAX_PLANS:
-            self._seen.popitem(last=False)
-        if seen < self.graph_after:
-            return None
-        self.stats["plans_built"] += 1
-        ws = torch.empty(int(lib.avsr_workspace_bytes(C.byref(self.cfg), B, T)), dtype=torch.uint8, device=device)
-        idx = device.index or 0
-        if idx not in self._capture_stream:
-            self._capture_stream[idx] = torch.cuda.Stream(device=device)   # the legacy default stream cannot capture
-        cs = self._capture_stream[idx]
-        cs.wait_stream(torch.cuda.current_stream(device))
-        plan = C.c_void_p()
-        check(lib.avsr_plan_create(C.byref(self.cfg), prepared.data_ptr(), B, T, ws.data_ptr(), ws.numel(), prec,
-                                   cs.cuda_stream, C.byref(plan)))
-        cs.synchronize()
-        self._plans[key] = (plan, ws)
-        while len(self._plans) > self.MAX_PLANS:
-            _, (old, _ws) = self._plans.popitem(last=False)
-            lib.avsr_plan_destroy(old)
-        return plan
+
+        def build():
+            self.stats["plans_built"] += 1
+            ws = torch.empty(int(lib.avsr_workspace_bytes(C.byref(self.cfg), B, T)), dtype=torch.uint8, device=device)
+            cs = self._plans.capture_stream(device)
+            plan = C.c_void_p()
+            check(lib.avsr_plan_create(C.byref(self.cfg), prepared.data_ptr(), B, T, ws.data_ptr(), ws.numel(), prec,
+                                       cs.cuda_stream, C.byref(plan)))
+            cs.synchronize()
+            return plan, ws
+
+        hit = self._plans.get(key, self.graph_after, build)
+        return None if hit is None else hit[0]

@@ -13,7 +13,7 @@ from typing import Dict, Optional, Tuple
 import torch
 
 from ._cabi import EncoderConfig, check, lib
-from .engine import PRECISIONS, _ptr, _stream_handle, default_precision, require_cuda
+from .engine import PRECISIONS, EncoderEngine, PlanCache, _ptr, _stream_handle, default_precision, require_cuda
 
 
 class PreparedHead:
@@ -21,20 +21,9 @@ class PreparedHead:
         self.cfg = EncoderConfig(d_model, n_heads, linear_units, num_blocks, cnn_kernel)
         self._buf: Dict[tuple, Tuple[tuple, torch.Tensor]] = {}
         self._ws: Dict[tuple, torch.Tensor] = {}
-        self._plans: Dict[tuple, tuple] = {}          # shape key -> (plan, workspace, enc_out, logp, argmax)
-        self._seen: Dict[tuple, int] = {}
-        self._capture_stream: Dict[int, torch.cuda.Stream] = {}
-
-    def __del__(self):
-        try:
-            for plan, *_ in self._plans.values():
-                lib.avsr_plan_destroy(plan)
-        except Exception:
-            pass
+        self._plans = PlanCache(EncoderEngine.MAX_PLANS)    # shape key -> (plan, workspace, enc_out, logp, argmax)
 
     def drop_plans(self) -> None:
-        for plan, *_ in self._plans.values():
-            lib.avsr_plan_destroy(plan)
         self._plans.clear()
 
     @staticmethod
@@ -141,30 +130,23 @@ def features_to_log_probs(proj: torch.nn.Linear, encoder, ctc, feats: torch.Tens
         st = _stream_handle(dev)
         key = (dev.index or 0, B, T, idim, odim, PRECISIONS[precision], prepared.data_ptr(), hbuf.data_ptr(), st,
                want_features, want_argmax)
-        hit = head._plans.get(key)
-        if hit is None:
-            seen = head._seen[key] = head._seen.get(key, 0) + 1
-            if seen >= encoder._engine.graph_after:
-                nbytes = int(lib.avsr_head_plan_workspace_bytes(C.byref(head.cfg), B, T, idim, odim))
-                ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-                eo = torch.empty(B, T, head.cfg.d_model, dtype=torch.float32, device=dev) if want_features else None
-                lp = torch.empty(B, T, odim, dtype=torch.float32, device=dev)
-                am = torch.empty(B, T, dtype=torch.int32, device=dev) if want_argmax else None
-                idx = dev.index or 0
-                if idx not in head._capture_stream:
-                    head._capture_stream[idx] = torch.cuda.Stream(device=dev)
-                cs = head._capture_stream[idx]
-                cs.wait_stream(torch.cuda.current_stream(dev))
-                plan = C.c_void_p()
-                with torch.cuda.device(dev):
-                    check(lib.avsr_head_plan_create(C.byref(head.cfg), prepared.data_ptr(), hbuf.data_ptr(), B, T, idim, odim,
-                                                    _ptr(eo), lp.data_ptr(), _ptr(am), ws.data_ptr(), nbytes,
-                                                    PRECISIONS[precision], cs.cuda_stream, C.byref(plan)))
-                cs.synchronize()
-                hit = head._plans[key] = (plan, ws, eo, lp, am)
-                while len(head._plans) > encoder._engine.MAX_PLANS:
-                    old = head._plans.pop(next(iter(head._plans)))
-                    lib.avsr_plan_destroy(old[0])
+
+        def build():
+            nbytes = int(lib.avsr_head_plan_workspace_bytes(C.byref(head.cfg), B, T, idim, odim))
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            eo = torch.empty(B, T, head.cfg.d_model, dtype=torch.float32, device=dev) if want_features else None
+            lp = torch.empty(B, T, odim, dtype=torch.float32, device=dev)
+            am = torch.empty(B, T, dtype=torch.int32, device=dev) if want_argmax else None
+            cs = head._plans.capture_stream(dev)
+            plan = C.c_void_p()
+            with torch.cuda.device(dev):
+                check(lib.avsr_head_plan_create(C.byref(head.cfg), prepared.data_ptr(), hbuf.data_ptr(), B, T, idim, odim,
+                                                _ptr(eo), lp.data_ptr(), _ptr(am), ws.data_ptr(), nbytes,
+                                                PRECISIONS[precision], cs.cuda_stream, C.byref(plan)))
+            cs.synchronize()
+            return plan, ws, eo, lp, am
+
+        hit = head._plans.get(key, encoder._engine.graph_after, build)
         if hit is not None:
             plan, _ws, eo, lp, am = hit
             with torch.cuda.device(dev):

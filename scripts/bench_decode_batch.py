@@ -53,8 +53,8 @@ def main():
     sync = (lambda: None) if dry else torch.cuda.synchronize
     if dry:
         sys.path.insert(0, os.path.join(ROOT, "tests"))
-        from emu import build_decoder_batch
-        lib = build_decoder_batch.load()
+        from emu import build
+        lib = build.load("decoder_batch")
         odim, d, H, ff, L, lo, hi = 37, 64, 1, 64, 1, 2, 9
         dsd = decoder_state_dict(4, odim, d, H, ff, L)
         hsd = head_state_dict(4, 64, d, odim)

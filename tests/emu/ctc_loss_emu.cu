@@ -1,4 +1,4 @@
-// HOST replay of the CTC loss (csrc/ctc_loss.cu) -- TEST INFRASTRUCTURE ONLY (tests/emu/build_ctc.py builds it into
+// HOST replay of the CTC loss (csrc/ctc_loss.cu) -- TEST INFRASTRUCTURE ONLY (tests/emu/build.py builds it into
 // tests/emu/_build/libavsr_ctc_loss_emu.so; nothing under auto_avsr_b200/ knows it exists).
 //
 // The CPU suite checks the label compaction, the extended-label mapping, the alpha / beta recursion and the gradient

@@ -1,5 +1,5 @@
 // HOST replay of the batched decoder / CTC-prefix schedule (several utterances in one session) -- TEST INFRASTRUCTURE
-// ONLY (tests/emu/build_decoder_batch.py builds it into tests/emu/_build/libavsr_decoder_batch_emu.so).
+// ONLY (tests/emu/build.py builds it into tests/emu/_build/libavsr_decoder_batch_emu.so).
 //
 // It is the one-utterance replay of decoder_emu.cu plus the batched entries, so one library serves both sides of the
 // "a batched row equals the same hypothesis decoded alone" checks.  The source attention of a batched step, which the
@@ -34,65 +34,34 @@ struct BatchHostBackend : HostBackend {
 extern "C" {
 size_t avsr_decoder_batch_session_bytes(const AvsrDecoderConfig* cfg, int U, const int32_t* lengths, int max_steps,
                                         int max_hyps) {
-  long sum_T;
-  int max_len;
-  if (check_batch_lengths(lengths, U, 0, &sum_T, &max_len) != AVSR_OK || max_steps <= 0 || max_hyps <= 0) return 0;
-  return layout_dec_batch_session(*cfg, U, sum_T, max_len, max_steps, max_hyps, nullptr).bytes;
+  return decoder_batch_session_bytes_entry(cfg, U, lengths, max_steps, max_hyps);
 }
 size_t avsr_decoder_batch_step_workspace_bytes(const AvsrDecoderConfig* cfg, int T_max, int max_steps, int max_hyps) {
-  return layout_dec_work(*cfg, T_max, max_steps, max_hyps, nullptr).bytes;
+  return decoder_step_workspace_bytes_entry(cfg, T_max, max_steps, max_hyps);
 }
 int avsr_decoder_batch_begin(const AvsrDecoderConfig* cfg, const void* prepared, const float* memory,
                              const int32_t* lengths, int U, int T_max, int max_steps, int max_hyps, void* session,
                              size_t session_bytes, int precision, void*) {
-  AVSR_REQUIRE(T_max > 0 && max_steps > 0 && max_hyps > 0, "emu: bad T_max / max_steps / max_hyps");
-  long sum_T;
-  int max_len;
-  AVSR_TRY(check_batch_lengths(lengths, U, T_max, &sum_T, &max_len));
-  const DecBatchSession S = layout_dec_batch_session(*cfg, U, sum_T, max_len, max_steps, max_hyps, session);
-  if (S.bytes > session_bytes) return AVSR_E_WORKSPACE;
-  const DecPrep P = layout_dec_prepared(*cfg, const_cast<void*>(prepared));
-  BatchHostBackend bk;
-  return begin_batch_body(bk, *cfg, P, S, memory, lengths, U, T_max, sum_T, precision);
+  return decoder_batch_begin_entry(BatchHostBackend{}, cfg, prepared, memory, lengths, U, T_max, max_steps, max_hyps,
+                                   session, session_bytes, precision);
 }
 int avsr_decoder_batch_step(const AvsrDecoderConfig* cfg, const void* prepared, void* session, size_t session_bytes,
                             const int32_t* lengths, int U, int T_max, int max_steps, int max_hyps, const int32_t* tokens,
                             const int32_t* anc, const int32_t* row_utt, int step, int n, float* logp, void* workspace,
                             size_t workspace_bytes, int precision, void*) {
-  AVSR_REQUIRE(T_max > 0 && max_steps > 0 && max_hyps > 0, "emu: bad T_max / max_steps / max_hyps");
-  AVSR_REQUIRE(step >= 0 && step < max_steps, "decoder_batch_step: step %d outside %d positions", step, max_steps);
-  AVSR_REQUIRE(n >= 0 && n <= max_hyps, "decoder_batch_step: n=%d hypotheses exceed %d beam slots", n, max_hyps);
-  AVSR_REQUIRE((step == 0 || anc) && row_utt, "emu: NULL anc / row_utt");
-  long sum_T;
-  int max_len;
-  AVSR_TRY(check_batch_lengths(lengths, U, T_max, &sum_T, &max_len));
-  if (n == 0) return AVSR_OK;
-  const DecBatchSession S = layout_dec_batch_session(*cfg, U, sum_T, max_len, max_steps, max_hyps, session);
-  const DecWork W = layout_dec_work(*cfg, T_max, max_steps, max_hyps, workspace);
-  if (S.bytes > session_bytes || W.bytes > workspace_bytes) return AVSR_E_WORKSPACE;
-  const DecPrep P = layout_dec_prepared(*cfg, const_cast<void*>(prepared));
-  BatchHostBackend bk;
-  return step_batch_body(bk, *cfg, P, S, W, tokens, anc, row_utt, step, n, U, T_max, sum_T, max_steps, max_hyps, logp,
-                         precision);
+  return decoder_batch_step_entry(BatchHostBackend{}, cfg, prepared, session, session_bytes, lengths, U, T_max,
+                                  max_steps, max_hyps, tokens, anc, row_utt, step, n, logp, workspace, workspace_bytes,
+                                  precision);
 }
 int avsr_ctc_prefix_batch_init(const float* logp, const int32_t* lengths, int U, int T_max, int O, int blank,
                                int32_t* lengths_dev, float* r0, void*) {
-  AVSR_REQUIRE(T_max > 0, "emu: bad T_max");
-  long sum_T;
-  int max_len;
-  AVSR_TRY(check_batch_lengths(lengths, U, T_max, &sum_T, &max_len));
-  BatchHostBackend bk;
-  AVSR_TRY(bk.upload_i32(lengths_dev, lengths, U));
-  return bk.for_each(U, CtcInitBatchElem{logp, lengths_dev, r0, U, T_max, O, blank});
+  return ctc_prefix_batch_init_entry(BatchHostBackend{}, logp, lengths, U, T_max, O, blank, lengths_dev, r0);
 }
 int avsr_ctc_prefix_batch_score(const float* logp, const int32_t* lengths, int U, int T_max, int O, int blank, int eos,
                                 int out_len, const int32_t* last_ids, const float* r_prev, const float* s_prev,
                                 const int32_t* cand, const int32_t* row_utt, int n, int S, float* local, float* r,
                                 float* log_psi, void*) {
-  AVSR_REQUIRE(U >= 1 && T_max > 0, "emu: bad U / T_max");
-  if (n == 0) return AVSR_OK;
-  BatchHostBackend bk;
-  return ctc_prefix_batch_body(bk, logp, lengths, T_max, O, blank, eos, out_len, last_ids, r_prev, s_prev, cand, row_utt,
-                               n, S, local, r, log_psi);
+  return ctc_prefix_batch_score_entry(BatchHostBackend{}, logp, lengths, U, T_max, O, blank, eos, out_len, last_ids,
+                                      r_prev, s_prev, cand, row_utt, n, S, local, r, log_psi);
 }
 }  // extern "C"

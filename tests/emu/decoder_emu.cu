@@ -5,7 +5,8 @@
 // already GPU-verified kernels -- the launch schedule, the buffer layouts, the slot / ancestor addressing and every
 // per-element functor of decoder_body.cuh -- by compiling that same header against this backend: functors run as plain
 // loops, the GEMM / LayerNorm / log-softmax launchers (verified on the GPU by the encoder tests) are replaced by
-// naive fp32 loops.  Same extern "C" names and signatures as include/avsr_b200.h, HOST pointers, AVSR_PREC_FP32 only.
+// naive fp32 loops.  Same extern "C" names and signatures as include/avsr_b200.h, forwarded to the same entry bodies
+// (argument checks, layouts, size checks) as csrc/decoder.cu; HOST pointers, AVSR_PREC_FP32 only.
 #include <stdarg.h>
 
 #include <vector>
@@ -89,56 +90,41 @@ extern "C" {
 const char* avsr_last_error(void) { return g_emu_err.c_str(); }
 uint64_t avsr_launch_count(void) { return g_launches.load(); }
 
-size_t avsr_decoder_prepared_bytes(const AvsrDecoderConfig* cfg) { return layout_dec_prepared(*cfg, nullptr).bytes; }
+size_t avsr_decoder_prepared_bytes(const AvsrDecoderConfig* cfg) { return decoder_prepared_bytes_entry(cfg); }
 int avsr_prepare_decoder(const AvsrDecoderConfig* cfg, const AvsrDecoderLayerParams* layers, const float* embed_w,
                          const float* after_norm_w, const float* after_norm_b, const float* out_w, const float* out_b,
                          void* prepared, size_t prepared_bytes, int precision, void*) {
-  const DecPrep P = layout_dec_prepared(*cfg, prepared);
-  if (P.bytes > prepared_bytes) return AVSR_E_WORKSPACE;
-  HostBackend bk;
-  return prepare_body(bk, *cfg, layers, embed_w, after_norm_w, after_norm_b, out_w, out_b, P, precision);
+  return prepare_decoder_entry(HostBackend{}, cfg, layers, embed_w, after_norm_w, after_norm_b, out_w, out_b, prepared,
+                               prepared_bytes, precision);
 }
 size_t avsr_decoder_session_bytes(const AvsrDecoderConfig* cfg, int T, int max_steps, int max_hyps) {
-  return layout_dec_session(*cfg, T, max_steps, max_hyps, nullptr).bytes;
+  return decoder_session_bytes_entry(cfg, T, max_steps, max_hyps);
 }
 int avsr_decoder_begin(const AvsrDecoderConfig* cfg, const void* prepared, const float* memory, int T, int max_steps,
                        int max_hyps, void* session, size_t session_bytes, int precision, void*) {
-  const DecSession S = layout_dec_session(*cfg, T, max_steps, max_hyps, session);
-  if (S.bytes > session_bytes) return AVSR_E_WORKSPACE;
-  const DecPrep P = layout_dec_prepared(*cfg, const_cast<void*>(prepared));
-  HostBackend bk;
-  return begin_body(bk, *cfg, P, S, memory, T, precision);
+  return decoder_begin_entry(HostBackend{}, cfg, prepared, memory, T, max_steps, max_hyps, session, session_bytes,
+                             precision);
 }
 size_t avsr_decoder_step_workspace_bytes(const AvsrDecoderConfig* cfg, int T, int max_steps, int max_hyps) {
-  return layout_dec_work(*cfg, T, max_steps, max_hyps, nullptr).bytes;
+  return decoder_step_workspace_bytes_entry(cfg, T, max_steps, max_hyps);
 }
 int avsr_decoder_step(const AvsrDecoderConfig* cfg, const void* prepared, void* session, size_t session_bytes, int T,
                       int max_steps, int max_hyps, const int32_t* tokens, const int32_t* anc, int step, int n, float* logp,
                       void* workspace, size_t workspace_bytes, int precision, void*) {
-  AVSR_REQUIRE(step >= 0 && step < max_steps && n >= 0 && n <= max_hyps && (step == 0 || anc), "emu: bad step / n");
-  if (n == 0) return AVSR_OK;
-  const DecSession S = layout_dec_session(*cfg, T, max_steps, max_hyps, session);
-  const DecWork W = layout_dec_work(*cfg, T, max_steps, max_hyps, workspace);
-  if (S.bytes > session_bytes || W.bytes > workspace_bytes) return AVSR_E_WORKSPACE;
-  const DecPrep P = layout_dec_prepared(*cfg, const_cast<void*>(prepared));
-  HostBackend bk;
-  return step_body(bk, *cfg, P, S, W, tokens, anc, step, n, T, max_steps, max_hyps, logp, precision);
+  return decoder_step_entry(HostBackend{}, cfg, prepared, session, session_bytes, T, max_steps, max_hyps, tokens, anc,
+                            step, n, logp, workspace, workspace_bytes, precision);
 }
 int avsr_ctc_prefix_init(const float* logp, int T, int O, int blank, float* r0, void*) {
-  HostBackend bk;
-  return bk.for_each(1, CtcInitElem{logp, r0, T, O, blank});
+  return ctc_prefix_init_entry(HostBackend{}, logp, T, O, blank, r0);
 }
 int avsr_ctc_prefix_score(const float* logp, int T, int O, int blank, int eos, int out_len, const int32_t* last_ids,
                           const float* r_prev, const float* s_prev, const int32_t* cand, int n, int S, float* local,
                           float* r, float* log_psi, void*) {
-  if (n == 0) return AVSR_OK;
-  HostBackend bk;
-  return ctc_prefix_body(bk, logp, T, O, blank, eos, out_len, last_ids, r_prev, s_prev, cand, n, S, local, r, log_psi);
+  return ctc_prefix_score_entry(HostBackend{}, logp, T, O, blank, eos, out_len, last_ids, r_prev, s_prev, cand, n, S,
+                                local, r, log_psi);
 }
 int avsr_ctc_prefix_select(const float* r, const float* log_psi, const int32_t* cand, const int32_t* parent,
                            const int32_t* token, int T, int O, int n, int S, int m, float* r_next, float* s_next, void*) {
-  if (m == 0) return AVSR_OK;
-  HostBackend bk;
-  return ctc_select_body(bk, r, log_psi, cand, parent, token, T, O, n, S, m, r_next, s_next);
+  return ctc_prefix_select_entry(HostBackend{}, r, log_psi, cand, parent, token, T, O, n, S, m, r_next, s_next);
 }
 }  // extern "C"

@@ -1,5 +1,5 @@
 // HOST replay of the decoder's training kernels (csrc/decoder_train.cu) -- TEST INFRASTRUCTURE ONLY
-// (tests/emu/build_decoder_train.py builds it into tests/emu/_build/libavsr_decoder_train_emu.so; nothing under
+// (tests/emu/build.py builds it into tests/emu/_build/libavsr_decoder_train_emu.so; nothing under
 // auto_avsr_b200/ knows it exists).
 //
 // The CPU suite checks the masks, dropout factors, softmax / backward combination and the label-smoothing and embedding

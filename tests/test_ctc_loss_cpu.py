@@ -21,8 +21,8 @@ HAVE_NVCC = shutil.which("nvcc") is not None or os.path.exists("/usr/local/cuda/
 def emu():
     if not HAVE_NVCC:
         pytest.skip("nvcc is needed to build the host replay")
-    from emu import build_ctc
-    return build_ctc.load()
+    from emu import build
+    return build.load("ctc")
 
 
 def emu_ctc(lib, logits, hlens, ys, odim, dnll, ignore_id=-1):

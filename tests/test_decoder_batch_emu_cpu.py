@@ -18,8 +18,8 @@ pytestmark = pytest.mark.skipif(not os.path.exists("/usr/local/cuda/bin/nvcc"), 
 
 @pytest.fixture(scope="module")
 def emu():
-    from emu import build_decoder_batch
-    return build_decoder_batch.load()
+    from emu import build
+    return build.load("decoder_batch")
 
 
 class _Params(torch.nn.Module):

@@ -36,8 +36,8 @@ def _ref_module(name):
 def emu():
     if not HAVE_NVCC:
         pytest.skip("nvcc is needed to build the host replay")
-    from emu import build_decoder_train
-    return build_decoder_train.load()
+    from emu import build
+    return build.load("decoder_train")
 
 
 # ------------------------------------------------------------------ attention core
