@@ -44,11 +44,11 @@ def _lin(x: Tensor, sd: Dict[str, Tensor], pfx: str) -> Tensor:
     return x @ sd[pfx + ".weight"].to(x.dtype).T + sd[pfx + ".bias"].to(x.dtype)
 
 
-def positional_table(length: int, d: int, dtype) -> Tensor:
+def positional_table(length: int, d: int, dtype, device=None) -> Tensor:
     """``PositionalEncoding.extend_pe`` (embedding.py:60-80): built in fp32 exactly as the reference does, then cast."""
-    pos = torch.arange(0, length, dtype=torch.float32).unsqueeze(1)
-    div = torch.exp(torch.arange(0, d, 2, dtype=torch.float32) * -(math.log(10000.0) / d))
-    pe = torch.zeros(length, d)
+    pos = torch.arange(0, length, dtype=torch.float32, device=device).unsqueeze(1)
+    div = torch.exp(torch.arange(0, d, 2, dtype=torch.float32, device=device) * -(math.log(10000.0) / d))
+    pe = torch.zeros(length, d, device=device)
     pe[:, 0::2] = torch.sin(pos * div)
     pe[:, 1::2] = torch.cos(pos * div)
     return pe.to(dtype)
@@ -65,7 +65,7 @@ def _mha(q_in: Tensor, kv_in: Tensor, sd: Dict[str, Tensor], pfx: str, H: int, c
     v = _lin(kv_in, sd, pfx + ".linear_v").view(n, -1, H, dk).transpose(1, 2)
     s = q @ k.transpose(-1, -2) / math.sqrt(dk)
     if causal:
-        s = s.masked_fill(~torch.tril(torch.ones(Lq, Lq, dtype=torch.bool)), float("-inf"))
+        s = s.masked_fill(~torch.tril(torch.ones(Lq, Lq, dtype=torch.bool, device=s.device)), float("-inf"))
     p = torch.softmax(s, dim=-1)
     ctx = (p @ v).transpose(1, 2).reshape(n, Lq, d)
     return _lin(ctx, sd, pfx + ".linear_out")
@@ -77,7 +77,7 @@ def decoder_hidden(sd: Dict[str, Tensor], ys: Tensor, memory: Tensor, n_heads: i
     dtype = memory.dtype
     d = sd["embed.0.weight"].shape[1]
     n, L = ys.shape
-    x = sd["embed.0.weight"].to(dtype)[ys] * math.sqrt(d) + positional_table(L, d, dtype)[None]
+    x = sd["embed.0.weight"].to(dtype)[ys] * math.sqrt(d) + positional_table(L, d, dtype, memory.device)[None]
     mem = memory[None].expand(n, -1, -1) if memory.dim() == 2 else memory
     for l in range(num_blocks):
         p = f"decoders.{l}."
@@ -105,9 +105,9 @@ def ctc_initial_state(logp: Tensor, blank: int = 0) -> Tuple[Tensor, Tensor]:
     """State of the empty prefix: r^n = logzero, r^b_t = sum_{tau<=t} log p_tau(blank); prefix score 0
     (ctc_prefix_score.py:87-98).  -> r (T, 2, 1), s (1,)."""
     T = logp.shape[0]
-    r = torch.full((T, 2, 1), LOGZERO, dtype=logp.dtype)
+    r = torch.full((T, 2, 1), LOGZERO, dtype=logp.dtype, device=logp.device)
     r[:, 1, 0] = torch.cumsum(logp[:, blank], 0)
-    return r, torch.zeros(1, dtype=logp.dtype)
+    return r, torch.zeros(1, dtype=logp.dtype, device=logp.device)
 
 
 def ctc_prefix_scores(logp: Tensor, out_len: int, last_ids: Sequence[int], r_prev: Tensor, s_prev: Tensor,
@@ -125,10 +125,10 @@ def ctc_prefix_scores(logp: Tensor, out_len: int, last_ids: Sequence[int], r_pre
     xc = logp[:, cand.reshape(-1)].reshape(T, n, S)                 # log p_t(candidate)
     xb = logp[:, blank].reshape(T, 1, 1)
     r_sum = torch.logaddexp(r_prev[:, 0], r_prev[:, 1])             # (T, n)
-    same = cand == torch.as_tensor(list(last_ids)).reshape(n, 1)    # candidate repeats the last label
+    same = cand == torch.as_tensor(list(last_ids), device=cand.device).reshape(n, 1)    # candidate repeats the last label
     log_phi = torch.where(same[None], r_prev[:, 1].unsqueeze(2), r_sum.unsqueeze(2))      # (T, n, S)
-    rn = torch.full((T, n, S), LOGZERO, dtype=dt)
-    rb = torch.full((T, n, S), LOGZERO, dtype=dt)
+    rn = torch.full((T, n, S), LOGZERO, dtype=dt, device=logp.device)
+    rb = torch.full((T, n, S), LOGZERO, dtype=dt, device=logp.device)
     if out_len == 0:
         rn[0] = xc[0]
     start = max(out_len, 1)
@@ -138,7 +138,7 @@ def ctc_prefix_scores(logp: Tensor, out_len: int, last_ids: Sequence[int], r_pre
     # log psi = logsumexp( phi_{t-1} + x_t  for t in [start, T),  r^n_{start-1} )
     phi_x = torch.cat([log_phi[:1], log_phi[:-1]], 0) + xc
     psi_c = torch.logsumexp(torch.cat([phi_x[start:], rn[start - 1:start]], 0), dim=0)    # (n, S)
-    log_psi = torch.full((n, O), LOGZERO, dtype=dt)
+    log_psi = torch.full((n, O), LOGZERO, dtype=dt, device=logp.device)
     log_psi.scatter_(1, cand, psi_c)
     log_psi[:, eos] = r_sum[T - 1]
     log_psi[:, blank] = LOGZERO
