@@ -83,6 +83,7 @@ class DecoderLayerParams(C.Structure):
 
 FRONTEND_VIDEO, FRONTEND_AUDIO = 0, 1
 FRONTEND_CONVS = 20
+FRONTEND_TAPS = 10
 
 
 class ConvBnParams(C.Structure):
@@ -175,6 +176,8 @@ SIGNATURES = {
     "avsr_prepare_frontend": (_I, [_I, C.POINTER(ConvBnParams), _P, _Z, _I, _P]),
     "avsr_frontend_workspace_bytes": (_Z, [_I, _I, _I, _I, _I, _I]),
     "avsr_frontend_forward": (_I, [_I, _P, _P, _I, _I, _I, _I, _P, _P, _Z, _I, _P]),
+    "avsr_frontend_forward_taps": (_I, [_I, _P, _P, _I, _I, _I, _I, _P, C.POINTER(_P), _P, _Z, _I, _P]),
+    "avsr_frontend_tap_shape": (_I, [_I, _I, _I, _I, _I, _I, C.POINTER(C.c_int)]),
     "avsr_conv_bn_act_workspace_bytes": (_Z, [_I] * 9),
     "avsr_conv_bn_act": (_I, [_P, _P, _P, _P, _P, _I, _P] + [_I] * 8 + [_P, _Z, _I, _P]),
 }

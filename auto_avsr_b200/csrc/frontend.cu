@@ -589,8 +589,10 @@ extern "C" size_t avsr_frontend_workspace_bytes(int modality, int B, int T_in, i
   return P.total;
 }
 
-extern "C" int avsr_frontend_forward(int modality, const void* prepared, const float* x, int B, int T_in, int H, int W,
-                                     float* out, void* workspace, size_t workspace_bytes, int precision, void* stream) {
+// the forward of avsr_frontend_forward; taps[i] != NULL receives stage i as fp32 (avsr_frontend_tap_shape)
+static int frontend_forward_body(int modality, const void* prepared, const float* x, int B, int T_in, int H, int W,
+                                 float* out, void* workspace, size_t workspace_bytes, int precision, void* stream,
+                                 float* const* taps) {
   AVSR_REQUIRE(modality == AVSR_FRONTEND_VIDEO || modality == AVSR_FRONTEND_AUDIO, "frontend: bad modality %d", modality);
   AVSR_REQUIRE(valid_precision(precision), "frontend: bad precision %d", precision);
   AVSR_REQUIRE(frontend_shape_ok(modality, B, T_in, H, W), "frontend: bad shape B=%d T=%d H=%d W=%d", B, T_in, H, W);
@@ -610,11 +612,16 @@ extern "C" int avsr_frontend_forward(int modality, const void* prepared, const f
   uint8_t* ws = reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(workspace), 256));
   const size_t b0 = P.pre_bytes > P.act_bytes ? P.pre_bytes : P.act_bytes;
   void* buf[4] = {ws, ws + b0, ws + b0 + P.act_bytes, ws + b0 + 2 * P.act_bytes};
+  auto tap = [&](int i, const void* src, long n) -> int {
+    if (taps && taps[i]) AVSR_LAUNCH(cvt_from_op_kernel, grid_1d(n), 256, 0, st, src, taps[i], n, kind);
+    return AVSR_OK;
+  };
 
   // stem (+ max-pool for video) -> buf[1]
   int cur = 1;
   if (modality == AVSR_FRONTEND_VIDEO) {
     AVSR_TRY(run_conv(kind, true, x, wt(0), sc(0), sh(0), nullptr, buf[0], P.stem, 1, st));
+    AVSR_TRY(tap(0, buf[0], conv_rows(P.stem) * 64));
     const long n = (long)P.N * P.H0 * P.W0 * 64;
     if (kind == OP_F16)
       AVSR_LAUNCH(maxpool3x3s2_kernel<__half>, grid_1d(n), 256, 0, st, (const __half*)buf[0], (__half*)buf[1], P.N,
@@ -624,7 +631,9 @@ extern "C" int avsr_frontend_forward(int modality, const void* prepared, const f
                   P.stem.Ho, P.stem.Wo, P.H0, P.W0, 64);
   } else {
     AVSR_TRY(run_conv(kind, true, x, wt(0), sc(0), sh(0), nullptr, buf[1], P.stem, 1, st));
+    AVSR_TRY(tap(0, buf[1], conv_rows(P.stem) * 64));
   }
+  AVSR_TRY(tap(1, buf[1], (long)P.N * P.H0 * P.W0 * 64));
   // BasicBlocks: h = SiLU(BN1(conv1 x)); r = BN(downsample x) or x; x = SiLU(BN2(conv2 h) + r)
   int h = P.H0, w = P.W0, j = 1;
   for (int l = 0; l < 4; ++l) {
@@ -644,6 +653,7 @@ extern "C" int avsr_frontend_forward(int modality, const void* prepared, const f
       const int dst = fr[2];
       AVSR_TRY(run_conv(kind, false, buf[fr[0]], wt(j + 1), sc(j + 1), sh(j + 1), buf[res], buf[dst], g2, 1, st));
       cur = dst;
+      AVSR_TRY(tap(2 + 2 * l + b, buf[cur], conv_rows(g2) * g2.Cout));
       h = g2.Ho; w = g2.Wo;
       j += ds ? 3 : 2;
     }
@@ -655,6 +665,40 @@ extern "C" int avsr_frontend_forward(int modality, const void* prepared, const f
     AVSR_LAUNCH(mean_rows_kernel<__half>, grid_1d(n), 256, 0, st, (const __half*)buf[cur], out, P.groups, Pn, 512);
   else
     AVSR_LAUNCH(mean_rows_kernel<float>, grid_1d(n), 256, 0, st, (const float*)buf[cur], out, P.groups, Pn, 512);
+  return AVSR_OK;
+}
+
+extern "C" int avsr_frontend_forward(int modality, const void* prepared, const float* x, int B, int T_in, int H, int W,
+                                     float* out, void* workspace, size_t workspace_bytes, int precision, void* stream) {
+  return frontend_forward_body(modality, prepared, x, B, T_in, H, W, out, workspace, workspace_bytes, precision, stream,
+                               nullptr);
+}
+
+extern "C" int avsr_frontend_forward_taps(int modality, const void* prepared, const float* x, int B, int T_in, int H,
+                                          int W, float* out, float* const* taps, void* workspace,
+                                          size_t workspace_bytes, int precision, void* stream) {
+  AVSR_REQUIRE(taps, "NULL argument");
+  return frontend_forward_body(modality, prepared, x, B, T_in, H, W, out, workspace, workspace_bytes, precision, stream,
+                               taps);
+}
+
+extern "C" int avsr_frontend_tap_shape(int modality, int B, int T_in, int H, int W, int tap, int* dims) {
+  AVSR_REQUIRE(modality == AVSR_FRONTEND_VIDEO || modality == AVSR_FRONTEND_AUDIO, "frontend: bad modality %d", modality);
+  AVSR_REQUIRE(frontend_shape_ok(modality, B, T_in, H, W), "frontend: bad shape B=%d T=%d H=%d W=%d", B, T_in, H, W);
+  AVSR_REQUIRE(tap >= 0 && tap < AVSR_FRONTEND_TAPS && dims, "frontend: bad tap %d or NULL dims", tap);
+  FrontendLayout L;
+  frontend_layout(modality, OP_F32, &L);
+  FrontendPlan P;
+  frontend_plan(modality, OP_F32, B, T_in, H, W, L, &P);
+  int h = P.H0, w = P.W0, c = 64, j = 1;
+  if (tap == 0) { h = P.stem.Ho; w = P.stem.Wo; }
+  for (int b = 0; b + 2 <= tap; ++b) {          // BasicBlock b = 2 * layer + index: conv1 sets the output geometry
+    const ConvGeom g1 = trunk_geom(P.N, h, w, L.conv[j]);
+    h = g1.Ho; w = g1.Wo; c = g1.Cout;
+    j += (b == 2 || b == 4 || b == 6) ? 3 : 2;
+  }
+  if (P.W0 == 0) w = 0;                          // audio shorter than one 640-sample frame: every tap is empty
+  dims[0] = P.N; dims[1] = h; dims[2] = w; dims[3] = c;
   return AVSR_OK;
 }
 

@@ -13,7 +13,7 @@ from typing import Dict, List, Sequence, Tuple
 
 import torch
 
-from ._cabi import FRONTEND_AUDIO, FRONTEND_CONVS, FRONTEND_VIDEO, ConvBnParams, check, lib
+from ._cabi import FRONTEND_AUDIO, FRONTEND_CONVS, FRONTEND_TAPS, FRONTEND_VIDEO, ConvBnParams, check, lib
 from .engine import PRECISIONS, _ptr, _stream_handle, require_cuda
 
 MODALITIES = {"video": FRONTEND_VIDEO, "audio": FRONTEND_AUDIO}
@@ -73,31 +73,63 @@ class PreparedFrontend:
         return ws
 
 
-def frontend_forward(prep: PreparedFrontend, modality: str, pairs, x: torch.Tensor, precision: str) -> torch.Tensor:
-    """video x (B, T, 1, H, W) -> (B, T, 512); audio x (B, samples, 1) -> (B, samples // 640, 512).  fp32 CUDA tensors."""
-    require_cuda(x, "front-end input")
-    x = x.detach().contiguous()
+def _geometry(modality: str, x: torch.Tensor) -> Tuple[int, int, int, int, int]:
+    """(B, T_in, H, W, output rows per utterance) of a video (B, T, 1, H, W) or audio (B, samples, 1) input"""
     if modality == "video":
         if x.dim() != 5 or x.size(2) != 1:
             raise ValueError(f"video front-end: input must be (B, T, 1, H, W), got {tuple(x.shape)}")
         B, T, _, H, W = x.shape
-        out = torch.empty(B, T, 512, dtype=torch.float32, device=x.device)
-    else:
-        if x.dim() != 3 or x.size(2) != 1:
-            raise ValueError(f"audio front-end: input must be (B, samples, 1), got {tuple(x.shape)}")
-        B, T, _ = x.shape
-        H = W = 1
-        out = torch.empty(B, T // 640, 512, dtype=torch.float32, device=x.device)
+        return B, T, H, W, T
+    if x.dim() != 3 or x.size(2) != 1:
+        raise ValueError(f"audio front-end: input must be (B, samples, 1), got {tuple(x.shape)}")
+    B, T, _ = x.shape
+    return B, T, 1, 1, T // 640
+
+
+def frontend_workspace_bytes(modality: str, x: torch.Tensor, precision: str) -> int:
+    B, T, H, W, _ = _geometry(modality, x)
+    return int(lib.avsr_frontend_workspace_bytes(MODALITIES[modality], B, T, H, W, PRECISIONS[precision]))
+
+
+def frontend_forward(prep: PreparedFrontend, modality: str, pairs, x: torch.Tensor, precision: str,
+                     taps=None, workspace=None) -> torch.Tensor:
+    """video x (B, T, 1, H, W) -> (B, T, 512); audio x (B, samples, 1) -> (B, samples // 640, 512).  fp32 CUDA tensors.
+    ``taps`` (tests): a list of ``FRONTEND_TAPS`` fp32 CUDA tensors or None, shaped by ``frontend_tap_shape``, that
+    receive the stage outputs (``avsr_frontend_forward_taps``); ``workspace``: a uint8 CUDA tensor to run in instead of
+    the cached one."""
+    require_cuda(x, "front-end input")
+    x = x.detach().contiguous()
+    B, T, H, W, rows = _geometry(modality, x)
+    out = torch.empty(B, rows, 512, dtype=torch.float32, device=x.device)
     buf = prep.prepare(modality, pairs, x.device, precision)
     if out.numel() == 0:
         return out
     m, p = MODALITIES[modality], PRECISIONS[precision]
     nbytes = int(lib.avsr_frontend_workspace_bytes(m, B, T, H, W, p))
-    ws = prep.workspace(nbytes, x.device)
+    ws = prep.workspace(nbytes, x.device) if workspace is None else workspace
     with torch.cuda.device(x.device):
-        check(lib.avsr_frontend_forward(m, buf.data_ptr(), x.data_ptr(), B, T, H, W, out.data_ptr(), ws.data_ptr(),
-                                        ws.numel(), p, _stream_handle(x.device)))
+        if taps is None:
+            check(lib.avsr_frontend_forward(m, buf.data_ptr(), x.data_ptr(), B, T, H, W, out.data_ptr(), ws.data_ptr(),
+                                            ws.numel(), p, _stream_handle(x.device)))
+        else:
+            if len(taps) != FRONTEND_TAPS:
+                raise ValueError(f"front-end taps: expected {FRONTEND_TAPS} entries, got {len(taps)}")
+            for i, t in enumerate(taps):
+                if t is not None and (t.dtype != torch.float32 or not t.is_contiguous() or t.device != x.device or
+                                      tuple(t.shape) != frontend_tap_shape(modality, B, T, H, W, i)):
+                    raise ValueError(f"front-end tap {i}: needs a contiguous fp32 tensor of shape "
+                                     f"{frontend_tap_shape(modality, B, T, H, W, i)} on {x.device}")
+            arr = (C.c_void_p * FRONTEND_TAPS)(*[None if t is None else t.data_ptr() for t in taps])
+            check(lib.avsr_frontend_forward_taps(m, buf.data_ptr(), x.data_ptr(), B, T, H, W, out.data_ptr(), arr,
+                                                 ws.data_ptr(), ws.numel(), p, _stream_handle(x.device)))
     return out
+
+
+def frontend_tap_shape(modality: str, B: int, T: int, H: int, W: int, tap: int) -> Tuple[int, int, int, int]:
+    """Shape of stage tap ``tap`` (``avsr_frontend_tap_shape``): (frames, H, W, C) for video, (B, 1, L, C) for audio."""
+    dims = (C.c_int * 4)()
+    check(lib.avsr_frontend_tap_shape(MODALITIES[modality], B, T, H, W, tap, dims))
+    return tuple(int(d) for d in dims)
 
 
 def conv_bn_act(x: torch.Tensor, weight: torch.Tensor, scale: torch.Tensor, shift: torch.Tensor, stride: int = 1,

@@ -479,6 +479,15 @@ int avsr_prepare_frontend(int modality, const AvsrConvBnParams *params, void *pr
 size_t avsr_frontend_workspace_bytes(int modality, int B, int T_in, int H, int W, int precision);
 int avsr_frontend_forward(int modality, const void *prepared, const float *x, int B, int T_in, int H, int W,
                           float *out, void *workspace, size_t workspace_bytes, int precision, void *stream);
+/* Stage taps for parity tests: the same forward, and taps[i] != NULL (HOST array of AVSR_FRONTEND_TAPS device
+ * pointers) receives stage i as fp32, channels-last (frames or utterances, H, W, C): 0 the stem after BN + SiLU (video:
+ * before the max-pool), 1 the trunk input (video: after the max-pool; audio: the stem again), 2..9 the output of each
+ * BasicBlock, layer1.0 .. layer4.1.  avsr_frontend_tap_shape writes a tap's 4 dims; audio taps are (B, 1, L, C). */
+#define AVSR_FRONTEND_TAPS 10
+int avsr_frontend_forward_taps(int modality, const void *prepared, const float *x, int B, int T_in, int H, int W,
+                               float *out, float *const *taps, void *workspace, size_t workspace_bytes, int precision,
+                               void *stream);
+int avsr_frontend_tap_shape(int modality, int B, int T_in, int H, int W, int tap, int dims[4]);
 
 /* One trunk convolution + BatchNorm (as scale, shift) [+ residual] [+ SiLU] on channels-last fp32 tensors, computed in
  * `precision` (inputs converted to operand storage in the workspace): x (N, H, W, C_in), w (C_out, C_in, KH, KW) in

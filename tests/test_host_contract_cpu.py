@@ -261,6 +261,17 @@ def _probe(lib, decoder_only):
         code(f"modality {mod} too small", "avsr_frontend_forward", mod, p, p, 2, 1280, 44, 44, p, p, fw - 1, PTF32, None)
         code(f"modality {mod} bad precision", "avsr_frontend_forward", mod, p, p, 2, 1280, 44, 44, p, p, fw, -1, None)
     code("bad modality", "avsr_frontend_forward", 5, p, p, 2, 1280, 44, 44, p, p, 1 << 30, PTF32, None)
+    taps = (C.c_void_p * 10)(*([p] * 10))
+    fw = _c("avsr_frontend_workspace_bytes", 0, 2, 7, 44, 44, PF16)
+    code("too small", "avsr_frontend_forward_taps", 0, p, p, 2, 7, 44, 44, p, taps, p, fw - 1, PF16, None)
+    code("NULL taps", "avsr_frontend_forward_taps", 0, p, p, 2, 7, 44, 44, p, None, p, fw, PF16, None)
+    code("bad precision", "avsr_frontend_forward_taps", 1, p, p, 2, 1280, 1, 1, p, taps, p, fw, 4, None)
+    dims = (C.c_int * 4)()
+    for mod, B, T, H, W in ((0, 2, 29, 88, 88), (0, 1, 1, 1, 1), (0, 2, 3, 45, 61), (1, 2, 16000, 1, 1), (1, 3, 639, 1, 1),
+                            (0, 2, 5, 0, 88), (2, 1, 5, 88, 88)):
+        for tap in (-1, 0, 1, 2, 5, 9, 10):
+            rc = int(lib.avsr_frontend_tap_shape(mod, B, T, H, W, tap, dims))
+            out[f"avsr_frontend_tap_shape{(mod, B, T, H, W, tap)!r}"] = f"{rc}: {list(dims) if rc == 0 else ''}"
     kw = _c("avsr_conv_bn_act_workspace_bytes", 2, 22, 22, 64, 64, 3, 3, 1, PF16)
     code("too small", "avsr_conv_bn_act", p, p, p, p, None, 1, p, 2, 22, 22, 64, 64, 3, 3, 1, p, kw - 1, PF16, None)
     code("bad precision", "avsr_conv_bn_act", p, p, p, p, None, 1, p, 2, 22, 22, 64, 64, 3, 3, 1, p, kw, 7, None)
