@@ -4,11 +4,15 @@
 // Hopper pipeline (sm_90a).  One persistent CTA owns a 128 x BN output tile at a time:
 //   warp 0        : TMA producer -- cp.async.bulk.tensor 2-D boxes (rows x 128 bytes, SWIZZLE_128B) of A and Bw into
 //                   a STAGES-deep shared-memory ring, completion on `full` mbarriers
-//   warpgroups 1-2: wgmma.mma_async (M = 64 rows each, N = BN, K = 32 bytes) x4 per stage straight from shared memory
-//                   into register accumulators; a stage goes back to the producer (`empty` mbarrier) once the wgmma
-//                   group that read it has retired.  Then the same 8 warps run the fused epilogue: accumulators ->
-//                   fp32 tile in shared memory -> lane-per-row reads, bias / ReLU / residual / GLU / head-major
-//                   scatter / conversion to the next operand's storage, coalesced global stores (epilogue.cuh)
+//   warpgroups 1-2: ping-pong consumers.  Warpgroup 1 owns the CTA's even work items, warpgroup 2 the odd ones; each
+//                   runs the whole 128 x BN tile: wgmma.mma_async (two M = 64 chains, rows 0-63 and 64-127, N = BN,
+//                   K = 32 bytes) x4 per stage straight from shared memory into register accumulators; a stage goes
+//                   back to the producer (`empty` mbarrier) once the wgmma group that read it has retired.  Then the
+//                   same 4 warps run the fused epilogue: accumulators -> fp32 tile in shared memory -> lane-per-row
+//                   reads, bias / ReLU / residual / GLU / head-major scatter / conversion to the next operand's
+//                   storage, coalesced global stores (epilogue.cuh).  Two ordering mbarriers alternate the
+//                   warpgroups, one for main loops and one for epilogues, so one warpgroup's epilogue runs while the
+//                   other's main loop issues wgmma, and only one epilogue at a time uses the shared fp32 tile
 // Operand storage (template TOp): float = TF32 (8 elements per MMA-K) or __half (16 per MMA-K; same 10-bit mantissa,
 // half the bytes, twice the rate).  Out-of-bounds rows of edge tiles are zero-filled by TMA and masked in the
 // epilogue.  The tile width is chosen per problem by a small cost model (bytes through L2 vs tensor-pipe time).
@@ -75,9 +79,8 @@ int make_tmap_3d(CUtensorMap* map, const void* base, uint64_t planes, uint64_t r
 }
 
 // ---------------------------------------------------------------- the kernel
-constexpr int TC_BM = 128;          // rows per CTA tile / per A box (two warpgroups of 64 rows)
+constexpr int TC_BM = 128;          // rows per CTA tile / per A box (two wgmma chains of 64 rows)
 constexpr int TC_THREADS = 384;     // warpgroup 0: TMA producer (warp 0); warpgroups 1-2: wgmma + epilogue
-constexpr int TC_EPI_THREADS = 256; // the two consumer warpgroups
 constexpr int TC_SMEM_BUDGET = 227 * 1024;   // one persistent CTA per SM
 
 template <int BN>
@@ -116,12 +119,14 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int K, int tiles_m,
                int tiles_n, int splits, EpiParams ep) {
   // PERSISTENT: cluster c processes cluster tiles c, c + clusters, ... (n fastest, so concurrently running CTAs share
-  // A rows in L2; gemm_schedule.cuh).  The TMA ring never drains between tiles: the producer fetches the next tile's
-  // k-blocks while the consumer warpgroups run the epilogue of the current one.
+  // A rows in L2; gemm_schedule.cuh).  The TMA ring never drains between tiles: the producer fills it in item order,
+  // and the consumer warpgroups take turns on the items (even / odd), so stage ownership follows the item index.
+  // The main-loop order barrier also keeps a warpgroup from waiting on a `full` phase that is two phases ahead.
   // Clusters of CM x CN CTAs (tensor maps with boxes of BN / CM rows of Bw and 128 / CN rows of A): the CM CTAs of a
   // cluster column share their Bw tile and each loads 1/CM of it, multicast to all of them; likewise the CN CTAs of a
-  // cluster row share A.  Every consumer warp releases a stage to the producer of every CTA of the cluster, so a
-  // stage is refilled (by any peer) only after all CTAs it lands in are done with it.
+  // cluster row share A.  Every warp of the consumer warpgroup that owns a stage's item releases the stage to the
+  // producer of every CTA of the cluster (peers walk the same items, so their warpgroups of the same parity own it),
+  // so a stage is refilled (by any peer) only after all CTAs it lands in are done with it.
   using Cfg = TcCfg<BN>;
   using Op = OpTraits<TOp>;
   constexpr int CS = CM * CN;
@@ -133,12 +138,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const uint32_t raw = smem_u32(tc_smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;       // SWIZZLE_128B tiles need 1024-byte alignment
   uint8_t* gen = tc_smem_raw + (base - raw);
-  const uint32_t bars = base + S * Cfg::kStageBytes;  // full[S], empty[S]
-  int* s_flag = reinterpret_cast<int*>(gen + S * Cfg::kStageBytes + 2 * S * 8);   // split-K: "this CTA arrived last"
+  const uint32_t bars = base + S * Cfg::kStageBytes;  // full[S], empty[S], order[2][2]
+  int* s_flag = reinterpret_cast<int*>(gen + S * Cfg::kStageBytes + (2 * S + 4) * 8);   // split-K: "arrived last"
   float* s_acc = reinterpret_cast<float*>(gen + S * Cfg::kStageBytes + 256);      // [TC_BM][LD]
   float* s_vec = s_acc + TC_BM * LD;                                               // [3][BN]
   auto full_bar = [&](int s) { return bars + 8u * s; };
   auto empty_bar = [&](int s) { return bars + 8u * (S + s); };
+  // consumer warpgroup g waits on order_bar(phase, g) for its turn at the main loop (phase 0) or at the epilogue
+  // (phase 1); the other warpgroup's 4 warps arrive on it when they finish theirs
+  auto order_bar = [&](int phase, int g) { return bars + 8u * (2 * S + 2 * phase + g); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nkb = K / KE;
@@ -153,8 +161,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    // empty: 8 consumer warps of each CTA the stage's loads land in
-    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8 * CS); }
+    // empty: the 4 warps of the consumer warpgroup that owns the stage's item, in each CTA the stage's loads land in
+    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 4 * CS); }
+    for (int i = 0; i < 4; ++i) mbar_init(order_bar(i >> 1, i & 1), 4);
     fence_barrier_init();
   }
   __syncthreads();
@@ -193,14 +202,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
   } else {
     setmaxnreg_inc<232>();
-    const int wg = (warp - 4) >> 2;              // consumer warpgroup: accumulator rows [64 wg, 64 wg + 64)
-    const int e = warp - 4;                      // epilogue warp 0..7
-    const int q = e & 3;                         // 32-row slab of the tile this warp drains
-    const int chalf = e >> 2;                    // which half of the tile's columns this warp drains
+    const int wg = (warp - 4) >> 2;              // consumer warpgroup: the CTA's items with index parity wg
+    const int q = warp & 3;                      // 32-row slab of the tile this warp drains (all BN columns)
     constexpr int RB = LD * 4;                               // accumulator row stride in bytes
     // transpose buffer of a chunk: the warp's own accumulator rows, from the chunk's first column (epilogue.cuh)
     auto stg_at = [&](int c) { return reinterpret_cast<uint8_t*>(s_acc + (q * 32) * LD + c); };
-    const int cb = chalf * (BN / 2), ce = cb + BN / 2;      // this warp's columns of the tile
+    auto wg_sync = [&] { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); };   // this warpgroup only
     const int pr = lane >> 3;                                // row (of 4) this lane emits per read iteration
     const int pc = lane & 7;                                 // 16-byte piece of the 128-byte row segment
     constexpr int OC = StageOp<TOp>::kCols;                  // operand columns per row segment (32 tf32 / 64 f16)
@@ -213,56 +220,73 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         v[j] = t.x; v[j + 1] = t.y; v[j + 2] = t.z; v[j + 3] = t.w;
       }
     };
-    float acc[BN / 2];
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    float acc[BN];                               // rows 0-63 of the tile in acc[0, BN/2), rows 64-127 in acc[BN/2, BN)
     // a stage is released to the producer of every CTA of the cluster (lane r -> CTA r)
     auto release = [&](int s) {
       if constexpr (CS == 1) { if (lane == 0) mbar_arrive(empty_bar(s)); }
       else { if (lane < CS) mbar_arrive_cluster(empty_bar(s), (uint32_t)lane); }
     };
-    int it = 0;
+    // this warp is done with its main loop / epilogue: the other warpgroup may start its own
+    auto pass_turn = [&](int phase) { __syncwarp(); if (lane == 0) mbar_arrive(order_bar(phase, wg ^ 1)); };
+    int it = 0, turn = 0;
 #pragma unroll 1
-    for (int item = cluster_id; item < total_items; item += clusters) {
+    for (int item = cluster_id, idx = 0; item < total_items; item += clusters, ++idx) {
     const TcWork w = tc_work_item(item, crank, tiles_m, tiles_n, CM, CN);
     const int split = w.split, tile = w.tm * tiles_n + w.tn;
     const int m0 = w.tm * TC_BM, n0 = w.tn * BN;
     const int kb0 = split * nkb / splits, kb1 = (split + 1) * nkb / splits;
+    if ((idx & 1) != wg) { it += kb1 - kb0; continue; }   // the other warpgroup's item: skip its stages
+    // warpgroup 0 goes first: its first wait is on the parity of the phase before phase 0, which passes at once
+    const uint32_t par = (uint32_t)(turn++ & 1) ^ (wg == 0 ? 1u : 0u);
+    // the first wgmma of the item overwrites the accumulator; zeroing it here only tells the compiler that the previous
+    // item's values are dead, so they need no registers during the epilogue
+#pragma unroll
+    for (int i = 0; i < BN; ++i) acc[i] = 0.f;
     // ---- main loop: one wgmma group in flight; a stage is released once the group that read it has retired
+    mbar_wait(order_bar(0, wg), par);
     for (int kb = kb0; kb < kb1; ++kb, ++it) {
       const int s = it % S;
       mbar_wait(full_bar(s), (it / S) & 1);
       const uint32_t a_addr = base + s * Cfg::kStageBytes;
-      const uint64_t a_desc = wgmma_desc_sw128(a_addr + wg * (64 * 128));
+      const uint64_t a_desc0 = wgmma_desc_sw128(a_addr);
+      const uint64_t a_desc1 = wgmma_desc_sw128(a_addr + 64 * 128);
       const uint64_t b_desc = wgmma_desc_sw128(a_addr + Cfg::kABytes);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k)  // one MMA-K = 32 bytes = +2 in the descriptor's 16-byte address field
-        Op::template mma<BN>(acc, a_desc + 2 * k, b_desc + 2 * k, (kb != kb0) || (k != 0));
+      for (int k = 0; k < 4; ++k) {  // one MMA-K = 32 bytes = +2 in the descriptor's 16-byte address field
+        Op::template mma<BN>(acc, a_desc0 + 2 * k, b_desc + 2 * k, (kb != kb0) || (k != 0));
+        Op::template mma<BN>(acc + BN / 2, a_desc1 + 2 * k, b_desc + 2 * k, (kb != kb0) || (k != 0));
+      }
       wgmma_commit();
       wgmma_wait<1>();
-      wgmma_fence_regs<BN / 2>(acc);
+      wgmma_fence_regs<BN>(acc);
       if (kb != kb0) release((it - 1) % S);
     }
+    pass_turn(0);                                  // every k-block is issued: the other main loop may start
     wgmma_wait<0>();
-    wgmma_fence_regs<BN / 2>(acc);
+    wgmma_fence_regs<BN>(acc);
     release((it - 1) % S);
-    if (!w.valid) continue;                        // past the matrix edge: took part in the loads, stores nothing
+    mbar_wait(order_bar(1, wg), par);              // the other warpgroup's epilogue is done with s_acc / s_vec
+    if (!w.valid) { pass_turn(1); continue; }      // past the matrix edge: took part in the loads, stores nothing
     // ---- accumulator -> shared memory (fp32 rows), the tile's per-column vectors next to it
-    asm volatile("bar.sync 1, 256;" ::: "memory");   // previous tile's readers of s_acc / s_vec are done
     {
-      const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+      const int r = (warp & 3) * 16 + (lane >> 2);
       const int c = 2 * (lane & 3);
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        *reinterpret_cast<float2*>(s_acc + r * LD + 8 * j + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
-        *reinterpret_cast<float2*>(s_acc + (r + 8) * LD + 8 * j + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      for (int h = 0; h < 2; ++h) {
+        const float* ah = acc + h * (BN / 2);
+        float* sh = s_acc + (h * 64 + r) * LD + c;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          *reinterpret_cast<float2*>(sh + 8 * j) = make_float2(ah[4 * j], ah[4 * j + 1]);
+          *reinterpret_cast<float2*>(sh + 8 * LD + 8 * j) = make_float2(ah[4 * j + 2], ah[4 * j + 3]);
+        }
       }
       float* s_bias = s_vec;
       float* s_u = s_vec + BN;
       float* s_v = s_vec + 2 * BN;
       const int D = ep.H * kHeadDim;
-      for (int cc = threadIdx.x - 128; cc < BN; cc += TC_EPI_THREADS) {
+      for (int cc = threadIdx.x & 127; cc < BN; cc += 128) {
         const int n = n0 + cc;
         float bv = 0.f, uv = 0.f, vv = 0.f;
         if constexpr (MODE != EPI_VT && MODE != EPI_POS) {
@@ -274,14 +298,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         s_bias[cc] = bv; s_u[cc] = uv; s_v[cc] = vv;
       }
     }
-    asm volatile("bar.sync 1, 256;" ::: "memory");
+    wg_sync();
     {
       const int mw = m0 + q * 32;                            // first row of this warp's 32-row slab
       if constexpr (MODE == EPI_GLU) {
         static_assert(MODE != EPI_GLU || BN % 128 == 0, "GLU pairs live 64 columns apart inside a 128-wide group");
 #pragma unroll 1
-        for (int g = 0; g < BN; g += 128) {
-          const int c = g + chalf * 32;
+        for (int c = 0; c < BN; c += (c & 32) ? 96 : 32) {   // value columns [g, g + 64) of each 128-wide group g
           uint8_t* stg = stg_at(c);
           float val[32], gate[32];
           acc_ld32(c, val);
@@ -298,7 +321,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       } else if constexpr (MODE == EPI_LINEAR) {
         if (!ep.round_out) {                                 // fp32 destination (+ residual)
 #pragma unroll 1
-          for (int c = cb; c < ce; c += 32) {
+          for (int c = 0; c < BN; c += 32) {
             uint8_t* stg = stg_at(c);
             float v[32];
             acc_ld32(c, v);
@@ -349,7 +372,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           }
         } else {                                             // operand-typed destination (FFN hidden)
 #pragma unroll 1
-          for (int c = cb; c < ce; c += OC) {
+          for (int c = 0; c < BN; c += OC) {
             uint8_t* stg = stg_at(c);
             float v[OC];
 #pragma unroll
@@ -370,7 +393,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if constexpr (MODE == EPI_VT) { const int m = mw + lane; row_bias = (m < ep.M) ? ep.bias[m] : 0.f; }
         const int D = ep.H * kHeadDim;
 #pragma unroll 1
-        for (int c = cb; c < ce; c += OC) {
+        for (int c = 0; c < BN; c += OC) {
           uint8_t* stg = stg_at(c);
           float v[OC];
 #pragma unroll
@@ -454,19 +477,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       if (splits > 1) {
         // ---- deterministic split-K fix-up ("last block reduces"): publish the partial, count arrivals per tile ----
         __threadfence();
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (threadIdx.x == 128) {
+        wg_sync();
+        if ((threadIdx.x & 127) == 0) {
           const int old = atomicAdd(ep.counters + tile, 1);
           const int last = (old == splits - 1);
           if (last) ep.counters[tile] = 0;                 // every slice has arrived: re-arm for the next launch
           *s_flag = last;
         }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
+        wg_sync();
         if (*s_flag) {
           __threadfence();                                 // acquire: the other slices' partial tiles are visible
           const int mw = m0 + q * 32;
 #pragma unroll 1
-          for (int c = cb; c < ce; c += 32) {
+          for (int c = 0; c < BN; c += 32) {
             const int n = n0 + c + pc * 4;
             const float4 bv = *reinterpret_cast<const float4*>(s_vec + c + pc * 4);
             // loads first (8 independent 16-byte loads in flight per slice, no store in between), stores last
@@ -500,6 +523,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
+    pass_turn(1);                                  // this warp is done with s_acc / s_vec / s_flag
     }  // tile loop
   }
   __syncthreads();
@@ -562,10 +586,9 @@ static int launch_tc(const void* A, const void* Bw, int M, int N, int K, int spl
 
 // ---------------------------------------------------------------- tile / split selection
 // Cost model (SM cycles) of one GEMM on persistent CTAs, one per SM: the busier of the tensor pipe (dense wgmma rate
-// per SM) and operand ingest (bytes the busiest SM pulls through L2, at an assumed ~64 B/cycle), plus the epilogue of
-// the last item (it does not overlap the main loop of a following item: the accumulator lives in the registers of the
-// warpgroups that also run the epilogue).  Split-K (only for GEMMs that accumulate into the fp32 residual stream)
-// spreads a long K over more SMs.
+// per SM) and operand ingest (bytes the busiest SM pulls through L2, at an assumed ~64 B/cycle), plus one epilogue:
+// the consumer warpgroups alternate items, so every epilogue but the SM's last runs under the other warpgroup's main
+// loop.  Split-K (only for GEMMs that accumulate into the fp32 residual stream) spreads a long K over more SMs.
 // It picks 1 x 1 clusters only.  Multicast clusters cut the modelled L2 -> SM bytes by 25 % (2x1, 1x2) or 50 % (2x2)
 // but measured about 1.8x slower at the S2 shapes on an H100 80GB HBM3 at 400 W (FFN w_1 1600x3072x768: 22.7 us at
 // 1x1, 42.6 us at 2x1): the main loop waits on load latency, not L2 bandwidth (DESIGN.md section 4); clusters stay
@@ -592,7 +615,7 @@ static TileChoice choose_tile(int mode, int M, int N, int K, int esz, bool opera
       const double kfrac = (double)((nkb + splits - 1) / splits) * (128 / esz);    // K elements of the longest slice
       const double t_mma = per_sm * 128.0 * bn * kfrac / mac_per_cycle;
       const double t_in = per_sm * (128.0 + bn) * kfrac * esz / ingest;
-      const double t_epi = per_sm * 128.0 * bn * 10.0 / 256.0 * 4.0;               // one item's epilogue, per item
+      const double t_epi = 128.0 * bn * 10.0 / 128.0 * 4.0;                        // the last item's epilogue
       // fix-up: the last arriver re-reads `splits` fp32 partial tiles through the same port
       const double t_red = splits > 1 ? (double)splits * 128.0 * bn * 4.0 / ingest : 0.0;
       const double est = (t_mma > t_in ? t_mma : t_in) + t_epi + t_red + 4000.0;
