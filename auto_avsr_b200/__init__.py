@@ -32,11 +32,12 @@ def install_decoder(model):
     return _install_decoder(model)
 
 
-def install_frontend(model):
+def install_frontend(model, library_train: bool = False):
     """Swap an already-built reference ``E2E``'s ResNet front-end for the CUDA drop-in (same parameters and buffers):
-    in eval the front-end then runs in libavsr_b200 from the raw clip or waveform."""
+    in eval the front-end then runs in libavsr_b200 from the raw clip or waveform; with ``library_train`` its training
+    forward and backward do too."""
     from .install import install_frontend as _install_frontend
-    return _install_frontend(model)
+    return _install_frontend(model, library_train=library_train)
 
 
 def __getattr__(name):

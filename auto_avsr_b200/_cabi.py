@@ -180,6 +180,21 @@ SIGNATURES = {
     "avsr_frontend_tap_shape": (_I, [_I, _I, _I, _I, _I, _I, C.POINTER(C.c_int)]),
     "avsr_conv_bn_act_workspace_bytes": (_Z, [_I] * 9),
     "avsr_conv_bn_act": (_I, [_P, _P, _P, _P, _P, _I, _P] + [_I] * 8 + [_P, _Z, _I, _P]),
+    "avsr_frontend_train_conv_workspace_bytes": (_Z, [_I] * 11),
+    "avsr_frontend_train_conv_fwd": (_I, [_P, _P, _P, _P] + [_I] * 10 + [_P, _Z, _I, _P]),
+    "avsr_frontend_train_bn_finalize": (_I, [_P, _I, _I, C.c_double, C.c_double, _P, _P, _P, _P, _P]),
+    "avsr_frontend_train_bn_act_fwd": (_I, [_P, _P, _P, _P, _P, _P, _I, _P, C.c_long, _I, _P]),
+    "avsr_frontend_train_bn_bwd_workspace_bytes": (_Z, [C.c_long, _I]),
+    "avsr_frontend_train_bn_bwd_sums": (_I, [_P] * 7 + [_I, _P, C.c_long, _I, _P, _Z, _P]),
+    "avsr_frontend_train_bn_bwd_dx": (_I, [_P] * 7 + [_I, _P, _F, _P, _P, C.c_long, _I, _P]),
+    "avsr_frontend_train_dgrad_workspace_bytes": (_Z, [_I] * 9),
+    "avsr_frontend_train_conv_dgrad": (_I, [_P, _P, _P] + [_I] * 8 + [_P, _Z, _I, _P]),
+    "avsr_frontend_train_wgrad_workspace_bytes": (_Z, [_I] * 10),
+    "avsr_frontend_train_conv_wgrad": (_I, [_P, _P, _P] + [_I] * 10 + [_P, _Z, _I, _P]),
+    "avsr_frontend_train_maxpool_fwd": (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
+    "avsr_frontend_train_maxpool_bwd": (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
+    "avsr_frontend_train_mean_rows": (_I, [_P, _P, C.c_long, _I, _I, _P]),
+    "avsr_frontend_train_mean_rows_bwd": (_I, [_P, _P, C.c_long, _I, _I, _P]),
 }
 
 if not os.path.exists(LIB_PATH):

@@ -189,7 +189,8 @@ template <> struct ConvOp<__half> {
 };
 
 // STEM: x is the fp32 clip / waveform (Cin = 1) gathered element by element; otherwise x is the TOp activation.
-template <typename TOp, int BN, bool STEM>
+// RAW (training): y is fp32 and receives the accumulator itself; scale, shift, resid and act are not read.
+template <typename TOp, int BN, bool STEM, bool RAW = false>
 __global__ void __launch_bounds__(CV_THREADS, 1)
 conv_tc_kernel(const void* __restrict__ xv, const TOp* __restrict__ w, const float* __restrict__ scale,
                const float* __restrict__ shift, const TOp* __restrict__ resid, TOp* __restrict__ y, ConvGeom g,
@@ -332,6 +333,10 @@ conv_tc_kernel(const void* __restrict__ xv, const TOp* __restrict__ w, const flo
     const int n = n0 + c;
     if (m >= M || n >= g.Cout) continue;
     const float4 a = *reinterpret_cast<const float4*>(s_acc + r * LD + c);
+    if constexpr (RAW) {
+      *reinterpret_cast<float4*>(reinterpret_cast<float*>(y) + m * g.Cout + n) = a;
+      continue;
+    }
     const float4 sc = *reinterpret_cast<const float4*>(scale + n);
     const float4 sh = *reinterpret_cast<const float4*>(shift + n);
     float v0 = fmaf(a.x, sc.x, sh.x), v1 = fmaf(a.y, sc.y, sh.y), v2 = fmaf(a.z, sc.z, sh.z), v3 = fmaf(a.w, sc.w, sh.w);
@@ -394,10 +399,10 @@ __global__ void mean_rows_kernel(const T* __restrict__ x, float* __restrict__ ou
 // ---------------------------------------------------------------- launchers
 static int grid_1d(long n) { long b = (n + 255) / 256; return (int)(b < 8192 ? (b > 0 ? b : 1) : 8192); }
 
-template <typename TOp, int BN, bool STEM>
+template <typename TOp, int BN, bool STEM, bool RAW = false>
 static int launch_conv_tc_t(const void* x, const void* w, const float* scale, const float* shift, const void* resid,
                             void* y, const ConvGeom& g, int act, cudaStream_t st) {
-  auto kernel = conv_tc_kernel<TOp, BN, STEM>;
+  auto kernel = conv_tc_kernel<TOp, BN, STEM, RAW>;
   AVSR_SET_MAX_SMEM(kernel, CvCfg<BN>::kSmem);
   const long M = conv_rows(g);
   const dim3 grid((unsigned)((M + CV_BM - 1) / CV_BM), (unsigned)cdiv(g.Cout, BN));
@@ -406,11 +411,11 @@ static int launch_conv_tc_t(const void* x, const void* w, const float* scale, co
   return AVSR_OK;
 }
 
-template <typename TOp, bool STEM>
+template <typename TOp, bool STEM, bool RAW = false>
 static int launch_conv_tc_bn(const void* x, const void* w, const float* scale, const float* shift, const void* resid,
                              void* y, const ConvGeom& g, int act, cudaStream_t st) {
-  if (g.Cout <= 64) return launch_conv_tc_t<TOp, 64, STEM>(x, w, scale, shift, resid, y, g, act, st);
-  return launch_conv_tc_t<TOp, 128, STEM>(x, w, scale, shift, resid, y, g, act, st);
+  if (g.Cout <= 64) return launch_conv_tc_t<TOp, 64, STEM, RAW>(x, w, scale, shift, resid, y, g, act, st);
+  return launch_conv_tc_t<TOp, 128, STEM, RAW>(x, w, scale, shift, resid, y, g, act, st);
 }
 
 // one conv + BN [+ resid] [+ SiLU]; x fp32 when `stem`, else operand storage of `kind`
@@ -744,5 +749,782 @@ extern "C" int avsr_conv_bn_act(const float* x, const float* w, const float* sca
   if (resid) AVSR_LAUNCH(cvt_to_op_kernel, grid_1d(ny), 256, 0, st, resid, ro, ny, kind);
   AVSR_TRY(run_conv(kind, false, xo, wo, scale, shift, resid ? ro : nullptr, yo, g, act, st));
   AVSR_LAUNCH(cvt_from_op_kernel, grid_1d(ny), 256, 0, st, (const void*)yo, y, ny, kind);
+  return AVSR_OK;
+}
+
+// ================================================================ training (batch-statistics BatchNorm)
+// The front-end's training path is a chain of library calls that auto_avsr_b200/frontend_train.py drives per conv unit
+// (conv -> BatchNorm -> [+ residual] -> [SiLU]).  Activations cross the boundary as fp32 channels-last tensors.
+//  - forward conv: the inference implicit GEMM (conv_tc_kernel, RAW epilogue: the fp32 accumulator) or, in fp32, the
+//    direct kernel with scale 1 and shift 0; then per-tile (count, mean, M2) of every channel and a fixed-order merge
+//    with Chan's formula in fp64 (no one-pass variance);
+//  - dgrad: stride 1 is the same implicit GEMM over dZ with the 180-degree-rotated weight; stride 2 splits the input
+//    gradient into its parity classes, each a stride-1 implicit GEMM with a 1- or 2-tap sub-filter per axis (no MAC on
+//    inserted zeros), scattered to the class's pixels;
+//  - wgrad: a CUDA-core fp32 GEMM over output pixels, split across the SMs with partials summed in a fixed order;
+//  - max-pool with a recorded winner (first maximum in scan order, NaN wins: torch's rule) and a gather backward.
+namespace avsr {
+
+constexpr int FT_ROWS = 256;      // rows per statistics tile
+
+__global__ void fill_f32_kernel(float* p, int n, float v) {
+  pdl_wait();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) p[i] = v;
+}
+
+// per-tile (count, mean, M2) of each channel of z (rows, C): part[tile][3][C], two passes over the tile in fp32
+__global__ void __launch_bounds__(128) ft_stats_partial_kernel(const float* __restrict__ z, double* __restrict__ part,
+                                                                long rows, int C) {
+  pdl_wait();
+  const int c = blockIdx.y * 128 + threadIdx.x;
+  if (c >= C) return;
+  const long r0 = (long)blockIdx.x * FT_ROWS, r1 = min(rows, r0 + FT_ROWS);
+  const int n = (int)(r1 - r0);
+  float s = 0.f;
+  for (long r = r0; r < r1; ++r) s += z[r * C + c];
+  const float mean = s / (float)n;
+  float q = 0.f;
+  for (long r = r0; r < r1; ++r) { const float d = z[r * C + c] - mean; q = fmaf(d, d, q); }
+  double* p = part + (long)blockIdx.x * 3 * C;
+  p[c] = n; p[C + c] = mean; p[2 * C + c] = q;
+}
+
+__device__ __forceinline__ void chan_merge(double& n, double& m, double& q, double nb, double mb, double qb) {
+  if (nb == 0.0) return;
+  const double nn = n + nb, d = mb - m;
+  m += d * (nb / nn);
+  q += qb + d * d * (n * nb / nn);
+  n = nn;
+}
+
+// one CTA per channel: thread t merges tiles t, t + 256, ... in order, then a fixed tree; out[3][C]
+__global__ void __launch_bounds__(256) ft_stats_merge_kernel(const double* __restrict__ part, int tiles, int C,
+                                                             double* __restrict__ out) {
+  pdl_wait();
+  __shared__ double sn[256], sm[256], sq[256];
+  const int c = blockIdx.x, t = threadIdx.x;
+  double n = 0, m = 0, q = 0;
+  for (int i = t; i < tiles; i += 256) {
+    const double* p = part + (long)i * 3 * C;
+    chan_merge(n, m, q, p[c], p[C + c], p[2 * C + c]);
+  }
+  sn[t] = n; sm[t] = m; sq[t] = q;
+  __syncthreads();
+  for (int h = 128; h > 0; h >>= 1) {
+    if (t < h) {
+      double a = sn[t], b = sm[t], e = sq[t];
+      chan_merge(a, b, e, sn[t + h], sm[t + h], sq[t + h]);
+      sn[t] = a; sm[t] = b; sq[t] = e;
+    }
+    __syncthreads();
+  }
+  if (t == 0) { out[c] = sn[0]; out[C + c] = sm[0]; out[2 * C + c] = sq[0]; }
+}
+
+// merge R ranks' (count, mean, M2) in rank order; mean, 1/sqrt(var + eps) with the biased variance; running statistics
+// (when given) move by `factor` toward the mean and the unbiased variance
+__global__ void ft_bn_finalize_kernel(const double* __restrict__ st, int R, int C, double eps, double factor,
+                                      float* __restrict__ running_mean, float* __restrict__ running_var,
+                                      float* __restrict__ mean, float* __restrict__ invstd) {
+  pdl_wait();
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  double n = 0, m = 0, q = 0;
+  for (int r = 0; r < R; ++r) chan_merge(n, m, q, st[(long)r * 3 * C + c], st[(long)r * 3 * C + C + c],
+                                         st[(long)r * 3 * C + 2 * C + c]);
+  const double var = n > 0 ? q / n : 0.0;
+  mean[c] = (float)m;
+  invstd[c] = (float)(1.0 / sqrt(var + eps));
+  if (running_mean) {
+    const double unb = n > 1 ? q / (n - 1) : var;
+    running_mean[c] = (float)((1.0 - factor) * running_mean[c] + factor * m);
+    running_var[c] = (float)((1.0 - factor) * running_var[c] + factor * unb);
+  }
+}
+
+__device__ __forceinline__ float ft_act_pre(float z, float m, float is, float g, float b) { return (z - m) * is * g + b; }
+__device__ __forceinline__ float silu_grad_acc(float h, float dy) {
+  const float s = sigmoidf_acc(h);
+  return dy * s * (1.0f + h * (1.0f - s));
+}
+
+// y = [SiLU]((z - mean) * invstd * gamma + beta [+ resid])
+__global__ void ft_bn_act_fwd_kernel(const float* __restrict__ z, const float* __restrict__ mean,
+                                     const float* __restrict__ invstd, const float* __restrict__ gamma,
+                                     const float* __restrict__ beta, const float* __restrict__ resid, int act,
+                                     float* __restrict__ y, long n, int C) {
+  pdl_wait();
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    float h = ft_act_pre(z[i], mean[c], invstd[c], gamma[c], beta[c]);
+    if (resid) h += resid[i];
+    y[i] = act ? h * sigmoidf_acc(h) : h;
+  }
+}
+
+// ds = dL/d(BN output): dy, through SiLU when act; per-tile [sum ds, sum ds * x_hat]: part[tile][2][C] (fp64)
+__global__ void __launch_bounds__(128) ft_bn_bwd_partial_kernel(const float* __restrict__ z, const float* __restrict__ dy,
+                                                                 const float* __restrict__ mean,
+                                                                 const float* __restrict__ invstd,
+                                                                 const float* __restrict__ gamma,
+                                                                 const float* __restrict__ beta,
+                                                                 const float* __restrict__ resid, int act,
+                                                                 double* __restrict__ part, long rows, int C) {
+  pdl_wait();
+  const int c = blockIdx.y * 128 + threadIdx.x;
+  if (c >= C) return;
+  const long r0 = (long)blockIdx.x * FT_ROWS, r1 = min(rows, r0 + FT_ROWS);
+  const float m = mean[c], is = invstd[c], g = gamma[c], b = beta[c];
+  float s = 0.f, q = 0.f;
+  for (long r = r0; r < r1; ++r) {
+    const long i = r * C + c;
+    const float xh = (z[i] - m) * is;
+    float ds = dy[i];
+    if (act) ds = silu_grad_acc(xh * g + b + (resid ? resid[i] : 0.f), ds);
+    s += ds;
+    q = fmaf(ds, xh, q);
+  }
+  part[(long)blockIdx.x * 2 * C + c] = s;
+  part[(long)blockIdx.x * 2 * C + C + c] = q;
+}
+
+// out[j] = sum_t part[t][j] in fp64, one CTA per column j: strided per-thread sums, then a fixed tree
+__global__ void __launch_bounds__(256) ft_sum_merge_kernel(const double* __restrict__ part, int tiles, int width,
+                                                           float* __restrict__ out) {
+  pdl_wait();
+  __shared__ double sh[256];
+  const int j = blockIdx.x, t = threadIdx.x;
+  double s = 0;
+  for (int i = t; i < tiles; i += 256) s += part[(long)i * width + j];
+  sh[t] = s;
+  __syncthreads();
+  for (int h = 128; h > 0; h >>= 1) {
+    if (t < h) sh[t] += sh[t + h];
+    __syncthreads();
+  }
+  if (t == 0) out[j] = (float)sh[0];
+}
+
+// dz = gamma * invstd * (ds - (sum ds + x_hat * sum ds x_hat) / count); dres (when given) = ds
+__global__ void ft_bn_bwd_dx_kernel(const float* __restrict__ z, const float* __restrict__ dy,
+                                    const float* __restrict__ mean, const float* __restrict__ invstd,
+                                    const float* __restrict__ gamma, const float* __restrict__ beta,
+                                    const float* __restrict__ resid, int act, const float* __restrict__ sums,
+                                    float inv_count, float* __restrict__ dz, float* __restrict__ dres, long n, int C) {
+  pdl_wait();
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    const float g = gamma[c], is = invstd[c];
+    const float xh = (z[i] - mean[c]) * is;
+    float ds = dy[i];
+    if (act) ds = silu_grad_acc(xh * g + beta[c] + (resid ? resid[i] : 0.f), ds);
+    if (dres) dres[i] = ds;
+    dz[i] = g * is * (ds - inv_count * (sums[c] + xh * sums[C + c]));
+  }
+}
+
+// ---------------------------------------------------------------- dgrad sub-filters
+// Input pixel i = s * a + r of an axis with K taps, stride s, padding p receives output o = a + d from tap
+// k = r + p - s * d for every d with 0 <= k < K.  The d of one class are contiguous: [dmin, dmin + n).
+struct AxisClass { int dmin, n; };
+static AxisClass axis_class(int K, int s, int p, int r) {
+  int lo = 1 << 30, hi = -(1 << 30);
+  for (int k = 0; k < K; ++k) {
+    const int t = r + p - k;
+    if (t % s != 0) continue;
+    const int d = t / s;
+    lo = d < lo ? d : lo;
+    hi = d > hi ? d : hi;
+  }
+  return lo > hi ? AxisClass{0, 0} : AxisClass{lo, hi - lo + 1};
+}
+
+// sub-filter of one parity class as implicit-GEMM rows: dst[ci][(ty * nx + tx) * Cout + co] = w[co][ci][ky][kx],
+// ky = ry + py - s * (dy0 + ty) (likewise x); w is torch's (Cout, Cin, KH, KW)
+__global__ void ft_dgrad_weight_kernel(const float* __restrict__ w, void* __restrict__ dst, int Cout, int Cin, int KH,
+                                       int KW, int s, int ry, int rx, int py, int px, int dy0, int dx0, int ny, int nx,
+                                       int kind) {
+  pdl_wait();
+  const int Kp = ny * nx * Cout;
+  const long n = (long)Cin * Kp;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const int ci = (int)(i / Kp), k = (int)(i - (long)ci * Kp);
+    const int tap = k / Cout, co = k - tap * Cout;
+    const int ty = tap / nx, tx = tap - ty * nx;
+    const int ky = ry + py - s * (dy0 + ty), kx = rx + px - s * (dx0 + tx);
+    float v = 0.f;
+    if (ky >= 0 && ky < KH && kx >= 0 && kx < KW) v = w[(((long)co * Cin + ci) * KH + ky) * KW + kx];
+    if (kind == OP_F16) reinterpret_cast<__half*>(dst)[i] = to_half_sat(v);
+    else reinterpret_cast<float*>(dst)[i] = kind == OP_TF32 ? round_tf32(v) : v;
+  }
+}
+
+// dx[n][s a + ry][s b + rx][c] = sub[n][a][b][c] (sub NULL: 0)
+__global__ void ft_scatter_class_kernel(const float* __restrict__ sub, float* __restrict__ dx, int N, int H, int W,
+                                        int C, int s, int ry, int rx, int Hc, int Wc) {
+  pdl_wait();
+  const long n = (long)N * Hc * Wc * C;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    const long p = i / C;
+    const int b = (int)(p % Wc), a = (int)((p / Wc) % Hc);
+    const long f = p / ((long)Wc * Hc);
+    dx[((f * H + (long)s * a + ry) * W + (long)s * b + rx) * C + c] = sub ? sub[i] : 0.f;
+  }
+}
+
+// ---------------------------------------------------------------- wgrad (CUDA cores, fp32)
+// dw_part[split][co][k] = sum over this split's output pixels m of dz[m][co] * x[src(m, k)], k = tap * Cin + c.
+// 64 x 64 outputs per CTA, 4 x 4 per thread, 16 pixels per step through shared memory.
+constexpr int WG_T = 64, WG_P = 16;
+
+__device__ __forceinline__ float ft_gather(const float* __restrict__ x, const ConvGeom& g, long m, int k) {
+  if (k >= g.K) return 0.f;
+  const int hw = g.Ho * g.Wo;
+  const int n = (int)(m / hw), r = (int)(m - (long)n * hw);
+  const int oy = r / g.Wo, ox = r - oy * g.Wo;
+  const int t = n % g.T;
+  const int tap = k / g.Cin, c = k - tap * g.Cin;
+  const int kx = tap % g.KW, q = tap / g.KW;
+  const int ky = q % g.KH, dt = q / g.KH;
+  const int tt = t + dt - g.pt, iy = oy * g.sh - g.ph + ky, ix = ox * g.sw - g.pw + kx;
+  if (tt < 0 || tt >= g.T || iy < 0 || iy >= g.H || ix < 0 || ix >= g.W) return 0.f;
+  return x[(long)(n - t + tt) * g.ld_frame + ((long)iy * g.W + ix) * g.Cin + c];
+}
+
+__global__ void __launch_bounds__(256) ft_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ dz,
+                                                       float* __restrict__ part, ConvGeom g, long rows_per_split,
+                                                       int Kw) {
+  pdl_wait();
+  __shared__ float sa[WG_P][WG_T];     // dz[pixel][co]
+  __shared__ float sb[WG_P][WG_T];     // x[pixel][k]
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const int k0 = blockIdx.x * WG_T, co0 = blockIdx.y * WG_T;
+  const long M = (long)g.N * g.Ho * g.Wo;
+  const long p0 = (long)blockIdx.z * rows_per_split, p1 = min(M, p0 + rows_per_split);
+  float acc[4][4] = {};
+  const int lp = tid >> 4, lc = (tid & 15) * 4;      // loader: pixel lp, columns lc .. lc + 3
+  for (long pb = p0; pb < p1; pb += WG_P) {
+    const long m = pb + lp;
+    const bool ok = m < p1;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      sa[lp][lc + e] = ok ? dz[m * g.Cout + co0 + lc + e] : 0.f;
+      sb[lp][lc + e] = ok ? ft_gather(x, g, m, k0 + lc + e) : 0.f;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int p = 0; p < WG_P; ++p) {
+      const float4 a = *reinterpret_cast<const float4*>(&sa[p][ty * 4]);
+      const float4 b = *reinterpret_cast<const float4*>(&sb[p][tx * 4]);
+      const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
+    }
+    __syncthreads();
+  }
+  float* out = part + (long)blockIdx.z * g.Cout * Kw;
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    *reinterpret_cast<float4*>(out + (long)(co0 + ty * 4 + i) * Kw + k0 + tx * 4) =
+        make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+}
+
+// The same partials on wgmma with TF32 operands: one warpgroup per 64 (co) x 64 (k) tile, 32 output pixels per K-block.
+// Both operands are channels-last, so each K-block is transposed on its way into the 128B-swizzled tiles: thread t
+// reads column t % 64 (a C_out channel of dz, a k of the gathered input) for pixels t / 64 + 2 i with coalesced
+// loads, rounds to TF32 and stores the element at (column, pixel).  Two stages: the loads of K-block kb + 1 run under
+// the MMAs of kb.  The pixel coordinates of a K-block are decoded once into shared memory.
+constexpr int WGT_PB = 32;               // pixels per K-block (128 bytes of TF32)
+constexpr int WGT_STAGE = 2 * 64 * 128;  // A (64 co rows) + B (64 k rows)
+constexpr int WGT_SMEM = 1024 + 2 * WGT_STAGE + 2 * WGT_PB * 16;
+
+__global__ void __launch_bounds__(128) ft_wgrad_tc_kernel(const float* __restrict__ x, const float* __restrict__ dz,
+                                                          float* __restrict__ part, ConvGeom g, long rows_per_split,
+                                                          int Kw) {
+  pdl_wait();
+  extern __shared__ uint8_t wg_smem_raw[];
+  const uint32_t raw = smem_u32(wg_smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;
+  uint8_t* gen = wg_smem_raw + (base - raw);
+  int4* table = reinterpret_cast<int4*>(gen + 2 * WGT_STAGE);      // [stage][pixel]: frame base, iy0, ix0, t (-1: none)
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int col = tid & 63, prow = tid >> 6;
+  const int k0 = blockIdx.x * 64, co0 = blockIdx.y * 64;
+  const long M = (long)g.N * g.Ho * g.Wo;
+  const long p0 = (long)blockIdx.z * rows_per_split, p1 = min(M, p0 + rows_per_split);
+  const int nkb = p1 > p0 ? (int)((p1 - p0 + WGT_PB - 1) / WGT_PB) : 0;
+  // this thread's k column: tap and channel, decoded once
+  const int k = k0 + col;
+  const bool kok = k < g.K;
+  const int tap = kok ? k / g.Cin : 0, cch = kok ? k - tap * g.Cin : 0;
+  const int kx = tap % g.KW, ky = (tap / g.KW) % g.KH, dt = tap / (g.KW * g.KH);
+  // input element of pixel (frame n, iy0, ix0) for this k: n * ld_frame + (iy0 * W + ix0) * Cin + koff
+  const long koff = (long)(dt - g.pt) * g.ld_frame + ((long)ky * g.W + kx) * g.Cin + cch;
+  const int hw = g.Ho * g.Wo;
+
+  float acc[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+
+#pragma unroll 1
+  for (int kb = 0; kb < nkb; ++kb) {
+    const int s = kb & 1;
+    const long pb = p0 + (long)kb * WGT_PB;
+    if (tid < WGT_PB) {
+      const long m = pb + tid;
+      int4 e = make_int4(0, 0, 0, -1);
+      if (m < p1) {
+        const int n = (int)(m / hw), r = (int)(m - (long)n * hw);
+        const int oy = r / g.Wo, ox = r - oy * g.Wo;
+        e = make_int4(n, oy * g.sh - g.ph, ox * g.sw - g.pw, n % g.T);
+      }
+      table[s * WGT_PB + tid] = e;
+    }
+    __syncthreads();          // the table is in; the MMAs of kb - 2 (which read stage s) retired before kb - 1's sync
+    uint8_t* sa = gen + s * WGT_STAGE;
+    uint8_t* sb = sa + 64 * 128;
+#pragma unroll 4
+    for (int i = 0; i < WGT_PB / 2; ++i) {
+      const int p = prow + 2 * i;
+      const int4 e = table[s * WGT_PB + p];
+      float a = 0.f, b = 0.f;
+      if (e.w >= 0) {
+        a = dz[(pb + p) * g.Cout + co0 + col];
+        const int tt = e.w + dt - g.pt, iy = e.y + ky, ix = e.z + kx;
+        if (kok && tt >= 0 && tt < g.T && iy >= 0 && iy < g.H && ix >= 0 && ix < g.W)
+          b = x[(long)e.x * g.ld_frame + ((long)e.y * g.W + e.z) * g.Cin + koff];
+      }
+      const uint32_t off = sw128(col, p >> 2) + (p & 3) * 4;
+      *reinterpret_cast<float*>(sa + off) = round_tf32(a);
+      *reinterpret_cast<float*>(sb + off) = round_tf32(b);
+    }
+    fence_proxy_async();
+    __syncthreads();
+    const uint64_t a_desc = wgmma_desc_sw128(base + s * WGT_STAGE);
+    const uint64_t b_desc = wgmma_desc_sw128(base + s * WGT_STAGE + 64 * 128);
+    wgmma_fence();
+#pragma unroll
+    for (int q = 0; q < 4; ++q) wgmma_tf32_n64(acc, a_desc + 2 * q, b_desc + 2 * q, (kb | q) != 0);
+    wgmma_commit();
+    wgmma_wait<1>();          // the MMAs of kb - 1 are done: stage s ^ 1 may be rewritten next iteration
+    wgmma_fence_regs<32>(acc);
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs<32>(acc);
+  float* out = part + (long)blockIdx.z * g.Cout * Kw;
+  const int r = (warp & 3) * 16 + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    *reinterpret_cast<float2*>(out + (long)(co0 + r) * Kw + k0 + 8 * j + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+    *reinterpret_cast<float2*>(out + (long)(co0 + r + 8) * Kw + k0 + 8 * j + c) =
+        make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+  }
+}
+
+// dw[co][c][tap] (torch layout) = sum over splits in order of part[split][co][tap * Cin + c]
+__global__ void ft_wgrad_finish_kernel(const float* __restrict__ part, float* __restrict__ dw, int splits, int Cout,
+                                       int Cin, int taps, int Kw) {
+  pdl_wait();
+  const long n = (long)Cout * Cin * taps;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const int tap = (int)(i % taps);
+    const long q = i / taps;
+    const int c = (int)(q % Cin), co = (int)(q / Cin);
+    const long j = (long)co * Kw + (long)tap * Cin + c;
+    float s = 0.f;
+    for (int sp = 0; sp < splits; ++sp) s += part[(long)sp * Cout * Kw + j];
+    dw[i] = s;
+  }
+}
+
+// ---------------------------------------------------------------- pooling with recorded winners
+__global__ void ft_maxpool_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, uint8_t* __restrict__ idx,
+                                      int N, int Hi, int Wi, int Ho, int Wo, int C) {
+  pdl_wait();
+  const long total = (long)N * Ho * Wo * C;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    const long p = i / C;
+    const int ox = (int)(p % Wo), oy = (int)((p / Wo) % Ho);
+    const long n = p / ((long)Wo * Ho);
+    float best = -INFINITY;
+    int win = 4;
+    for (int dy = 0; dy < 3; ++dy) {
+      const int iy = 2 * oy - 1 + dy;
+      if (iy < 0 || iy >= Hi) continue;
+      for (int dx = 0; dx < 3; ++dx) {
+        const int ix = 2 * ox - 1 + dx;
+        if (ix < 0 || ix >= Wi) continue;
+        const float v = x[((n * Hi + iy) * Wi + ix) * C + c];
+        if (v > best || isnan(v)) { best = v; win = dy * 3 + dx; }
+      }
+    }
+    y[i] = best;
+    idx[i] = (uint8_t)win;
+  }
+}
+
+// dx[pixel] = sum of dy over the (at most 4) windows whose recorded winner is this pixel, in a fixed order
+__global__ void ft_maxpool_bwd_kernel(const float* __restrict__ dy, const uint8_t* __restrict__ idx,
+                                      float* __restrict__ dx, int N, int Hi, int Wi, int Ho, int Wo, int C) {
+  pdl_wait();
+  const long total = (long)N * Hi * Wi * C;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    const long p = i / C;
+    const int ix = (int)(p % Wi), iy = (int)((p / Wi) % Hi);
+    const long n = p / ((long)Wi * Hi);
+    float s = 0.f;
+    for (int oy = iy / 2 - 1; oy <= iy / 2 + 1; ++oy) {
+      const int ky = iy - (2 * oy - 1);
+      if (oy < 0 || oy >= Ho || ky < 0 || ky > 2) continue;
+      for (int ox = ix / 2 - 1; ox <= ix / 2 + 1; ++ox) {
+        const int kx = ix - (2 * ox - 1);
+        if (ox < 0 || ox >= Wo || kx < 0 || kx > 2) continue;
+        const long o = ((n * Ho + oy) * Wo + ox) * C + c;
+        if (idx[o] == ky * 3 + kx) s += dy[o];
+      }
+    }
+    dx[i] = s;
+  }
+}
+
+// dx[g * P + j][c] = dout[g][c] / P
+__global__ void ft_mean_rows_bwd_kernel(const float* __restrict__ dout, float* __restrict__ dx, long G, int P, int C) {
+  pdl_wait();
+  const long total = G * P * C;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    const long gi = i / ((long)P * C);
+    dx[i] = dout[gi * C + c] / (float)P;
+  }
+}
+
+// ---------------------------------------------------------------- host side
+// stem: 0 a trunk conv (x (N, H, W, C_in), padding (K - 1) / 2); 1 the video stem (x (N = B * T frames, H, W), T frames
+// per utterance); 2 the audio stem (x (N, W) samples already cut to whole 640-sample frames)
+static bool ft_geom(int stem, int N, int T, int H, int W, int Cin, int Cout, int KH, int KW, int stride, ConvGeom* g) {
+  if (N < 0 || H < 1 || W < 1) return false;
+  if (stem == 1) {
+    if (T < 1 || N % T != 0) return false;
+    *g = ConvGeom{};
+    g->N = N; g->T = T; g->H = H; g->W = W; g->Cin = 1; g->Cout = 64;
+    g->KT = 5; g->KH = 7; g->KW = 7; g->sh = 2; g->sw = 2; g->pt = 2; g->ph = 3; g->pw = 3;
+    g->Ho = (H + 6 - 7) / 2 + 1; g->Wo = (W + 6 - 7) / 2 + 1;
+    g->ld_frame = (long)H * W; g->K = 245; g->Kp = 256;
+    return true;
+  }
+  if (stem == 2) {
+    if (H != 1 || W % 640 != 0) return false;
+    *g = ConvGeom{};
+    g->N = N; g->T = 1; g->H = 1; g->W = W; g->Cin = 1; g->Cout = 64;
+    g->KT = 1; g->KH = 1; g->KW = 80; g->sh = 1; g->sw = 4; g->pt = 0; g->ph = 0; g->pw = 38;
+    g->Ho = 1; g->Wo = (W + 76 - 80) / 4 + 1;
+    g->ld_frame = W; g->K = 80; g->Kp = 128;
+    return true;
+  }
+  if (stem != 0 || Cin < 64 || Cin % 64 || Cout < 64 || Cout % 64 || (KH != 1 && KH != 3) || (KW != 1 && KW != 3) ||
+      (stride != 1 && stride != 2))
+    return false;
+  const ConvSpec c{Cin, Cout, 1, KH, KW, stride, KH * KW * Cin, KH * KW * Cin};
+  *g = trunk_geom(N, H, W, c);
+  return true;
+}
+
+static size_t ft_tiles(long rows) { return (size_t)((rows + FT_ROWS - 1) / FT_ROWS); }
+
+struct FtConvWs { size_t xop, wop, unit, part, total; };
+static FtConvWs ft_conv_ws(const ConvGeom& g, int stem, int kind) {
+  const size_t esz = operand_bytes(kind);
+  FtConvWs w{};
+  w.xop = stem ? 0 : align_up((size_t)g.N * g.H * g.W * g.Cin * esz, 256);
+  w.wop = align_up((size_t)g.Cout * g.Kp * esz, 256);
+  w.unit = align_up(2 * (size_t)g.Cout * 4, 256);
+  w.part = align_up(ft_tiles(conv_rows(g)) * 3 * g.Cout * 8, 256);
+  w.total = w.xop + w.wop + w.unit + w.part + 256;
+  return w;
+}
+
+static int run_conv_raw(int kind, bool stem, const void* x, const void* w, const float* ones, const float* zeros,
+                        float* z, const ConvGeom& g, cudaStream_t st) {
+  if (kind == OP_F32) return run_conv(kind, stem, x, w, ones, zeros, nullptr, z, g, 0, st);
+  const long M = conv_rows(g);
+  if (M <= 0) return AVSR_OK;
+  AVSR_REQUIRE(M / CV_BM < (long)INT32_MAX, "conv: too many output pixels");
+  if (kind == OP_F16)
+    return stem ? launch_conv_tc_bn<__half, true, true>(x, w, nullptr, nullptr, nullptr, z, g, 0, st)
+                : launch_conv_tc_bn<__half, false, true>(x, w, nullptr, nullptr, nullptr, z, g, 0, st);
+  return stem ? launch_conv_tc_bn<float, true, true>(x, w, nullptr, nullptr, nullptr, z, g, 0, st)
+              : launch_conv_tc_bn<float, false, true>(x, w, nullptr, nullptr, nullptr, z, g, 0, st);
+}
+
+struct FtDgradWs { size_t dzop, wop, unit, sub, total; };
+static FtDgradWs ft_dgrad_ws(const ConvGeom& g, int kind) {
+  const size_t esz = operand_bytes(kind);
+  FtDgradWs w{};
+  w.dzop = align_up((size_t)conv_rows(g) * g.Cout * esz, 256);
+  w.wop = align_up((size_t)g.Cin * g.KH * g.KW * g.Cout * esz, 256);     // the largest sub-filter is the whole filter
+  w.unit = align_up(2 * (size_t)g.Cin * 4, 256);
+  const int s = g.sh;
+  const size_t hc = (size_t)(g.H + s - 1) / s, wc = (size_t)(g.W + s - 1) / s;
+  w.sub = s == 1 ? 0 : align_up((size_t)g.N * hc * wc * g.Cin * 4, 256);
+  w.total = w.dzop + w.wop + w.unit + w.sub + 256;
+  return w;
+}
+
+static int ft_wgrad_splits(const ConvGeom& g) {
+  const long M = conv_rows(g);
+  const int tiles = cdiv(g.K, WG_T) * (g.Cout / WG_T);
+  long s = (132L * 4 + tiles - 1) / tiles;
+  const long max_s = (M + 255) / 256;              // at least 256 pixels per split
+  if (s > max_s) s = max_s;
+  return (int)(s < 1 ? 1 : s);
+}
+static size_t ft_wgrad_ws(const ConvGeom& g) {
+  const int Kw = cdiv(g.K, WG_T) * WG_T;
+  return align_up((size_t)ft_wgrad_splits(g) * g.Cout * Kw * 4, 256) + 256;
+}
+
+}  // namespace avsr
+
+static bool ft_prec_ok(int precision) { return valid_precision(precision); }
+
+extern "C" size_t avsr_frontend_train_conv_workspace_bytes(int stem, int N, int T, int H, int W, int C_in, int C_out,
+                                                           int KH, int KW, int stride, int precision) {
+  ConvGeom g;
+  if (!ft_prec_ok(precision) || !ft_geom(stem, N, T, H, W, C_in, C_out, KH, KW, stride, &g)) return 0;
+  return ft_conv_ws(g, stem, operand_kind(precision)).total;
+}
+
+extern "C" int avsr_frontend_train_conv_fwd(const float* x, const float* w, float* z, double* stats, int stem, int N,
+                                            int T, int H, int W, int C_in, int C_out, int KH, int KW, int stride,
+                                            void* workspace, size_t workspace_bytes, int precision, void* stream) {
+  AVSR_REQUIRE(ft_prec_ok(precision), "frontend train conv: bad precision %d", precision);
+  ConvGeom g;
+  AVSR_REQUIRE(ft_geom(stem, N, T, H, W, C_in, C_out, KH, KW, stride, &g),
+               "frontend train conv: unsupported shape stem=%d N=%d T=%d H=%d W=%d C_in=%d C_out=%d KH=%d KW=%d "
+               "stride=%d", stem, N, T, H, W, C_in, C_out, KH, KW, stride);
+  AVSR_REQUIRE(x && w && z && stats && workspace, "NULL argument");
+  const int kind = operand_kind(precision);
+  const FtConvWs L = ft_conv_ws(g, stem, kind);
+  AVSR_REQUIRE_BYTES(L.total, workspace_bytes, "frontend train conv workspace");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const long M = conv_rows(g);
+  if (M == 0) return AVSR_OK;
+  uint8_t* p = reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(workspace), 256));
+  void* xo = p; p += L.xop;
+  void* wo = p; p += L.wop;
+  float* ones = reinterpret_cast<float*>(p); p += L.unit;
+  double* part = reinterpret_cast<double*>(p);
+  const int taps = g.KT * g.KH * g.KW;
+  AVSR_LAUNCH(reorder_weight_kernel, grid_1d((long)g.Cout * g.Kp), 256, 0, st, w, wo, g.Cout, g.Cin, taps, g.Kp, kind);
+  AVSR_LAUNCH(fill_f32_kernel, cdiv(g.Cout, 256), 256, 0, st, ones, g.Cout, 1.f);
+  AVSR_LAUNCH(fill_f32_kernel, cdiv(g.Cout, 256), 256, 0, st, ones + g.Cout, g.Cout, 0.f);
+  const void* xin = x;
+  if (!stem) {
+    const long nx = (long)g.N * g.H * g.W * g.Cin;
+    AVSR_LAUNCH(cvt_to_op_kernel, grid_1d(nx), 256, 0, st, x, xo, nx, kind);
+    xin = xo;
+  }
+  AVSR_TRY(run_conv_raw(kind, stem != 0, xin, wo, ones, ones + g.Cout, z, g, st));
+  const int tiles = (int)ft_tiles(M);
+  AVSR_LAUNCH(ft_stats_partial_kernel, dim3(tiles, cdiv(g.Cout, 128)), 128, 0, st, (const float*)z, part, M, g.Cout);
+  AVSR_LAUNCH(ft_stats_merge_kernel, g.Cout, 256, 0, st, (const double*)part, tiles, g.Cout, stats);
+  return AVSR_OK;
+}
+
+extern "C" int avsr_frontend_train_bn_finalize(const double* stats, int ranks, int C, double eps, double factor,
+                                               float* running_mean, float* running_var, float* mean, float* invstd,
+                                               void* stream) {
+  AVSR_REQUIRE(ranks >= 1 && C >= 1 && eps >= 0.0 && factor >= 0.0 && factor <= 1.0,
+               "frontend train bn: bad ranks=%d C=%d eps or factor", ranks, C);
+  AVSR_REQUIRE(stats && mean && invstd && (running_mean != nullptr) == (running_var != nullptr), "NULL argument");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  AVSR_LAUNCH(ft_bn_finalize_kernel, cdiv(C, 128), 128, 0, st, stats, ranks, C, eps, factor, running_mean, running_var,
+              mean, invstd);
+  return AVSR_OK;
+}
+
+extern "C" int avsr_frontend_train_bn_act_fwd(const float* z, const float* mean, const float* invstd,
+                                              const float* gamma, const float* beta, const float* resid, int act,
+                                              float* y, long rows, int C, void* stream) {
+  AVSR_REQUIRE(rows >= 0 && C >= 1, "frontend train bn: bad rows=%ld C=%d", rows, C);
+  AVSR_REQUIRE(z && mean && invstd && gamma && beta && y, "NULL argument");
+  if (rows == 0) return AVSR_OK;
+  AVSR_LAUNCH(ft_bn_act_fwd_kernel, grid_1d(rows * C), 256, 0, reinterpret_cast<cudaStream_t>(stream), z, mean,
+              invstd, gamma, beta, resid, act, y, rows * C, C);
+  return AVSR_OK;
+}
+
+extern "C" size_t avsr_frontend_train_bn_bwd_workspace_bytes(long rows, int C) {
+  if (rows < 0 || C < 1) return 0;
+  return align_up(ft_tiles(rows) * 2 * C * 8, 256) + 256;
+}
+
+extern "C" int avsr_frontend_train_bn_bwd_sums(const float* z, const float* dy, const float* mean, const float* invstd,
+                                               const float* gamma, const float* beta, const float* resid, int act,
+                                               float* sums, long rows, int C, void* workspace, size_t workspace_bytes,
+                                               void* stream) {
+  AVSR_REQUIRE(rows >= 1 && C >= 1, "frontend train bn: bad rows=%ld C=%d", rows, C);
+  AVSR_REQUIRE(z && dy && mean && invstd && gamma && beta && sums && workspace, "NULL argument");
+  AVSR_REQUIRE_BYTES(avsr_frontend_train_bn_bwd_workspace_bytes(rows, C), workspace_bytes,
+                     "frontend train bn backward workspace");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  double* part = reinterpret_cast<double*>(align_up(reinterpret_cast<uintptr_t>(workspace), 256));
+  const int tiles = (int)ft_tiles(rows);
+  AVSR_LAUNCH(ft_bn_bwd_partial_kernel, dim3(tiles, cdiv(C, 128)), 128, 0, st, z, dy, mean, invstd, gamma, beta, resid,
+              act, part, rows, C);
+  AVSR_LAUNCH(ft_sum_merge_kernel, 2 * C, 256, 0, st, (const double*)part, tiles, 2 * C, sums);
+  return AVSR_OK;
+}
+
+extern "C" int avsr_frontend_train_bn_bwd_dx(const float* z, const float* dy, const float* mean, const float* invstd,
+                                             const float* gamma, const float* beta, const float* resid, int act,
+                                             const float* sums, float inv_count, float* dz, float* dres, long rows,
+                                             int C, void* stream) {
+  AVSR_REQUIRE(rows >= 0 && C >= 1, "frontend train bn: bad rows=%ld C=%d", rows, C);
+  AVSR_REQUIRE(z && dy && mean && invstd && gamma && beta && sums && dz, "NULL argument");
+  if (rows == 0) return AVSR_OK;
+  AVSR_LAUNCH(ft_bn_bwd_dx_kernel, grid_1d(rows * C), 256, 0, reinterpret_cast<cudaStream_t>(stream), z, dy, mean,
+              invstd, gamma, beta, resid, act, sums, inv_count, dz, dres, rows * C, C);
+  return AVSR_OK;
+}
+
+extern "C" size_t avsr_frontend_train_dgrad_workspace_bytes(int N, int H, int W, int C_in, int C_out, int KH, int KW,
+                                                            int stride, int precision) {
+  ConvGeom g;
+  if (!ft_prec_ok(precision) || !ft_geom(0, N, 1, H, W, C_in, C_out, KH, KW, stride, &g)) return 0;
+  return ft_dgrad_ws(g, operand_kind(precision)).total;
+}
+
+extern "C" int avsr_frontend_train_conv_dgrad(const float* dz, const float* w, float* dx, int N, int H, int W, int C_in,
+                                              int C_out, int KH, int KW, int stride, void* workspace,
+                                              size_t workspace_bytes, int precision, void* stream) {
+  AVSR_REQUIRE(ft_prec_ok(precision), "frontend train dgrad: bad precision %d", precision);
+  ConvGeom g;
+  AVSR_REQUIRE(ft_geom(0, N, 1, H, W, C_in, C_out, KH, KW, stride, &g),
+               "frontend train dgrad: unsupported shape N=%d H=%d W=%d C_in=%d C_out=%d KH=%d KW=%d stride=%d", N, H,
+               W, C_in, C_out, KH, KW, stride);
+  AVSR_REQUIRE(dz && w && dx && workspace, "NULL argument");
+  const int kind = operand_kind(precision);
+  const FtDgradWs L = ft_dgrad_ws(g, kind);
+  AVSR_REQUIRE_BYTES(L.total, workspace_bytes, "frontend train dgrad workspace");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (N == 0) return AVSR_OK;
+  uint8_t* p = reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(workspace), 256));
+  void* dzo = p; p += L.dzop;
+  void* wo = p; p += L.wop;
+  float* ones = reinterpret_cast<float*>(p); p += L.unit;
+  float* sub = reinterpret_cast<float*>(p);
+  const long nz = conv_rows(g) * g.Cout;
+  AVSR_LAUNCH(cvt_to_op_kernel, grid_1d(nz), 256, 0, st, dz, dzo, nz, kind);
+  AVSR_LAUNCH(fill_f32_kernel, cdiv(g.Cin, 256), 256, 0, st, ones, g.Cin, 1.f);
+  AVSR_LAUNCH(fill_f32_kernel, cdiv(g.Cin, 256), 256, 0, st, ones + g.Cin, g.Cin, 0.f);
+  const int s = g.sh;           // both axes (a 1-D conv has H = KH = 1: its odd rows are empty)
+  for (int ry = 0; ry < s; ++ry) {
+    for (int rx = 0; rx < s; ++rx) {
+      const AxisClass cy = axis_class(g.KH, s, g.ph, ry), cx = axis_class(g.KW, s, g.pw, rx);
+      const int Hc = (g.H - ry + s - 1) / s, Wc = (g.W - rx + s - 1) / s;
+      if (Hc <= 0 || Wc <= 0) continue;
+      if (cy.n == 0 || cx.n == 0) {
+        AVSR_LAUNCH(ft_scatter_class_kernel, grid_1d((long)N * Hc * Wc * g.Cin), 256, 0, st, (const float*)nullptr,
+                    dx, N, g.H, g.W, g.Cin, s, ry, rx, Hc, Wc);
+        continue;
+      }
+      // the class as a stride-1 conv over dz: output (Hc, Wc, C_in), taps (cy.n, cx.n) over C_out
+      ConvGeom c{};
+      c.N = N; c.T = 1; c.H = g.Ho; c.W = g.Wo; c.Cin = g.Cout; c.Ho = Hc; c.Wo = Wc; c.Cout = g.Cin;
+      c.KT = 1; c.KH = cy.n; c.KW = cx.n; c.sh = 1; c.sw = 1; c.pt = 0; c.ph = -cy.dmin; c.pw = -cx.dmin;
+      c.ld_frame = (long)g.Ho * g.Wo * g.Cout; c.K = cy.n * cx.n * g.Cout; c.Kp = c.K;
+      AVSR_LAUNCH(ft_dgrad_weight_kernel, grid_1d((long)g.Cin * c.Kp), 256, 0, st, w, wo, g.Cout, g.Cin, g.KH, g.KW,
+                  s, ry, rx, g.ph, g.pw, cy.dmin, cx.dmin, cy.n, cx.n, kind);
+      if (s == 1) {
+        AVSR_TRY(run_conv_raw(kind, false, dzo, wo, ones, ones + g.Cin, dx, c, st));
+      } else {
+        AVSR_TRY(run_conv_raw(kind, false, dzo, wo, ones, ones + g.Cin, sub, c, st));
+        AVSR_LAUNCH(ft_scatter_class_kernel, grid_1d((long)N * Hc * Wc * g.Cin), 256, 0, st, (const float*)sub, dx,
+                    N, g.H, g.W, g.Cin, s, ry, rx, Hc, Wc);
+      }
+    }
+  }
+  return AVSR_OK;
+}
+
+extern "C" size_t avsr_frontend_train_wgrad_workspace_bytes(int stem, int N, int T, int H, int W, int C_in, int C_out,
+                                                            int KH, int KW, int stride) {
+  ConvGeom g;
+  if (!ft_geom(stem, N, T, H, W, C_in, C_out, KH, KW, stride, &g)) return 0;
+  return ft_wgrad_ws(g);
+}
+
+extern "C" int avsr_frontend_train_conv_wgrad(const float* x, const float* dz, float* dw, int stem, int N, int T, int H,
+                                              int W, int C_in, int C_out, int KH, int KW, int stride, void* workspace,
+                                              size_t workspace_bytes, int precision, void* stream) {
+  AVSR_REQUIRE(ft_prec_ok(precision), "frontend train wgrad: bad precision %d", precision);
+  ConvGeom g;
+  AVSR_REQUIRE(ft_geom(stem, N, T, H, W, C_in, C_out, KH, KW, stride, &g),
+               "frontend train wgrad: unsupported shape stem=%d N=%d T=%d H=%d W=%d C_in=%d C_out=%d KH=%d KW=%d "
+               "stride=%d", stem, N, T, H, W, C_in, C_out, KH, KW, stride);
+  AVSR_REQUIRE(x && dz && dw && workspace, "NULL argument");
+  AVSR_REQUIRE_BYTES(ft_wgrad_ws(g), workspace_bytes, "frontend train wgrad workspace");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  float* part = reinterpret_cast<float*>(align_up(reinterpret_cast<uintptr_t>(workspace), 256));
+  const int Kw = cdiv(g.K, WG_T) * WG_T, splits = ft_wgrad_splits(g);
+  const long M = conv_rows(g);
+  const long per = ((M + splits - 1) / splits + WGT_PB - 1) / WGT_PB * WGT_PB;    // a multiple of both K-blocks
+  if (operand_kind(precision) == OP_F32) {
+    AVSR_LAUNCH(ft_wgrad_kernel, dim3(Kw / WG_T, g.Cout / WG_T, splits), 256, 0, st, x, dz, part, g, per, Kw);
+  } else {
+    AVSR_SET_MAX_SMEM(ft_wgrad_tc_kernel, WGT_SMEM);
+    AVSR_LAUNCH(ft_wgrad_tc_kernel, dim3(Kw / WG_T, g.Cout / WG_T, splits), 128, WGT_SMEM, st, x, dz, part, g, per, Kw);
+  }
+  const int taps = g.KT * g.KH * g.KW;
+  AVSR_LAUNCH(ft_wgrad_finish_kernel, grid_1d((long)g.Cout * g.Cin * taps), 256, 0, st, (const float*)part, dw, splits,
+              g.Cout, g.Cin, taps, Kw);
+  return AVSR_OK;
+}
+
+extern "C" int avsr_frontend_train_maxpool_fwd(const float* x, float* y, uint8_t* idx, int N, int Hi, int Wi, int C,
+                                               void* stream) {
+  AVSR_REQUIRE(N >= 0 && Hi >= 1 && Wi >= 1 && C >= 1, "frontend train maxpool: bad shape");
+  AVSR_REQUIRE(x && y && idx, "NULL argument");
+  const int Ho = (Hi - 1) / 2 + 1, Wo = (Wi - 1) / 2 + 1;
+  const long n = (long)N * Ho * Wo * C;
+  if (n == 0) return AVSR_OK;
+  AVSR_LAUNCH(ft_maxpool_fwd_kernel, grid_1d(n), 256, 0, reinterpret_cast<cudaStream_t>(stream), x, y, idx, N, Hi, Wi,
+              Ho, Wo, C);
+  return AVSR_OK;
+}
+
+extern "C" int avsr_frontend_train_maxpool_bwd(const float* dy, const uint8_t* idx, float* dx, int N, int Hi, int Wi,
+                                               int C, void* stream) {
+  AVSR_REQUIRE(N >= 0 && Hi >= 1 && Wi >= 1 && C >= 1, "frontend train maxpool: bad shape");
+  AVSR_REQUIRE(dy && idx && dx, "NULL argument");
+  const int Ho = (Hi - 1) / 2 + 1, Wo = (Wi - 1) / 2 + 1;
+  const long n = (long)N * Hi * Wi * C;
+  if (n == 0) return AVSR_OK;
+  AVSR_LAUNCH(ft_maxpool_bwd_kernel, grid_1d(n), 256, 0, reinterpret_cast<cudaStream_t>(stream), dy, idx, dx, N, Hi,
+              Wi, Ho, Wo, C);
+  return AVSR_OK;
+}
+
+extern "C" int avsr_frontend_train_mean_rows(const float* x, float* out, long G, int P, int C, void* stream) {
+  AVSR_REQUIRE(G >= 0 && P >= 1 && C >= 1, "frontend train mean: bad shape");
+  AVSR_REQUIRE(x && out, "NULL argument");
+  if (G == 0) return AVSR_OK;
+  AVSR_LAUNCH(mean_rows_kernel<float>, grid_1d(G * C), 256, 0, reinterpret_cast<cudaStream_t>(stream), x, out, G, P, C);
+  return AVSR_OK;
+}
+
+extern "C" int avsr_frontend_train_mean_rows_bwd(const float* dout, float* dx, long G, int P, int C, void* stream) {
+  AVSR_REQUIRE(G >= 0 && P >= 1 && C >= 1, "frontend train mean: bad shape");
+  AVSR_REQUIRE(dout && dx, "NULL argument");
+  if (G == 0) return AVSR_OK;
+  AVSR_LAUNCH(ft_mean_rows_bwd_kernel, grid_1d(G * P * C), 256, 0, reinterpret_cast<cudaStream_t>(stream), dout, dx, G,
+              P, C);
   return AVSR_OK;
 }

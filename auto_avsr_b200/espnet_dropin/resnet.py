@@ -3,7 +3,8 @@
 
 Every sub-module is a plain ``nn.Conv*`` / ``nn.BatchNorm*``, so Lightning's ``sync_batchnorm`` conversion still
 applies.  ``train()``: the sub-modules run as ordinary torch modules (autograd, running-statistics updates), exactly as
-in the reference.  ``eval()``: one ``avsr_frontend_forward`` call on prepared weights (auto_avsr_b200/frontend.py), reading
+in the reference -- or, with ``library_train = True`` and CUDA inputs, forward and backward run in libavsr_b200
+(auto_avsr_b200/frontend_train.py) on the same parameters and buffers.  ``eval()``: one ``avsr_frontend_forward`` call on prepared weights (auto_avsr_b200/frontend.py), reading
 the BatchNorm constants from whatever ``_BatchNorm`` module sits in each slot.  CPU tensors are refused: there is no CPU
 fallback for the eval path.  Only ``relu_type="swish"`` (the one ``E2E`` builds) is implemented."""
 from __future__ import annotations
@@ -105,6 +106,8 @@ class ResNet1D(nn.Module):
 class _LibraryFrontend(nn.Module):
     modality = ""
     precision: Optional[str] = None
+    #: train() forward and backward in the library instead of torch sub-modules (install_frontend(..., library_train=True))
+    library_train: bool = False
     _prep: Optional[PreparedFrontend] = None
 
     def conv_bn_pairs(self) -> List[Tuple[nn.Module, nn.Module]]:
@@ -115,6 +118,10 @@ class _LibraryFrontend(nn.Module):
             self._prep = PreparedFrontend()
         return frontend_forward(self._prep, self.modality, self.conv_bn_pairs(), xs_pad,
                                 self.precision or default_precision())
+
+    def _library_train_forward(self, xs_pad):
+        from ..frontend_train import frontend_train_forward
+        return frontend_train_forward(self, xs_pad)
 
 
 class Conv3dResNet(_LibraryFrontend):
@@ -141,6 +148,8 @@ class Conv3dResNet(_LibraryFrontend):
     def forward(self, xs_pad):
         if not self.training:
             return self._library_forward(xs_pad)
+        if self.library_train:
+            return self._library_train_forward(xs_pad)
         xs_pad = xs_pad.transpose(2, 1)
         B = xs_pad.size(0)
         xs_pad = self.frontend3D(xs_pad)
@@ -170,6 +179,8 @@ class Conv1dResNet(_LibraryFrontend):
     def forward(self, xs_pad):
         if not self.training:
             return self._library_forward(xs_pad)
+        if self.library_train:
+            return self._library_train_forward(xs_pad)
         T = xs_pad.size(1)
         xs_pad = xs_pad[:, : T // 640 * 640, :].transpose(1, 2)
         return self.trunk(xs_pad).transpose(1, 2)

@@ -106,12 +106,13 @@ def install_decoder(model):
     return model
 
 
-def install_frontend(model):
+def install_frontend(model, library_train: bool = False):
     """The ResNet front-end.  ``E2E`` builds it through ``video_resnet()`` / ``audio_resnet()`` (e2e_asr_conformer.py:26-29),
     so this re-homes ``model.frontend`` of an existing ``E2E`` onto the drop-in ``Conv3dResNet`` / ``Conv1dResNet``: the
     very same ``Parameter`` and buffer objects, each sub-module's train / eval mode and BatchNorm settings, and therefore
     an unchanged ``model.state_dict()``.  In eval the front-end then runs in libavsr_b200 from the raw clip or waveform;
-    in train it stays torch autograd."""
+    in train it stays torch autograd unless ``library_train`` is set, in which case the training forward and backward
+    on CUDA tensors run in libavsr_b200 too (auto_avsr_b200/frontend_train.py)."""
     from .espnet_dropin.resnet import Conv1dResNet, Conv3dResNet
 
     old = model.frontend
@@ -126,6 +127,7 @@ def install_frontend(model):
         if isinstance(mod, torch.nn.modules.batchnorm._BatchNorm):
             mod.eps, mod.momentum = src.eps, src.momentum
         mod.training = src.training
+    new.library_train = bool(library_train)
     model.frontend = new
     return model
 

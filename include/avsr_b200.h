@@ -498,6 +498,62 @@ int avsr_conv_bn_act(const float *x, const float *w, const float *scale, const f
                      int act, float *y, int N, int H, int W, int C_in, int C_out, int KH, int KW, int stride,
                      void *workspace, size_t workspace_bytes, int precision, void *stream);
 
+/* ---- ResNet front-ends, training (batch-statistics BatchNorm).  Building blocks that auto_avsr_b200/frontend_train.py
+ * chains per conv unit (conv -> BatchNorm -> [+ residual] -> [SiLU]); every tensor is DEVICE fp32, channels-last.
+ * `stem`: 0 a trunk conv, x (N, H, W, C_in), w (C_out, C_in, KH, KW), padding (K - 1) / 2, stride 1 or 2 (audio: H = KH =
+ * 1); 1 the video stem, x (N = B * T frames, H, W) with T frames per utterance, w (64, 1, 5, 7, 7); 2 the audio stem,
+ * x (N, W) samples with W a multiple of 640, w (64, 1, 80).  C_in, C_out and KH, KW, stride are ignored for the stems.
+ *
+ * avsr_frontend_train_conv_fwd: z (output pixels, C_out) = conv(x, w) in `precision` (TF32 / F16 on wgmma, FP32 on CUDA
+ * cores), and stats (3, C_out) fp64 = each channel's (count, mean, M2) over all output pixels, merged in a fixed order
+ * with Chan's formula. */
+size_t avsr_frontend_train_conv_workspace_bytes(int stem, int N, int T, int H, int W, int C_in, int C_out, int KH,
+                                                int KW, int stride, int precision);
+int avsr_frontend_train_conv_fwd(const float *x, const float *w, float *z, double *stats, int stem, int N, int T, int H,
+                                 int W, int C_in, int C_out, int KH, int KW, int stride, void *workspace,
+                                 size_t workspace_bytes, int precision, void *stream);
+/* stats: (ranks, 3, C) fp64, merged in rank order -> mean, invstd = 1 / sqrt(biased var + eps) (C fp32).  When
+ * running_mean / running_var are given they become (1 - factor) * old + factor * (mean, unbiased var). */
+int avsr_frontend_train_bn_finalize(const double *stats, int ranks, int C, double eps, double factor,
+                                    float *running_mean, float *running_var, float *mean, float *invstd, void *stream);
+/* y = [SiLU]((z - mean) * invstd * gamma + beta [+ resid]), (rows, C); resid may be NULL */
+int avsr_frontend_train_bn_act_fwd(const float *z, const float *mean, const float *invstd, const float *gamma,
+                                   const float *beta, const float *resid, int act, float *y, long rows, int C,
+                                   void *stream);
+/* Backward of bn_act_fwd.  bwd_sums: sums (2, C) = [sum ds, sum ds * x_hat] with ds = dL/d(BatchNorm output) (dy through
+ * the SiLU when act), summed in a fixed order.  bwd_dx: dz = gamma * invstd * (ds - inv_count * (sums[0] + x_hat *
+ * sums[1])) and, when dres is given, dres = ds (the residual's gradient). */
+size_t avsr_frontend_train_bn_bwd_workspace_bytes(long rows, int C);
+int avsr_frontend_train_bn_bwd_sums(const float *z, const float *dy, const float *mean, const float *invstd,
+                                    const float *gamma, const float *beta, const float *resid, int act, float *sums,
+                                    long rows, int C, void *workspace, size_t workspace_bytes, void *stream);
+int avsr_frontend_train_bn_bwd_dx(const float *z, const float *dy, const float *mean, const float *invstd,
+                                  const float *gamma, const float *beta, const float *resid, int act, const float *sums,
+                                  float inv_count, float *dz, float *dres, long rows, int C, void *stream);
+/* Input gradient of a trunk conv: dx (N, H, W, C_in) from dz (N, Ho, Wo, C_out), one stride-1 implicit GEMM per parity
+ * class of the input (TF32 / F16 on wgmma, FP32 on CUDA cores). */
+size_t avsr_frontend_train_dgrad_workspace_bytes(int N, int H, int W, int C_in, int C_out, int KH, int KW, int stride,
+                                                 int precision);
+int avsr_frontend_train_conv_dgrad(const float *dz, const float *w, float *dx, int N, int H, int W, int C_in, int C_out,
+                                   int KH, int KW, int stride, void *workspace, size_t workspace_bytes, int precision,
+                                   void *stream);
+/* Weight gradient dw (torch layout, like w) = sum over output pixels of dz x im2col(x): wgmma with TF32 operands
+ * (AVSR_PREC_TF32 / AVSR_PREC_F16) or fp32 on CUDA cores (AVSR_PREC_FP32); the pixel axis is split across the SMs and
+ * the partials are summed in a fixed order. */
+size_t avsr_frontend_train_wgrad_workspace_bytes(int stem, int N, int T, int H, int W, int C_in, int C_out, int KH,
+                                                 int KW, int stride);
+int avsr_frontend_train_conv_wgrad(const float *x, const float *dz, float *dw, int stem, int N, int T, int H, int W,
+                                   int C_in, int C_out, int KH, int KW, int stride, void *workspace,
+                                   size_t workspace_bytes, int precision, void *stream);
+/* MaxPool (1,3,3) / (1,2,2) / pad (0,1,1) on (N, Hi, Wi, C): idx (N, Ho, Wo, C) records the winner dy * 3 + dx, the first
+ * maximum in window scan order (a NaN wins); the backward gathers dy into each pixel from the windows that chose it. */
+int avsr_frontend_train_maxpool_fwd(const float *x, float *y, uint8_t *idx, int N, int Hi, int Wi, int C, void *stream);
+int avsr_frontend_train_maxpool_bwd(const float *dy, const uint8_t *idx, float *dx, int N, int Hi, int Wi, int C,
+                                    void *stream);
+/* out (G, C) = mean of each group of P consecutive rows of x (G * P, C); the backward broadcasts dout / P */
+int avsr_frontend_train_mean_rows(const float *x, float *out, long G, int P, int C, void *stream);
+int avsr_frontend_train_mean_rows_bwd(const float *dout, float *dx, long G, int P, int C, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
