@@ -84,6 +84,9 @@ class DecoderLayerParams(C.Structure):
 FRONTEND_VIDEO, FRONTEND_AUDIO = 0, 1
 FRONTEND_CONVS = 20
 FRONTEND_TAPS = 10
+#: avsr_linear_operands_split: fp32 partial planes of rows x n, and int tile counters, the caller provides
+SPLIT_PLANES = 8
+SPLIT_COUNTERS = 4096
 
 
 class ConvBnParams(C.Structure):
@@ -112,6 +115,7 @@ SIGNATURES = {
     "avsr_linear_workspace_bytes": (_Z, [_I, _I, _I, _I]),
     "avsr_linear": (_I, [_P, _P, _P, _P, _F, _I, _P, _I, _I, _I, _I, _P, _Z, _P]),
     "avsr_linear_operands": (_I, [_P, _P, _P, _P, _F, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "avsr_linear_operands_split": (_I, [_P, _P, _P, _P, _F, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
     "avsr_attention_workspace_bytes": (_Z, [_I, _I, _I]),
     "avsr_relpos_attention": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _Z, _I, _P]),
     "avsr_dwconv_bn_silu": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _Z, _P]),

@@ -773,6 +773,17 @@ int avsr_linear_operands(const void* x_op, const void* w_op, const float* bias, 
                   reinterpret_cast<cudaStream_t>(stream));
 }
 
+int avsr_linear_operands_split(const void* x_op, const void* w_op, const float* bias, const float* resid, float alpha,
+                               void* y, int rows, int n, int k, int relu, int y_is_operand, int precision,
+                               float* partial, int* counters, void* stream) {
+  AVSR_REQUIRE(x_op && w_op && y && partial && counters, "NULL argument");
+  AVSR_REQUIRE(valid_precision(precision), "bad precision %d", precision);
+  EpiParams e = epi_linear(rows, n, bias, y, resid, alpha, relu, (y_is_operand && precision != AVSR_PREC_FP32) ? 1 : 0);
+  e.partial = partial;
+  e.counters = counters;
+  return run_gemm(precision, EPI_LINEAR, x_op, w_op, rows, n, k, e, reinterpret_cast<cudaStream_t>(stream));
+}
+
 // (B,T,H*64) -> (B,H,T,64) with optional per-channel bias add; or -> (B,H,64,Tp) when transpose != 0
 __global__ void split_heads_kernel(const float* __restrict__ src, const float* __restrict__ bias, void* __restrict__ dst,
                                    int B, int T, int H, int Tp, int transpose, int kind) {

@@ -16,6 +16,8 @@
 // Operand storage (template TOp): float = TF32 (8 elements per MMA-K) or __half (16 per MMA-K; same 10-bit mantissa,
 // half the bytes, twice the rate).  Out-of-bounds rows of edge tiles are zero-filled by TMA and masked in the
 // epilogue.  The tile width is chosen per problem by a small cost model (bytes through L2 vs tensor-pipe time).
+#include <cstring>
+
 #include "common.cuh"
 #include "epilogue.cuh"
 #include "gemm_schedule.cuh"
@@ -117,7 +119,7 @@ template <> struct OpTraits<__half> {
 template <int MODE, int BN, typename TOp, int CM, int CN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int K, int tiles_m,
-               int tiles_n, int splits, EpiParams ep) {
+               int tiles_n, int splits, int streamk, EpiParams ep) {
   // PERSISTENT: cluster c processes cluster tiles c, c + clusters, ... (n fastest, so concurrently running CTAs share
   // A rows in L2; gemm_schedule.cuh).  The TMA ring never drains between tiles: the producer fills it in item order,
   // and the consumer warpgroups take turns on the items (even / odd), so stage ownership follows the item index.
@@ -150,11 +152,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nkb = K / KE;
-  // split-K (LINEAR into the residual stream only, 1 x 1 clusters): work item = (tile, K-slice); slice-major order so
-  // that CTAs running at the same time reduce into different tiles.
+  // this CTA's pieces (gemm_schedule.cuh): the cluster / equal-slice list, or with `streamk` (LINEAR into the residual
+  // stream only, 1 x 1 clusters) an equal share of the (tile, k-block) steps of all gridDim.x CTAs
+  const bool sk = CS == 1 && streamk != 0;
   const int crank = CS > 1 ? (int)cluster_ctarank() : 0;
   const int cluster_id = blockIdx.x / CS, clusters = gridDim.x / CS;
-  const int total_items = tc_cluster_items(tiles_m, tiles_n, splits, CM, CN);
+  const int npieces = sk ? tc_streamk_pieces(blockIdx.x, gridDim.x, tiles_m * tiles_n, nkb)
+                         : tc_slice_pieces(cluster_id, clusters, tiles_m, tiles_n, splits, CM, CN);
+  auto piece_at = [&](int j) {
+    return sk ? tc_streamk_piece(j, blockIdx.x, gridDim.x, tiles_n, tiles_m * tiles_n, nkb)
+              : tc_slice_piece(j, cluster_id, clusters, crank, tiles_m, tiles_n, nkb, splits, CM, CN);
+  };
 
   pdl_launch_dependents();
   AVSR_TSPAN_OPEN(400 + MODE, (unsigned)BN);
@@ -180,11 +188,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       for (int j = 0; j < CN; ++j) a_mask |= (uint16_t)(1u << (cm + CM * j));
       for (int i = 0; i < CM; ++i) b_mask |= (uint16_t)(1u << (i + CM * cn));
       int it = 0;                                   // running k-block counter across tiles
-      for (int item = cluster_id; item < total_items; item += clusters) {
-        const TcWork w = tc_work_item(item, crank, tiles_m, tiles_n, CM, CN);
+      for (int j = 0; j < npieces; ++j) {
+        const TcPiece w = piece_at(j);
         const int m0 = w.tm * TC_BM, n0 = w.tn * BN;
-        const int kb0 = w.split * nkb / splits, kb1 = (w.split + 1) * nkb / splits;
-        for (int kb = kb0; kb < kb1; ++kb, ++it) {
+        for (int kb = w.kb0; kb < w.kb1; ++kb, ++it) {
           const int s = it % S;
           const uint32_t ph = (it / S) & 1;
           mbar_wait(empty_bar(s), ph ^ 1);
@@ -230,12 +237,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     auto pass_turn = [&](int phase) { __syncwarp(); if (lane == 0) mbar_arrive(order_bar(phase, wg ^ 1)); };
     int it = 0, turn = 0;
 #pragma unroll 1
-    for (int item = cluster_id, idx = 0; item < total_items; item += clusters, ++idx) {
-    const TcWork w = tc_work_item(item, crank, tiles_m, tiles_n, CM, CN);
-    const int split = w.split, tile = w.tm * tiles_n + w.tn;
+    for (int idx = 0; idx < npieces; ++idx) {
+    const TcPiece w = piece_at(idx);
+    const int tile = w.tm * tiles_n + w.tn;
     const int m0 = w.tm * TC_BM, n0 = w.tn * BN;
-    const int kb0 = split * nkb / splits, kb1 = (split + 1) * nkb / splits;
-    if ((idx & 1) != wg) { it += kb1 - kb0; continue; }   // the other warpgroup's item: skip its stages
+    const int kb0 = w.kb0, kb1 = w.kb1;
+    if ((idx & 1) != wg) { it += kb1 - kb0; continue; }   // the other warpgroup's piece: skip its stages
     // warpgroup 0 goes first: its first wait is on the parity of the phase before phase 0, which passes at once
     const uint32_t par = (uint32_t)(turn++ & 1) ^ (wg == 0 ? 1u : 0u);
     // the first wgmma of the item overwrites the accumulator; zeroing it here only tells the compiler that the previous
@@ -269,6 +276,22 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     mbar_wait(order_bar(1, wg), par);              // the other warpgroup's epilogue is done with s_acc / s_vec
     if (!w.valid) { pass_turn(1); continue; }      // past the matrix edge: took part in the loads, stores nothing
     // ---- accumulator -> shared memory (fp32 rows), the tile's per-column vectors next to it
+    // fp32 LINEAR into a residual, whole tile: the warp's residual slab is loaded 64 columns at a time, the first 64
+    // once the accumulator registers are free, the next while the previous ones are stored (lane: rows it8 * 4 + pr of
+    // the slab, columns 32 * cc + 4 * pc of the tile; every load of an element precedes its store by the same thread,
+    // so resid may be out).  One round trip per 64 columns instead of one per 32.
+    constexpr int RC = BN / 32 < 2 ? BN / 32 : 2;             // 32-column chunks of residual in registers
+    float4 res[RC][8];
+    const bool res_tile = MODE == EPI_LINEAR && !ep.round_out && w.npieces == 1 && ep.resid != nullptr;
+    auto load_res = [&](int cc, float4* dst) {
+      const int n = n0 + 32 * cc + pc * 4;
+#pragma unroll
+      for (int it8 = 0; it8 < 8; ++it8) {
+        const int m = m0 + q * 32 + it8 * 4 + pr;
+        dst[it8] = (m < ep.M && n < ep.N) ? *reinterpret_cast<const float4*>(ep.resid + (long)m * ep.ldo + n)
+                                          : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+    };
     {
       const int r = (warp & 3) * 16 + (lane >> 2);
       const int c = 2 * (lane & 3);
@@ -280,6 +303,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         for (int j = 0; j < BN / 8; ++j) {
           *reinterpret_cast<float2*>(sh + 8 * j) = make_float2(ah[4 * j], ah[4 * j + 1]);
           *reinterpret_cast<float2*>(sh + 8 * LD + 8 * j) = make_float2(ah[4 * j + 2], ah[4 * j + 3]);
+        }
+      }
+      if constexpr (MODE == EPI_LINEAR) {
+        if (res_tile) {
+#pragma unroll
+          for (int cc = 0; cc < RC; ++cc) load_res(cc, res[cc]);
         }
       }
       float* s_bias = s_vec;
@@ -319,56 +348,41 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           __syncwarp();
         }
       } else if constexpr (MODE == EPI_LINEAR) {
-        if (!ep.round_out) {                                 // fp32 destination (+ residual)
-#pragma unroll 1
-          for (int c = 0; c < BN; c += 32) {
-            uint8_t* stg = stg_at(c);
-            float v[32];
-            acc_ld32(c, v);
-            const float* sb = s_vec + c;
-            if (splits == 1) {
+        if (!ep.round_out && w.npieces == 1) {              // fp32 destination (+ residual), whole tile
+          // the lane reads its output pieces straight from the accumulator rows (the layout emit reads)
 #pragma unroll
-              for (int j = 0; j < 32; ++j) { v[j] += sb[j]; if (ep.relu) v[j] = fmaxf(v[j], 0.f); }
-            }
-            stage_write_f32(stg, RB, lane, v, false);
-            __syncwarp();
-            const int n = n0 + c + pc * 4;
-            if (splits > 1) {
-              // split-K: this K-slice's raw partial tile goes to the fp32 workspace (coalesced 16-byte stores); the
-              // last CTA to arrive for this tile sums the slices in fixed order (below) -> deterministic
-              float* part = ep.partial + (long)split * ep.M * ep.ldo;
-#pragma unroll
-              for (int it8 = 0; it8 < 8; ++it8) {
-                const int m = mw + it8 * 4 + pr;
-                const uint4 pay = stage_read(stg, RB, it8, lane);
-                if (m < ep.M && n < ep.N) *reinterpret_cast<uint4*>(part + (long)m * ep.ldo + n) = pay;
-              }
-            } else {
-            // residual pieces first (8 independent coalesced loads in flight), then combine + store: a load may not
-            // be hoisted above a store by the compiler (possible aliasing), so the order is made explicit here
-            float4 r[8];
-            if (ep.resid) {
-#pragma unroll
-              for (int it8 = 0; it8 < 8; ++it8) {
-                const int m = mw + it8 * 4 + pr;
-                r[it8] = (m < ep.M && n < ep.N) ? *reinterpret_cast<const float4*>(ep.resid + (long)m * ep.ldo + n)
-                                                : make_float4(0.f, 0.f, 0.f, 0.f);
-              }
-            }
+          for (int cc = 0; cc < BN / 32; ++cc) {
+            const int c = 32 * cc, n = n0 + c + pc * 4;
+            const float4 bv = *reinterpret_cast<const float4*>(s_vec + c + pc * 4);
 #pragma unroll
             for (int it8 = 0; it8 < 8; ++it8) {
               const int m = mw + it8 * 4 + pr;
-              const uint4 pay = stage_read(stg, RB, it8, lane);
-              float4 o = *reinterpret_cast<const float4*>(&pay);
-              if (ep.resid) {
-                o.x = r[it8].x + ep.alpha * o.x; o.y = r[it8].y + ep.alpha * o.y;
-                o.z = r[it8].z + ep.alpha * o.z; o.w = r[it8].w + ep.alpha * o.w;
+              float4 o = *reinterpret_cast<const float4*>(s_acc + (q * 32 + it8 * 4 + pr) * LD + c + pc * 4);
+              o.x += bv.x; o.y += bv.y; o.z += bv.z; o.w += bv.w;
+              if (ep.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
+              if (res_tile) {
+                const float4 r = res[cc % RC][it8];
+                o.x = r.x + ep.alpha * o.x; o.y = r.y + ep.alpha * o.y;
+                o.z = r.z + ep.alpha * o.z; o.w = r.w + ep.alpha * o.w;
               }
               if (m < ep.M && n < ep.N)
                 *reinterpret_cast<float4*>(reinterpret_cast<float*>(ep.out) + (long)m * ep.ldo + n) = o;
             }
+            if (res_tile && cc + RC < BN / 32) load_res(cc + RC, res[cc % RC]);
+          }
+        } else if (!ep.round_out) {                          // fp32 partial of a piece of a shared tile
+          // its raw partial tile goes to plane `piece` of the fp32 workspace (coalesced 16-byte stores); the last CTA
+          // to arrive for this tile sums the pieces in fixed order (below) -> deterministic
+          float* part = ep.partial + (long)w.piece * ep.M * ep.ldo;
+#pragma unroll 1
+          for (int c = 0; c < BN; c += 32) {
+            const int n = n0 + c + pc * 4;
+#pragma unroll
+            for (int it8 = 0; it8 < 8; ++it8) {
+              const int m = mw + it8 * 4 + pr;
+              const float4 pay = *reinterpret_cast<const float4*>(s_acc + (q * 32 + it8 * 4 + pr) * LD + c + pc * 4);
+              if (m < ep.M && n < ep.N) *reinterpret_cast<float4*>(part + (long)m * ep.ldo + n) = pay;
             }
-            __syncwarp();
           }
         } else {                                             // operand-typed destination (FFN hidden)
 #pragma unroll 1
@@ -474,20 +488,22 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     }
     if constexpr (MODE == EPI_LINEAR) {
-      if (splits > 1) {
-        // ---- deterministic split-K fix-up ("last block reduces"): publish the partial, count arrivals per tile ----
+      if (w.npieces > 1) {
+        // ---- deterministic fix-up ("last block reduces"): publish the partial, count arrivals per tile.  No CTA
+        // waits for another: the one that arrives last finishes the tile, the others are done.
         __threadfence();
         wg_sync();
         if ((threadIdx.x & 127) == 0) {
           const int old = atomicAdd(ep.counters + tile, 1);
-          const int last = (old == splits - 1);
-          if (last) ep.counters[tile] = 0;                 // every slice has arrived: re-arm for the next launch
+          const int last = (old == w.npieces - 1);
+          if (last) ep.counters[tile] = 0;                 // every piece has arrived: re-arm for the next launch
           *s_flag = last;
         }
         wg_sync();
         if (*s_flag) {
-          __threadfence();                                 // acquire: the other slices' partial tiles are visible
+          __threadfence();                                 // acquire: the other pieces' partial tiles are visible
           const int mw = m0 + q * 32;
+          const float* own = s_acc + (q * 32 + pr) * LD + pc * 4;   // this piece's partial, still in shared memory
 #pragma unroll 1
           for (int c = 0; c < BN; c += 32) {
             const int n = n0 + c + pc * 4;
@@ -497,12 +513,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             bool ok[8];
 #pragma unroll
             for (int it8 = 0; it8 < 8; ++it8) { a[it8] = bv; ok[it8] = (mw + it8 * 4 + pr < ep.M) && (n < ep.N); }
-            for (int sp = 0; sp < splits; ++sp) {        // fixed order: slice 0, 1, ... regardless of arrival order
+            for (int sp = 0; sp < w.npieces; ++sp) {     // fixed order: piece 0, 1, ... regardless of arrival order
               const float* part = ep.partial + (long)sp * ep.M * ep.ldo;
+              if (sp == w.piece) {
 #pragma unroll
-              for (int it8 = 0; it8 < 8; ++it8)
-                t4[it8] = ok[it8] ? __ldcg(reinterpret_cast<const float4*>(part + (long)(mw + it8 * 4 + pr) * ep.ldo + n))
-                                  : make_float4(0.f, 0.f, 0.f, 0.f);
+                for (int it8 = 0; it8 < 8; ++it8) t4[it8] = *reinterpret_cast<const float4*>(own + it8 * 4 * LD + c);
+              } else {
+#pragma unroll
+                for (int it8 = 0; it8 < 8; ++it8)
+                  t4[it8] = ok[it8] ? __ldcg(reinterpret_cast<const float4*>(part + (long)(mw + it8 * 4 + pr) * ep.ldo + n))
+                                    : make_float4(0.f, 0.f, 0.f, 0.f);
+              }
 #pragma unroll
               for (int it8 = 0; it8 < 8; ++it8) { a[it8].x += t4[it8].x; a[it8].y += t4[it8].y; a[it8].z += t4[it8].z; a[it8].w += t4[it8].w; }
             }
@@ -558,8 +579,8 @@ static int max_active_clusters(Kernel kernel, int cs, int smem) {
 }
 
 template <int MODE, int BN, typename TOp, int CM, int CN>
-static int launch_tc(const void* A, const void* Bw, int M, int N, int K, int splits, const EpiParams& ep,
-                     cudaStream_t st) {
+static int launch_tc(const void* A, const void* Bw, int M, int N, int K, int splits, bool streamk,
+                     const EpiParams& ep, cudaStream_t st) {
   using Cfg = TcCfg<BN>;
   constexpr int CS = CM * CN;
   auto kernel = gemm_tc_kernel<MODE, BN, TOp, CM, CN>;
@@ -568,7 +589,15 @@ static int launch_tc(const void* A, const void* Bw, int M, int N, int K, int spl
   AVSR_TRY(make_tmap_2d(&tmB, Bw, (uint64_t)N, (uint64_t)K, (uint64_t)K, BN / CM, (int)sizeof(TOp)));
   AVSR_SET_MAX_SMEM(kernel, Cfg::kSmem);
   const int tiles_m = cdiv(M, TC_BM), tiles_n = cdiv(N, BN);
-  if (CS > 1 || splits > kMaxSplits || tiles_m * tiles_n > kSplitCounters) splits = 1;   // caller's workspace contract
+  if (CS > 1 || splits > kMaxSplits || tiles_m * tiles_n > kSplitCounters) {   // caller's workspace contract
+    splits = 1;
+    streamk = false;
+  }
+  if (streamk) {
+    const int grid = tc_streamk_ctas(num_sms(), tiles_m * tiles_n, K / OpTraits<TOp>::kElemsPerBlock);
+    AVSR_LAUNCH_CLUSTER(kernel, grid, TC_THREADS, Cfg::kSmem, st, 1, tmA, tmB, K, tiles_m, tiles_n, 1, 1, ep);
+    return AVSR_OK;
+  }
   const int total = tc_cluster_items(tiles_m, tiles_n, splits, CM, CN);
   int slots = num_sms();
   if constexpr (CS > 1) {
@@ -580,7 +609,7 @@ static int launch_tc(const void* A, const void* Bw, int M, int N, int K, int spl
     slots = active;
   }
   const int grid = (total < slots ? total : slots) * CS;
-  AVSR_LAUNCH_CLUSTER(kernel, grid, TC_THREADS, Cfg::kSmem, st, CS, tmA, tmB, K, tiles_m, tiles_n, splits, ep);
+  AVSR_LAUNCH_CLUSTER(kernel, grid, TC_THREADS, Cfg::kSmem, st, CS, tmA, tmB, K, tiles_m, tiles_n, splits, 0, ep);
   return AVSR_OK;
 }
 
@@ -588,38 +617,56 @@ static int launch_tc(const void* A, const void* Bw, int M, int N, int K, int spl
 // Cost model (SM cycles) of one GEMM on persistent CTAs, one per SM: the busier of the tensor pipe (dense wgmma rate
 // per SM) and operand ingest (bytes the busiest SM pulls through L2, at an assumed ~64 B/cycle), plus one epilogue:
 // the consumer warpgroups alternate items, so every epilogue but the SM's last runs under the other warpgroup's main
-// loop.  Split-K (only for GEMMs that accumulate into the fp32 residual stream) spreads a long K over more SMs.
+// loop.  Split-K and stream-K (only for GEMMs that accumulate into the fp32 residual stream) spread a long K over more
+// SMs; stream-K is charged what it measured (below).
 // It picks 1 x 1 clusters only.  Multicast clusters cut the modelled L2 -> SM bytes by 25 % (2x1, 1x2) or 50 % (2x2)
 // but measured about 1.8x slower at the S2 shapes on an H100 80GB HBM3 at 400 W (FFN w_1 1600x3072x768: 22.7 us at
 // 1x1, 42.6 us at 2x1): the main loop waits on load latency, not L2 bandwidth (DESIGN.md section 4); clusters stay
 // reachable through AVSR_B200_TILE for sweeps.
-struct TileChoice { int bn, splits, cm, cn; };
+struct TileChoice { int bn, splits, cm, cn; bool streamk; };
 static const int kTileWidths[] = {64, 128};
+// Stream-K as measured on an H100 80GB HBM3 at 700 W (1980 MHz), against the data-parallel schedule at the encoder's
+// residual shapes (DESIGN.md section 4): the data-parallel w_2 main loop already pulls ~9 TB/s from L2 on its 78
+// SMs, so on 132 SMs a k-block costs about 3x the modelled per-SM time (FFN w_2 1600x768x3072 f16: 28.4 k-blocks per
+// SM in 41.7 us), and a launch carries ~20 us of partial-tile traffic and fix-up on its critical path (out
+// 1600x768x768: 7.1 k-blocks per SM in 24.5 us).  So it stays a candidate for long-K GEMMs with few tiles, and the
+// encoder's GEMMs keep the data-parallel schedule.
+constexpr double kStreamKStepFactor = 3.0;
+constexpr double kStreamKFixed = 40000.0;
 
-static TileChoice choose_tile(int mode, int M, int N, int K, int esz, bool operand_dest, bool can_split) {
+static TileChoice choose_tile(int mode, int M, int N, int K, int esz, bool operand_dest, bool can_split,
+                              bool can_streamk) {
   const double mac_per_cycle = esz == 2 ? 2048.0 : 1024.0;   // per SM, dense f16 / tf32
   const double ingest = 64.0;                                // operand bytes per cycle per SM
   const int nkb = K / (128 / esz);
   const int sms = num_sms();
   double best = 1e30;
-  TileChoice pick{128, 1, 1, 1};
+  TileChoice pick{128, 1, 1, 1, false};
   for (const int bn : kTileWidths) {
     if (mode == EPI_GLU && bn % 128 != 0) continue;
     if (bn == 64 && esz == 2 && (mode != EPI_LINEAR || operand_dest)) continue;   // needs 64-column row segments
     if (bn > 64 && N <= bn / 2) continue;                                          // mostly empty tile
     const long tiles = (long)cdiv(M, 128) * cdiv(N, bn);
+    const double t_epi = 128.0 * bn * 10.0 / 128.0 * 4.0;                          // the SM's last epilogue
+    // the busiest SM's main loop over `steps` k-blocks
+    auto t_main = [&](long steps) {
+      const double t_mma = steps * 128.0 * bn * (128 / esz) / mac_per_cycle;
+      const double t_in = steps * (128.0 + bn) * 128.0 / ingest;
+      return t_mma > t_in ? t_mma : t_in;
+    };
     for (int splits = 1; splits <= (can_split ? kMaxSplits : 1); ++splits) {
       if (splits > nkb) break;
-      const long items = tiles * splits;
-      const long per_sm = (items + sms - 1) / sms;
-      const double kfrac = (double)((nkb + splits - 1) / splits) * (128 / esz);    // K elements of the longest slice
-      const double t_mma = per_sm * 128.0 * bn * kfrac / mac_per_cycle;
-      const double t_in = per_sm * (128.0 + bn) * kfrac * esz / ingest;
-      const double t_epi = 128.0 * bn * 10.0 / 128.0 * 4.0;                        // the last item's epilogue
+      const long per_sm = (tiles * splits + sms - 1) / sms;
       // fix-up: the last arriver re-reads `splits` fp32 partial tiles through the same port
       const double t_red = splits > 1 ? (double)splits * 128.0 * bn * 4.0 / ingest : 0.0;
-      const double est = (t_mma > t_in ? t_mma : t_in) + t_epi + t_red + 4000.0;
-      if (est < best) { best = est; pick = TileChoice{bn, splits, 1, 1}; }
+      const double est = t_main(per_sm * ((nkb + splits - 1) / splits)) + t_epi + t_red + 4000.0;
+      if (est < best) { best = est; pick = TileChoice{bn, splits, 1, 1, false}; }
+    }
+    if (can_streamk && tiles <= kSplitCounters) {
+      // stream-K: equal shares of the tiles * nkb steps at the measured rate
+      const long ctas = tc_streamk_ctas(sms, (int)tiles, nkb);
+      const double est = kStreamKStepFactor * t_main((tiles * nkb + ctas - 1) / ctas) + t_epi + kStreamKFixed;
+      if (est < best) { best = est; pick = TileChoice{bn, 1, 1, 1, true}; }
     }
   }
   return pick;
@@ -628,10 +675,10 @@ static TileChoice choose_tile(int mode, int M, int N, int K, int esz, bool opera
 template <int MODE, int BN, typename TOp>
 static int dispatch_cluster(TileChoice t, const void* A, const void* Bw, int M, int N, int K, const EpiParams& ep,
                             cudaStream_t st) {
-  if (t.cm == 1 && t.cn == 1) return launch_tc<MODE, BN, TOp, 1, 1>(A, Bw, M, N, K, t.splits, ep, st);
-  if (t.cm == 2 && t.cn == 1) return launch_tc<MODE, BN, TOp, 2, 1>(A, Bw, M, N, K, 1, ep, st);
-  if (t.cm == 1 && t.cn == 2) return launch_tc<MODE, BN, TOp, 1, 2>(A, Bw, M, N, K, 1, ep, st);
-  if (t.cm == 2 && t.cn == 2) return launch_tc<MODE, BN, TOp, 2, 2>(A, Bw, M, N, K, 1, ep, st);
+  if (t.cm == 1 && t.cn == 1) return launch_tc<MODE, BN, TOp, 1, 1>(A, Bw, M, N, K, t.splits, t.streamk, ep, st);
+  if (t.cm == 2 && t.cn == 1) return launch_tc<MODE, BN, TOp, 2, 1>(A, Bw, M, N, K, 1, false, ep, st);
+  if (t.cm == 1 && t.cn == 2) return launch_tc<MODE, BN, TOp, 1, 2>(A, Bw, M, N, K, 1, false, ep, st);
+  if (t.cm == 2 && t.cn == 2) return launch_tc<MODE, BN, TOp, 2, 2>(A, Bw, M, N, K, 1, false, ep, st);
   set_error("gemm_tc: no kernel for cluster %dx%d", t.cm, t.cn);
   return AVSR_E_INVALID;
 }
@@ -651,15 +698,19 @@ template <typename TOp>
 static int dispatch_mode(int mode, const void* A, const void* Bw, int M, int N, int K, const EpiParams& ep,
                          cudaStream_t st) {
   const bool operand_dest = mode != EPI_GLU && (mode != EPI_LINEAR || ep.round_out != 0);
-  // split-K adds partial sums into the destination: only when the destination IS the residual it accumulates into.
-  // Split-K needs the caller's fp32 workspace + zeroed tile counters (EpiParams::partial / counters); the slices
-  // are summed in fixed order by the last-arriving CTA, so the result does not depend on scheduling.  Opt-in
-  // (AVSR_B200_SPLITK=1): the fix-up re-reads `splits` fp32 tiles as a serial tail.
+  // split-K and stream-K add partial sums into the destination: only when the destination IS the residual it
+  // accumulates into.  Both need the caller's fp32 workspace + zeroed tile counters (EpiParams::partial / counters);
+  // the pieces of a tile are summed in fixed order by the last-arriving CTA, so the result does not depend on
+  // scheduling.  Stream-K is a candidate of the cost model whenever the workspace is there; equal-slice split-K is
+  // opt-in (AVSR_B200_SPLITK=1).
+  const bool can_streamk = mode == EPI_LINEAR && !ep.round_out && !ep.relu && ep.resid != nullptr &&
+                           ep.partial != nullptr && ep.counters != nullptr;
   static const bool allow_split = [] { const char* e = getenv("AVSR_B200_SPLITK"); return e && e[0] == '1'; }();
-  const bool can_split = allow_split && mode == EPI_LINEAR && !ep.round_out && !ep.relu && ep.resid != nullptr &&
-                         ep.partial != nullptr && ep.counters != nullptr;
-  TileChoice t = choose_tile(mode, M, N, K, (int)sizeof(TOp), operand_dest, can_split);
-  if (const char* force = getenv("AVSR_B200_TILE")) {        // "BN[,SPLITS[,CMxCN]]" -- tuning / profiling aid
+  const bool can_split = allow_split && can_streamk;
+  TileChoice t = choose_tile(mode, M, N, K, (int)sizeof(TOp), operand_dest, can_split, can_streamk);
+  // "BN[,SPLITS[,CMxCN]]" runs exactly that tile, split and cluster shape; "BN,sk" runs stream-K at that tile width
+  // where the GEMM can take it (tuning / profiling aid)
+  if (const char* force = getenv("AVSR_B200_TILE")) {
     int bn = 0, sp = 1, cm = 1, cn = 1;
     const int got = sscanf(force, "%d,%d,%dx%d", &bn, &sp, &cm, &cn);
     if (got >= 1 && (bn == 64 || bn == 128) && (mode != EPI_GLU || bn % 128 == 0) &&
@@ -667,7 +718,9 @@ static int dispatch_mode(int mode, const void* A, const void* Bw, int M, int N, 
       if (got < 4 || cm < 1 || cm > 2 || cn < 1 || cn > 2) cm = cn = 1;
       if (got < 2 || !can_split || sp < 1 || cm * cn > 1) sp = 1;
       const int nkb = K / (128 / (int)sizeof(TOp));
-      t = TileChoice{bn, sp > nkb ? nkb : sp, cm, cn};
+      const char* comma = strchr(force, ',');
+      const bool sk = got == 1 && comma && strcmp(comma + 1, "sk") == 0 && can_streamk;
+      t = TileChoice{bn, sp > nkb ? nkb : sp, cm, cn, sk};
     }
   }
   AVSR_REQUIRE(mode == EPI_VT || N % 8 == 0, "gemm_tc: N=%d must be a multiple of 8", N);

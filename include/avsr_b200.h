@@ -150,6 +150,12 @@ int avsr_linear(const float *x, const float *w, const float *bias, const float *
  * kernel in isolation (roofline), not by the modules. */
 int avsr_linear_operands(const void *x_op, const void *w_op, const float *bias, const float *resid, float alpha,
                          void *y, int rows, int n, int k, int relu, int y_is_operand, int precision, void *stream);
+/* The same with the split workspace the encoder gives its residual-stream GEMMs, so that one GEMM takes the schedule
+ * decision it takes inside the forward (stream-K or split-K when y is fp32, resid != NULL and relu == 0):
+ * partial: 8 x rows x n fp32 scratch; counters: 4096 ints, zero on entry (the kernel leaves them zero again). */
+int avsr_linear_operands_split(const void *x_op, const void *w_op, const float *bias, const float *resid,
+                               float alpha, void *y, int rows, int n, int k, int relu, int y_is_operand,
+                               int precision, float *partial, int *counters, void *stream);
 
 /* RelPositionMultiHeadedAttention core (transformer/attention.py:174-189 + :59-82), d_k = 64:
  *   scores[b,h,i,j] = ((q_i+u_h).k_j + (q_i+v_h).p_h[rel=i-j]) / 8, key mask j >= lengths[b],

@@ -4,7 +4,8 @@
     python scripts/bench_gemm_shapes.py [--lib NAME=PATH ...] [--tiles auto 128,1,2x1 ...] [--precision f16]
 
 Each (build, tile) runs in its own process (AVSR_B200_LIB selects the build, AVSR_B200_TILE = "BN[,SPLITS[,CMxCN]]"
-the tile; "auto" is the cost model's pick).  Every shape replays a CUDA graph of 24 launches over 24 distinct weight
+or "BN,sk" (stream-K) the tile; "auto" is the cost model's pick).  The residual shapes (w_2, out / pw2) go through
+avsr_linear_operands_split with the encoder's split workspace, so they take the schedule they take in the forward.  Every shape replays a CUDA graph of 24 launches over 24 distinct weight
 matrices, as bench.py's roofline does, and reports us per launch, TFLOP/s, the modelled L2 -> SM operand bytes of the
 tile and cluster shape (each CTA pulls 1/CN of its A tile and 1/CM of its weight tile) and the implied GB/s.  QKV and
 pw1 run here as plain LINEAR GEMMs with operand-typed output at the QKV / pw1 shapes; their scatter and GLU epilogues
@@ -35,11 +36,18 @@ for name, M, N, K, relu, opdest, resid in %(shapes)r:
     b = torch.zeros(N, device=dev)
     y = torch.zeros(M, N, device=dev, dtype=tdt if opdest else torch.float32)
     r = y if resid else None
+    # the residual GEMMs get the encoder's split workspace, so they take the schedule they take in the forward
+    part = torch.empty(_cabi.SPLIT_PLANES * M * N, device=dev)
+    cnt = torch.zeros(_cabi.SPLIT_COUNTERS, device=dev, dtype=torch.int32)
     st = torch.cuda.current_stream(dev).cuda_stream
     def go(w):
-        _cabi.check(_cabi.lib.avsr_linear_operands(x.data_ptr(), w.data_ptr(), b.data_ptr(),
-                                                   None if r is None else r.data_ptr(), 0.5, y.data_ptr(), M, N, K,
-                                                   relu, opdest, PRECISIONS[prec], st))
+        if resid:
+            _cabi.check(_cabi.lib.avsr_linear_operands_split(x.data_ptr(), w.data_ptr(), b.data_ptr(), r.data_ptr(),
+                                                             0.5, y.data_ptr(), M, N, K, relu, opdest,
+                                                             PRECISIONS[prec], part.data_ptr(), cnt.data_ptr(), st))
+        else:
+            _cabi.check(_cabi.lib.avsr_linear_operands(x.data_ptr(), w.data_ptr(), b.data_ptr(), None, 0.5,
+                                                       y.data_ptr(), M, N, K, relu, opdest, PRECISIONS[prec], st))
     for w in ws[:3]: go(w)
     torch.cuda.synchronize()
     graph = torch.cuda.CUDAGraph()
