@@ -28,14 +28,10 @@ dev = torch.device("cuda:0")
 torch.backends.cudnn.allow_tf32 = False
 torch.backends.cuda.matmul.allow_tf32 = False
 # relative bounds, about 4x the largest errors observed on an H100 80GB HBM3
-# (per unit: fp32 3.0e-6, tf32 / f16 6.7e-4; whole front-end: fp32 1.1e-5, tf32 / f16 7.8e-3, the video stem's
-# gradients 9.1e-2 in tf32 / f16)
+# (per unit: fp32 3.0e-6, tf32 / f16 6.7e-4; whole front-end: fp32 1.1e-5, tf32 / f16 7.5e-3, the video stem's
+# gradients 5.1e-3 with the max-pool winners pinned)
 TOL_UNIT = {{"fp32": 1.2e-5, "tf32": 2.7e-3, "f16": 2.7e-3}}
 TOL_FE = {{"fp32": 5e-5, "tf32": 3e-2, "f16": 3e-2}}
-# the video stem's gradients sit behind the max-pool: with 11-bit operands a near-tie window can pick another winner
-# than float64 does and route its gradient one pixel over, which the stem's weight gradient (a sum with cancellation)
-# shows most
-TOL_STEM = {{"fp32": 5e-5, "tf32": 0.4, "f16": 0.4}}
 
 def rel(a, b):
     b = b.double().cpu()
@@ -138,14 +134,27 @@ def test_whole_frontend_vs_float64(prec):
     """One training step of each front-end against the reference modules in float64 on the CPU: video with 9 frames
     per utterance, 45x61 frames and all-zero padded frames (every max-pool window ties), video with 1 frame per
     utterance; audio with a waveform that is not a multiple of 640.  (Batches whose layer4 BatchNorm sees only a handful
-    of positions per channel are left out: its backward cancels so strongly that 11-bit operands lose the gradient.)  Output, the 60 parameter gradients, the 40 running buffers and num_batches_tracked."""
+    of positions per channel are left out: upstream error is amplified through the chain there; each unit on its own
+    is checked at such batches in test_zz_gpu_frontend_train_stages.py.)  Output, the 60 parameter gradients, the 40
+    running buffers and num_batches_tracked.  The float64 video chain's max-pool routes through the windows' winners
+    the library recorded, whose float64 values must match float64 max_pool3d within the bound: with 11-bit operands
+    a near-tie window can pick another winner than float64 does, and the stem's weight gradient (a sum with
+    cancellation) would show the misrouted gradient, not the library's arithmetic."""
     run_child(f"""
+from oracle.frontend_train_stages import pool_by_winner
 prec = {prec!r}
 g = torch.Generator().manual_seed(11)
 cases = [("video", torch.randn(2, 9, 1, 45, 61, generator=g)), ("video", torch.randn(3, 1, 1, 88, 88, generator=g)),
          ("audio", torch.randn(2, 2 * 640 + 333, 1, generator=g))]
 cases[0][1][1, 4:] = 0.0          # a zero-padded tail: constant stem output, every max-pool window ties
-worst = worst_stem = 0.0
+worst = worst_stem = worst_gap = 0.0
+pool0 = FT.MaxPoolFn
+class RecordWinners:
+    @staticmethod
+    def apply(x):
+        y, idx = pool0.apply(x)
+        winners.append(idx.cpu())
+        return y, idx
 for mod, x in cases:
     lib = build(mod).to(dev)
     lib.library_train, lib.precision = True, prec
@@ -153,28 +162,41 @@ for mod, x in cases:
         out_shape = reference(mod).double()(x.double()).shape
     ref = reference(mod).double()
     wts = torch.randn(out_shape, generator=g)
+    winners = []
+    FT.MaxPoolFn = RecordWinners
+    try:
+        o, gl, bl = step(lib, x.to(dev), wts.to(dev))
+    finally:
+        FT.MaxPoolFn = pool0
+    def pin(mod_, inp, out):
+        pinned = pool_by_winner(inp[0], winners[0])
+        # the library's winners hold a window maximum of the float64 stem output, up to the stem's own error
+        gap.append(rel(pinned.detach(), out.detach()))
+        return pinned
+    gap = []
+    for p in ref.modules():
+        if isinstance(p, torch.nn.MaxPool3d):
+            p.register_forward_hook(pin)
     o64, g64, b64 = step(ref, x.double(), wts.double())
-    o, gl, bl = step(lib, x.to(dev), wts.to(dev))
     assert len(gl) == 60 and len([k for k in bl if not k.endswith("num_batches_tracked")]) == 40
     errs = {{"out": rel(o, o64)}}
+    if gap:
+        errs["pinned_pool_vs_max_pool3d"] = gap[0]
+        worst_gap = max(worst_gap, gap[0])
     for k in g64: errs["grad." + k] = rel(gl[k], g64[k])
     for k in b64:
         if k.endswith("num_batches_tracked"):
             assert int(bl[k]) == int(b64[k]) == int(NBT0[mod][k]) + 1, k
         else:
             errs["buf." + k] = rel(bl[k], b64[k])
-    stem = {{k: v for k, v in errs.items() if k.startswith("grad.frontend3D")}}
-    rest = {{k: v for k, v in errs.items() if k not in stem}}
     print(mod, tuple(x.shape), sorted(errs.items(), key=lambda kv: -kv[1])[:5])
-    name, e = max(rest.items(), key=lambda kv: kv[1])
+    name, e = max(errs.items(), key=lambda kv: kv[1])
     worst = max(worst, e)
+    worst_stem = max([worst_stem] + [v for k, v in errs.items() if k.startswith("grad.frontend3D")])
     assert e < TOL_FE[prec], (mod, tuple(x.shape), name, e)
-    if stem:
-        name, e = max(stem.items(), key=lambda kv: kv[1])
-        worst_stem = max(worst_stem, e)
-        assert e < TOL_STEM[prec], (mod, tuple(x.shape), name, e)
 record("whole_frontend_train", prec, worst, TOL_FE[prec])
-record("whole_frontend_train_video_stem_grads", prec, worst_stem, TOL_STEM[prec])
+record("whole_frontend_train_video_stem_grads", prec, worst_stem, TOL_FE[prec])
+record("whole_frontend_train_pinned_pool_vs_max_pool3d", prec, worst_gap, TOL_FE[prec])
 print("CHILD-OK")
 """)
 
