@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("AVSR_B200_LIB") or os.path.join(_HERE, "csrc", "libavsr_b200.so")
 
 OK, E_INVALID, E_CUDA, E_WORKSPACE = 0, 1, 2, 3
-PREC_FP32, PREC_TF32, PREC_F16 = 0, 1, 2
+PREC_FP32, PREC_TF32, PREC_F16, PREC_BF16 = 0, 1, 2, 16
 ABI_VERSION = 10
 
 

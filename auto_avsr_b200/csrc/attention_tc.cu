@@ -1,4 +1,4 @@
-// Fused rel-pos flash attention on the Hopper tensor cores (wgmma, fp32 accumulate), TF32 or fp16 operands.
+// Fused rel-pos flash attention on the Hopper tensor cores (wgmma, fp32 accumulate), TF32, fp16 or bf16 operands.
 //
 //   scores[i,j] = ((q_i+u).k_j + (q_i+v).p[rel=i-j]) / 8 ;  keys j >= len[b] masked ;  ctx = softmax_j(scores) @ v
 // (transformer/attention.py:174-189 + :59-82 of the reference).  The reference materialises the (T x 2T-1) product
@@ -16,9 +16,10 @@
 //   wgmma  O [64 x 64] += P . V_tile             (registers; left in flight while the next tile's S and G are issued)
 // Loads overlap the math without a producer warp: once S and G of tile j (and P.V of tile j-1) have retired, thread 0
 // issues the K tile and band of tile j+1 (`kb_full`) and the V tile of tile j (`v_full`, awaited just before P.V), so
-// the next tile's K and band arrive during this tile's softmax and P.V.  fp16 needs 74 KB of shared memory, so three
-// CTAs (warpgroups) share an SM: at S2 the 336 (h, b, query tile) CTAs fit one wave of 3 x 132.
-// TF32: V arrives as v^T (B,H,64,Tp), K-major.  fp16: V keeps its natural (B,H,T,64) layout (MN-major B operand).
+// the next tile's K and band arrive during this tile's softmax and P.V.  fp16 / bf16 need 74 KB of shared memory, so
+// three CTAs (warpgroups) share an SM: at S2 the 336 (h, b, query tile) CTAs fit one wave of 3 x 132.
+// TF32: V arrives as v^T (B,H,64,Tp), K-major.  fp16 / bf16: V keeps its natural (B,H,T,64) layout (MN-major B
+// operand), and P is stored in the operand type.
 // Padded QUERY rows are computed like any other row (the reference masks keys only).
 #include "common.cuh"
 #include "sm90.cuh"
@@ -35,20 +36,20 @@ constexpr int AT_GLD = 64 + 4;   // fp32 row stride of the pre-skewed G tile (sp
 
 template <typename TOp>
 struct AtCfg {
-  static constexpr int kAtoms = 64 * (int)sizeof(TOp) / 128;   // 128-byte atoms along a 64-wide row (2 tf32 / 1 f16)
+  static constexpr int kAtoms = 64 * (int)sizeof(TOp) / 128;   // 128-byte atoms along a 64-wide row (2 tf32 / 1 16-bit)
   static constexpr int kSteps = 64 * (int)sizeof(TOp) / 32;    // MMA-K steps over 64 elements
   static constexpr int kQu = 0;
   static constexpr int kQv = kQu + AT_BQ * 128 * kAtoms;
   static constexpr int kK = kQv + AT_BQ * 128 * kAtoms;
   static constexpr int kPb = kK + AT_BKV * 128 * kAtoms;
-  static constexpr int kV = kPb + AT_BAND * 128 * kAtoms;      // tf32: [64 d][64 keys]; f16: [64 keys][64 d]
+  static constexpr int kV = kPb + AT_BAND * 128 * kAtoms;      // tf32: [64 d][64 keys]; 16-bit: [64 keys][64 d]
   static constexpr int kP = kV + 64 * 128 * kAtoms;
   static constexpr int kG = kP + AT_BQ * 128 * kAtoms;
   static constexpr int kBars = kG + AT_BQ * AT_GLD * 4;        // q_full, kb_full, v_full
   static constexpr int kSmem = kBars + 64 + 1024;
   static constexpr uint32_t kKbBytes = (AT_BKV + AT_BAND) * 128 * kAtoms;
   static constexpr uint32_t kVBytes = 64 * 128 * kAtoms;
-  // CTAs per SM the shared memory allows (228 KB per SM, 1 KB of it reserved per CTA): fp16 3, TF32 1
+  // CTAs per SM the shared memory allows (228 KB per SM, 1 KB of it reserved per CTA): fp16 / bf16 3, TF32 1
   static constexpr int kCtasPerSm = (228 * 1024) / (kSmem + 1024);
 };
 
@@ -65,7 +66,10 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_const
                     const __grid_constant__ CUtensorMap tmP, const int32_t* __restrict__ lengths, TOp* __restrict__ ctx,
                     int T, int H, int round_out) {
   using Cfg = AtCfg<TOp>;
-  constexpr bool kF16 = sizeof(TOp) == 2;
+  constexpr bool kF16 = sizeof(TOp) == 2;                       // a 16-bit operand type: f16 or bf16
+  constexpr bool kBF16 = std::is_same<TOp, __nv_bfloat16>::value;
+  // P and the context are packed two at a time in the operand type
+  auto pack2 = [](float a, float b) -> uint32_t { if constexpr (kBF16) return pack_bf162(a, b); else return pack_half2_sat(a, b); };
   extern __shared__ uint8_t at_smem_raw[];
   const uint32_t raw = smem_u32(at_smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
@@ -140,7 +144,8 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_const
     for (int ks = 0; ks < Cfg::kSteps; ++ks) {
       const uint64_t dq = at_desc(base + Cfg::kQu, AT_BQ, ks), dk = at_desc(base + Cfg::kK, AT_BKV, ks);
       const uint64_t dv = at_desc(base + Cfg::kQv, AT_BQ, ks), dp = at_desc(base + Cfg::kPb, AT_BAND, ks);
-      if constexpr (kF16) { wgmma_f16_n64(sc, dq, dk, ks != 0); wgmma_f16_n128(g, dv, dp, ks != 0); }
+      if constexpr (kBF16) { wgmma_bf16_n64(sc, dq, dk, ks != 0); wgmma_bf16_n128(g, dv, dp, ks != 0); }
+      else if constexpr (kF16) { wgmma_f16_n64(sc, dq, dk, ks != 0); wgmma_f16_n128(g, dv, dp, ks != 0); }
       else { wgmma_tf32_n64(sc, dq, dk, ks != 0); wgmma_tf32_n128(g, dv, dp, ks != 0); }
     }
     wgmma_commit();
@@ -209,7 +214,7 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_const
         const float p1 = exp2f(sc[4 * j + 2 * rr + 1] - mx[rr]);
         l_run[rr] += p0 + p1;
         if constexpr (kF16) {
-          *reinterpret_cast<uint32_t*>(gen + Cfg::kP + r * 128 + ((j ^ (r & 7)) << 4) + cq * 2) = pack_half2_sat(p0, p1);
+          *reinterpret_cast<uint32_t*>(gen + Cfg::kP + r * 128 + ((j ^ (r & 7)) << 4) + cq * 2) = pack2(p0, p1);
         } else {
           const int atom = j >> 2, chunk = 2 * (j & 3) + (cq >> 2);
           *reinterpret_cast<float2*>(gen + Cfg::kP + atom * (AT_BQ * 128) + r * 128 + ((chunk ^ (r & 7)) << 4) +
@@ -224,7 +229,8 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_const
 #pragma unroll
     for (int ks = 0; ks < Cfg::kSteps; ++ks) {
       const uint64_t dp = at_desc(base + Cfg::kP, AT_BQ, ks);
-      if constexpr (kF16) wgmma_f16_n64_bmn(o, dp, wgmma_desc_sw128(base + Cfg::kV + ks * 16 * 128), 1);
+      if constexpr (kBF16) wgmma_bf16_n64_bmn(o, dp, wgmma_desc_sw128(base + Cfg::kV + ks * 16 * 128), 1);
+      else if constexpr (kF16) wgmma_f16_n64_bmn(o, dp, wgmma_desc_sw128(base + Cfg::kV + ks * 16 * 128), 1);
       else wgmma_tf32_n64(o, dp, at_desc(base + Cfg::kV, 64, ks), 1);
     }
     wgmma_commit();
@@ -245,7 +251,7 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_const
       for (int j = 0; j < 8; ++j) {
         float a = o[4 * j + 2 * rr] * inv, c = o[4 * j + 2 * rr + 1] * inv;
         if constexpr (kF16) {
-          *reinterpret_cast<uint32_t*>(dst + 8 * j + cq) = pack_half2_sat(a, c);
+          *reinterpret_cast<uint32_t*>(dst + 8 * j + cq) = pack2(a, c);
         } else {
           if (round_out) { a = round_tf32(a); c = round_tf32(c); }
           *reinterpret_cast<float2*>(dst + 8 * j + cq) = make_float2(a, c);
@@ -264,14 +270,15 @@ static int attention_wg(const TOp* qu, const TOp* qv, const TOp* kk, const TOp* 
                         cudaStream_t st) {
   using Cfg = AtCfg<TOp>;
   constexpr int esz = (int)sizeof(TOp);
+  constexpr int kind = op_kind_of<TOp>();
   CUtensorMap tmQu, tmQv, tmK, tmV, tmP;
   const uint64_t rows = (uint64_t)B * H * T;
-  AVSR_TRY(make_tmap_2d(&tmQu, qu, rows, 64, 64, AT_BQ, esz));
-  AVSR_TRY(make_tmap_2d(&tmQv, qv, rows, 64, 64, AT_BQ, esz));
-  AVSR_TRY(make_tmap_2d(&tmK, kk, rows, 64, 64, AT_BKV, esz));
-  if (esz == 2) AVSR_TRY(make_tmap_2d(&tmV, v, rows, 64, 64, AT_BKV, esz));
-  else AVSR_TRY(make_tmap_2d(&tmV, v, (uint64_t)B * H * 64, (uint64_t)Tp, (uint64_t)Tp, 64, esz));
-  AVSR_TRY(make_tmap_3d(&tmP, pos, (uint64_t)H, (uint64_t)Rp, 64, 64, (uint64_t)Rp * 64, AT_BAND, esz));
+  AVSR_TRY(make_tmap_2d(&tmQu, qu, rows, 64, 64, AT_BQ, kind));
+  AVSR_TRY(make_tmap_2d(&tmQv, qv, rows, 64, 64, AT_BQ, kind));
+  AVSR_TRY(make_tmap_2d(&tmK, kk, rows, 64, 64, AT_BKV, kind));
+  if (esz == 2) AVSR_TRY(make_tmap_2d(&tmV, v, rows, 64, 64, AT_BKV, kind));
+  else AVSR_TRY(make_tmap_2d(&tmV, v, (uint64_t)B * H * 64, (uint64_t)Tp, (uint64_t)Tp, 64, kind));
+  AVSR_TRY(make_tmap_3d(&tmP, pos, (uint64_t)H, (uint64_t)Rp, 64, 64, (uint64_t)Rp * 64, AT_BAND, kind));
   AVSR_SET_MAX_SMEM(attention_wg_kernel<TOp>, Cfg::kSmem);
   dim3 grid(H, B, cdiv(T, AT_BQ));
   AVSR_LAUNCH(attention_wg_kernel<TOp>, grid, AT_THREADS, Cfg::kSmem, st, tmQu, tmQv, tmK, tmV, tmP, lengths, ctx, T, H,
@@ -287,11 +294,18 @@ int attention_tc(const float* qu, const float* qv, const float* kk, const float*
   return attention_wg<float>(qu, qv, kk, vt, pos, lengths, ctx, B, T, H, Tp, Rp, round_out, st);
 }
 
-int attention_f16(const __half* qu, const __half* qv, const __half* kk, const __half* vv, const __half* pos,
-                  const int32_t* lengths, __half* ctx, int B, int T, int H, int Rp, cudaStream_t st) {
-  AVSR_REQUIRE(Rp >= 2 * T - 1, "attention_f16: bad Rp=%d for T=%d", Rp, T);
+int attention_op16(int kind, const void* qu, const void* qv, const void* kk, const void* vv, const void* pos,
+                   const int32_t* lengths, void* ctx, int B, int T, int H, int Rp, cudaStream_t st) {
+  AVSR_REQUIRE(op16(kind), "attention_op16: operand kind %d", kind);
+  AVSR_REQUIRE(Rp >= 2 * T - 1, "attention_op16: bad Rp=%d for T=%d", Rp, T);
   if (B <= 0 || T <= 0) return AVSR_OK;
-  return attention_wg<__half>(qu, qv, kk, vv, pos, lengths, ctx, B, T, H, T, Rp, 0, st);
+  if (kind == OP_BF16) {
+    using B16 = __nv_bfloat16;
+    return attention_wg<B16>((const B16*)qu, (const B16*)qv, (const B16*)kk, (const B16*)vv, (const B16*)pos, lengths,
+                             (B16*)ctx, B, T, H, T, Rp, 0, st);
+  }
+  return attention_wg<__half>((const __half*)qu, (const __half*)qv, (const __half*)kk, (const __half*)vv,
+                              (const __half*)pos, lengths, (__half*)ctx, B, T, H, T, Rp, 0, st);
 }
 
 }  // namespace avsr

@@ -1,5 +1,6 @@
 // Shared internals of libavsr_b200: error plumbing, launch accounting, the GEMM epilogue family.
 #pragma once
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -10,6 +11,7 @@
 #include <cstdlib>
 #include <string>
 #include <tuple>
+#include <type_traits>
 #include <utility>
 
 #include "../../include/avsr_b200.h"
@@ -180,14 +182,29 @@ __device__ __forceinline__ float warp_max(float v) {
 //   OP_TF32 : fp32 container, value rounded to TF32 (10-bit mantissa) -> wgmma .tf32
 //   OP_F16  : IEEE half (same 10-bit mantissa as TF32, 5-bit exponent, saturating) -> wgmma .f16;
 //             half the bytes through L2/shared memory and twice the MMA rate of .tf32
-enum OperandKind : int { OP_F32 = 0, OP_TF32 = 1, OP_F16 = 2 };
+//   OP_BF16 : bfloat16 (7-bit mantissa, fp32's 8-bit exponent, round to nearest even, no saturation) -> wgmma .bf16;
+//             the bytes and the rate of OP_F16, the range of fp32
+enum OperandKind : int { OP_F32 = 0, OP_TF32 = 1, OP_F16 = 2, OP_BF16 = 3 };
 
-static inline bool valid_precision(int p) { return p == AVSR_PREC_FP32 || p == AVSR_PREC_TF32 || p == AVSR_PREC_F16; }
+static inline bool valid_precision(int p) {
+  return p == AVSR_PREC_FP32 || p == AVSR_PREC_TF32 || p == AVSR_PREC_F16 || p == AVSR_PREC_BF16;
+}
 // AVSR_PREC_* -> how the operands of that precision's contractions are stored
 static inline int operand_kind(int precision) {
-  return precision == AVSR_PREC_F16 ? OP_F16 : (precision == AVSR_PREC_TF32 ? OP_TF32 : OP_F32);
+  return precision == AVSR_PREC_F16    ? OP_F16
+         : precision == AVSR_PREC_BF16 ? OP_BF16
+         : precision == AVSR_PREC_TF32 ? OP_TF32
+                                       : OP_F32;
 }
-static inline size_t operand_bytes(int kind) { return kind == OP_F16 ? 2 : 4; }
+// 2-byte operand storage (f16 or bf16): the same layouts, the same tile shapes, the same byte counts
+AVSR_HD bool op16(int kind) { return kind == OP_F16 || kind == OP_BF16; }
+static inline bool prec16(int precision) { return op16(operand_kind(precision)); }
+static inline size_t operand_bytes(int kind) { return op16(kind) ? 2 : 4; }
+// the operand kind a tensor-core kernel instantiated for element type TOp reads (float: TF32)
+template <typename TOp>
+constexpr int op_kind_of() {
+  return sizeof(TOp) == 4 ? OP_TF32 : (std::is_same<TOp, __half>::value ? OP_F16 : OP_BF16);
+}
 
 __device__ __forceinline__ __half to_half_sat(float x) {
   unsigned short r;
@@ -206,7 +223,14 @@ __device__ __forceinline__ uint32_t pack_half2_sat_relu(float a, float b) {
   asm("cvt.rn.relu.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
   return r;
 }
-// store 4 consecutive operand values (dst 16-byte aligned for float, 8-byte aligned for half)
+// two floats -> packed bfloat16s (a in the low half), round to nearest even, no saturation (beyond the largest finite
+// bf16 a value rounds to +-inf like any IEEE conversion), NaN stays NaN: ONE conversion instruction
+__device__ __forceinline__ uint32_t pack_bf162(float a, float b) {
+  uint32_t r;
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
+  return r;
+}
+// store 4 consecutive operand values (dst 16-byte aligned for float, 8-byte aligned for half / bfloat16)
 template <typename TOp>
 __device__ __forceinline__ void store_op4(TOp* dst, float a, float b, float c, float d);
 template <>
@@ -222,15 +246,32 @@ __device__ __forceinline__ void store_op4<__half>(__half* dst, float a, float b,
   v.y = *reinterpret_cast<uint32_t*>(&hi);
   *reinterpret_cast<uint2*>(dst) = v;
 }
+template <>
+__device__ __forceinline__ void store_op4<__nv_bfloat16>(__nv_bfloat16* dst, float a, float b, float c, float d) {
+  *reinterpret_cast<uint2*>(dst) = make_uint2(pack_bf162(a, b), pack_bf162(c, d));
+}
 template <typename TOp>
 __device__ __forceinline__ void store_op1(TOp* dst, float a);
 template <>
 __device__ __forceinline__ void store_op1<float>(float* dst, float a) { *dst = round_tf32(a); }
 template <>
 __device__ __forceinline__ void store_op1<__half>(__half* dst, float a) { *dst = to_half_sat(a); }
-// runtime-kind store used by the elementwise kernels (kind is warp-uniform)
+template <>
+__device__ __forceinline__ void store_op1<__nv_bfloat16>(__nv_bfloat16* dst, float a) { *dst = __float2bfloat16_rn(a); }
+// runtime-kind stores / loads used by the elementwise kernels (kind is warp-uniform; a negative kind is plain fp32)
+__device__ __forceinline__ void store_kind1(void* base, long idx, int kind, float v) {
+  if (kind == OP_F16) reinterpret_cast<__half*>(base)[idx] = to_half_sat(v);
+  else if (kind == OP_BF16) reinterpret_cast<__nv_bfloat16*>(base)[idx] = __float2bfloat16_rn(v);
+  else reinterpret_cast<float*>(base)[idx] = kind == OP_TF32 ? round_tf32(v) : v;
+}
+__device__ __forceinline__ float load_kind1(const void* base, long idx, int kind) {
+  if (kind == OP_F16) return __half2float(reinterpret_cast<const __half*>(base)[idx]);
+  if (kind == OP_BF16) return __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(base)[idx]);
+  return reinterpret_cast<const float*>(base)[idx];
+}
 __device__ __forceinline__ void store_kind4(void* base, long idx, int kind, float a, float b, float c, float d) {
   if (kind == OP_F16) store_op4<__half>(reinterpret_cast<__half*>(base) + idx, a, b, c, d);
+  else if (kind == OP_BF16) store_op4<__nv_bfloat16>(reinterpret_cast<__nv_bfloat16*>(base) + idx, a, b, c, d);
   else if (kind == OP_TF32) store_op4<float>(reinterpret_cast<float*>(base) + idx, a, b, c, d);
   else *reinterpret_cast<float4*>(reinterpret_cast<float*>(base) + idx) = make_float4(a, b, c, d);
 }
@@ -260,7 +301,7 @@ struct EpiParams {
   const float* pos_v;
   float* partial;     // split-K: fp32 workspace [splits][M][ldo] for the partial tiles (deterministic fix-up)
   int* counters;      // split-K: one arrival counter per output tile, zero on entry, reset by the last arriver
-  void* qu;           // operand-typed (float for OP_F32/OP_TF32, __half for OP_F16)
+  void* qu;           // operand-typed (float for OP_F32/OP_TF32, __half for OP_F16, __nv_bfloat16 for OP_BF16)
   void* qv;
   void* kk;
   void* vt;
@@ -333,7 +374,7 @@ __device__ __forceinline__ void put(void* base, long idx, float v, bool operand)
 }
 
 // Scalar (one element) epilogue: used by the CUDA-core GEMM and by the tensor-core kernel's ragged edges.
-// TOp = float serves OP_F32 (round_out = 0) and OP_TF32 (round_out = 1); TOp = __half serves OP_F16.
+// TOp = float serves OP_F32 (round_out = 0) and OP_TF32 (round_out = 1); __half OP_F16, __nv_bfloat16 OP_BF16.
 template <int MODE, typename TOp = float>
 __device__ __forceinline__ void epi_store(const EpiParams& p, int m, int n, float acc) {
   if (m >= p.M || n >= p.N) return;
@@ -380,7 +421,7 @@ __device__ __forceinline__ void epi_store_glu(const EpiParams& p, int m, int n_v
 // ---------------------------------------------------------------- kernel launchers (defined in the .cu files)
 // fp32 CUDA-core GEMM (gemm_simt.cu)
 int gemm_simt(int mode, const float* A, const float* Bw, int M, int N, int K, const EpiParams& ep, cudaStream_t st);
-// wgmma GEMM (gemm_tc.cu); opk = OP_TF32 (A, Bw are float) or OP_F16 (A, Bw are __half)
+// wgmma GEMM (gemm_tc.cu); opk = OP_TF32 (A, Bw are float), OP_F16 (__half) or OP_BF16 (__nv_bfloat16)
 int gemm_tc(int mode, int opk, const void* A, const void* Bw, int M, int N, int K, const EpiParams& ep, cudaStream_t st);
 
 // elementwise.cu
@@ -407,8 +448,9 @@ int attention_simt(const float* qu, const float* qv, const float* kk, const floa
 int attention_tc(const float* qu, const float* qv, const float* kk, const float* vt, const float* pos,
                  const int32_t* lengths, float* ctx, int B, int T, int H, int Tp, int Rp, int round_out,
                  cudaStream_t st);
-// fp16 operands (attention_tc.cu): qu, qv, kk, vv all (B,H,T,64) __half (V in its natural layout); ctx __half
-int attention_f16(const __half* qu, const __half* qv, const __half* kk, const __half* vv, const __half* pos,
-                  const int32_t* lengths, __half* ctx, int B, int T, int H, int Rp, cudaStream_t st);
+// 2-byte operands (attention_tc.cu), kind OP_F16 or OP_BF16: qu, qv, kk, vv all (B,H,T,64) (V in its natural
+// layout); ctx (B*T, H*64) in the same storage
+int attention_op16(int kind, const void* qu, const void* qv, const void* kk, const void* vv, const void* pos,
+                   const int32_t* lengths, void* ctx, int B, int T, int H, int Rp, cudaStream_t st);
 
 }  // namespace avsr

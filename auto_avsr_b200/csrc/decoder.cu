@@ -31,7 +31,8 @@ __global__ void __launch_bounds__(256) for_each_kernel(long count, F f) {
 constexpr int kGaRows = 64, kGaTile = 64, kGaLd = 65, kGaThreads = 256;
 constexpr size_t kGaFixedSmem = (3 * kGaRows * kGaLd + kGaRows + 8) * sizeof(float);
 
-__global__ void __launch_bounds__(kGaThreads) grouped_src_attention_kernel(
+// (the minimum of 1 CTA per SM lets ptxas go past 64 registers: with the bf16 store next to the f16 one it spilled)
+__global__ void __launch_bounds__(kGaThreads, 1) grouped_src_attention_kernel(
     const float* __restrict__ q, const float* __restrict__ kv, const int32_t* __restrict__ row_utt,
     const int32_t* __restrict__ utt_off, const int32_t* __restrict__ utt_len, int U, long sum_T, int n, int H, int dk,
     int D, int T_max, float sqrt_dk, float* __restrict__ scores, int kind, void* __restrict__ ctx) {

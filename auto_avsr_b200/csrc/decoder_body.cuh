@@ -143,12 +143,13 @@ static inline DecWork layout_dec_work(const AvsrDecoderConfig& c, int T, int max
 }
 
 // ------------------------------------------------------------------ per-element functors
+// bf16: round to nearest even, no saturation, on the device and in the host replay alike (__float2bfloat16_rn)
 AVSR_HD void store_operand(void* base, long idx, int kind, float v) {
 #ifdef __CUDA_ARCH__
-  if (kind == OP_F16) reinterpret_cast<__half*>(base)[idx] = to_half_sat(v);
-  else reinterpret_cast<float*>(base)[idx] = kind == OP_TF32 ? round_tf32(v) : v;
+  store_kind1(base, idx, kind, v);
 #else
   if (kind == OP_F16) reinterpret_cast<__half*>(base)[idx] = __float2half_rn(v);
+  else if (kind == OP_BF16) reinterpret_cast<__nv_bfloat16*>(base)[idx] = __float2bfloat16_rn(v);
   else reinterpret_cast<float*>(base)[idx] = v;
 #endif
 }
@@ -509,7 +510,7 @@ int project_memory_kv(BK& bk, const AvsrDecoderConfig& c, const DecPrep& P, cons
   // Row chunks of <= 192 frames: every launch stays in the M < 256 regime of the persistent one-CTA GEMM -- the same
   // kernel variant (fp32 output + bias) every step GEMM of this path uses; once per utterance, so the extra launches
   // do not matter.
-  const size_t esz = prec == AVSR_PREC_F16 ? 2 : 4;
+  const size_t esz = operand_bytes(operand_kind(prec));
   constexpr int kChunk = 192;
   for (int l = 0; l < c.num_blocks; ++l)
     for (int r0 = 0; r0 < T; r0 += kChunk) {

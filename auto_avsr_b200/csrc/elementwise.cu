@@ -235,6 +235,8 @@ __global__ void sinusoid_kernel(void* __restrict__ pe, int T, int d, int out_kin
     const long idx = (long)m * d + 2 * c;
     if (out_kind == OP_F16) {
       *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(pe) + idx) = __halves2half2(to_half_sat(s), to_half_sat(co));
+    } else if (out_kind == OP_BF16) {
+      *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(pe) + idx) = pack_bf162(s, co);
     } else if (out_kind == OP_TF32) {
       *reinterpret_cast<float2*>(reinterpret_cast<float*>(pe) + idx) = make_float2(round_tf32(s), round_tf32(co));
     } else {

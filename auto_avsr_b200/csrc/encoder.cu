@@ -79,13 +79,10 @@ static int check_cfg(const AvsrEncoderConfig* c) {
 }
 
 // ------------------------------------------------------------------ preparation kernels
-// copy with conversion to an operand storage kind (OP_F32 plain copy, OP_TF32 rounded fp32, OP_F16 half)
+// copy with conversion to an operand storage kind (OP_F32 plain copy, OP_TF32 rounded fp32, OP_F16 half, OP_BF16)
 __global__ void copy_round_kernel(const float* __restrict__ src, void* __restrict__ dst, long n, int kind, float scale) {
-  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
-    const float v = src[i] * scale;
-    if (kind == OP_F16) reinterpret_cast<__half*>(dst)[i] = to_half_sat(v);
-    else reinterpret_cast<float*>(dst)[i] = kind == OP_TF32 ? round_tf32(v) : v;
-  }
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x)
+    store_kind1(dst, i, kind, src[i] * scale);
 }
 // pointwise_cov1 (2D, D[,1]) -> rows interleaved in groups of 64: [g*128, +64) value channels g*64.., then their gates
 __global__ void glu_interleave_kernel(const float* __restrict__ w, const float* __restrict__ b, void* __restrict__ wo,
@@ -94,9 +91,7 @@ __global__ void glu_interleave_kernel(const float* __restrict__ w, const float* 
   const int g = r >> 7, wi = r & 127;
   const int src = wi < 64 ? g * 64 + wi : D + g * 64 + (wi - 64);
   for (int k = threadIdx.x; k < D; k += blockDim.x) {
-    const float v = w[(long)src * D + k];
-    if (kind == OP_F16) reinterpret_cast<__half*>(wo)[(long)r * D + k] = to_half_sat(v);
-    else reinterpret_cast<float*>(wo)[(long)r * D + k] = kind == OP_TF32 ? round_tf32(v) : v;
+    store_kind1(wo, (long)r * D + k, kind, w[(long)src * D + k]);
   }
   if (threadIdx.x == 0) bo[r] = b[src];
 }
@@ -181,7 +176,8 @@ __global__ void fill_lengths_kernel(int32_t* dst, const int32_t* src, int B, int
 // fp16 operand stores saturate (cvt.rn.satfinite, common.cuh): a value beyond +-65504 becomes +-65504 silently.  The
 // checked forward (avsr_encoder_forward_checked) scans every operand tensor right after its producer and counts the
 // elements that sit AT the saturation value (or are NaN): non-zero means the fp16 path left its range for these
-// weights / inputs and the caller must fall back to tf32 / fp32 precision -- the drop-in raises (engine.py).
+// weights / inputs and the caller must fall back to bf16 (fp32's range), tf32 or fp32 -- the drop-in raises
+// (engine.py).
 __global__ void count_saturated_kernel(const uint4* __restrict__ p, long n16, unsigned long long* count) {
   unsigned local = 0;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n16; i += (long)gridDim.x * blockDim.x) {
@@ -258,7 +254,7 @@ static int forward_body(const AvsrEncoderConfig& c, const Prepared& P, const Wor
   const int opk = operand_kind(prec);           // storage of every tensor that feeds a contraction
   const int opr = prec != AVSR_PREC_FP32;       // "destination is operand-typed" flag of the epilogues
   const size_t stage_bytes = (size_t)N * D * sizeof(float);
-  if (prec != AVSR_PREC_F16) sat = nullptr;     // only the fp16 operand storage saturates
+  if (prec != AVSR_PREC_F16) sat = nullptr;     // only the fp16 operand storage saturates (bf16 has fp32's range)
   auto chk = [&](const void* buf, size_t nelems) -> int { return count_saturated(buf, nelems, sat, st); };
 
   // split-K tile counters must be zero on entry (they re-arm themselves; this covers a first use / an aborted run)
@@ -273,8 +269,8 @@ static int forward_body(const AvsrEncoderConfig& c, const Prepared& P, const Wor
     AVSR_TRY(compute_pos(c, P, W, T, prec, ps));
     if (aux) AVSR_CUDA_TRY(cudaEventRecord(aux->join, ps));
   }
-  // v^T pad columns [T, Tp) must be finite (FP32 / TF32 paths; the F16 path keeps V un-transposed)
-  if (W.Tp != T && prec != AVSR_PREC_F16)
+  // v^T pad columns [T, Tp) must be finite (FP32 / TF32 paths; the 16-bit paths keep V un-transposed)
+  if (W.Tp != T && !prec16(prec))
     AVSR_CUDA_TRY(cudaMemsetAsync(W.vt, 0, (size_t)B * D * W.Tp * sizeof(float), st));
 
   for (int l = 0; l < L; ++l) {
@@ -299,7 +295,7 @@ static int forward_body(const AvsrEncoderConfig& c, const Prepared& P, const Wor
       EpiParams e{};
       e.M = N; e.bias = w.qk_b; e.T = T; e.H = H; e.pos_u = w.pos_u; e.pos_v = w.pos_v;
       e.qu = W.qu; e.qv = W.qv; e.kk = W.kk; e.vt = W.vt; e.round_out = opr;
-      if (prec == AVSR_PREC_F16) {
+      if (prec16(prec)) {
         // one QKV projection; V keeps the (B,H,T,64) layout (the P.V MMA reads it as an MN-major operand)
         e.N = 3 * D;
         AVSR_TRY(run_gemm(prec, EPI_QK, W.xn, w.qk_w, N, 3 * D, D, e, st));
@@ -317,9 +313,8 @@ static int forward_body(const AvsrEncoderConfig& c, const Prepared& P, const Wor
     if (l == 0) AVSR_TRY(chk(W.pos, (size_t)L * W.Rp * D / 8 * 8));
     {
       const void* pos_l = op_offset(W.pos, (size_t)l * H * W.Rp * kHeadDim, prec);
-      if (prec == AVSR_PREC_F16)
-        AVSR_TRY(attention_f16((const __half*)W.qu, (const __half*)W.qv, (const __half*)W.kk, (const __half*)W.vt,
-                               (const __half*)pos_l, lengths, (__half*)W.ctx, B, T, H, W.Rp, st));
+      if (prec16(prec))
+        AVSR_TRY(attention_op16(opk, W.qu, W.qv, W.kk, W.vt, pos_l, lengths, W.ctx, B, T, H, W.Rp, st));
       else if (prec == AVSR_PREC_TF32)
         AVSR_TRY(attention_tc(W.qu, W.qv, W.kk, W.vt, (const float*)pos_l, lengths, W.ctx, B, T, H, W.Tp, W.Rp, 1, st));
       else
@@ -385,7 +380,7 @@ static int forward_impl(const AvsrEncoderConfig* cfg, const void* prepared, cons
 static int plan_branches(int B, int T, int precision) {
   int want = 1;
   if (const char* e = getenv("AVSR_B200_BRANCHES")) want = atoi(e);
-  if (precision != AVSR_PREC_F16 || want < 2) return 1;
+  if (!prec16(precision) || want < 2) return 1;
   if (want > kMaxBranches) want = kMaxBranches;
   if (want > B) want = B;
   while (want > 1 && (long)(B / want) * T < 256) --want;   // slices of fewer than 256 rows leave GEMM tiles half empty
@@ -741,7 +736,7 @@ int avsr_layernorm(const float* x, const float* gamma, const float* beta, float*
 }
 
 size_t avsr_linear_workspace_bytes(int rows, int n, int k, int precision) {
-  if (precision != AVSR_PREC_F16 || rows <= 0 || n <= 0 || k <= 0) return 16;
+  if (!prec16(precision) || rows <= 0 || n <= 0 || k <= 0) return 16;
   return align_up((size_t)rows * k * 2, 256) + align_up((size_t)n * k * 2, 256);
 }
 
@@ -751,13 +746,14 @@ int avsr_linear(const float* x, const float* w, const float* bias, const float* 
   AVSR_REQUIRE(valid_precision(precision), "bad precision %d", precision);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const void *xa = x, *wa = w;
-  if (precision == AVSR_PREC_F16 && rows > 0 && n > 0) {
-    AVSR_REQUIRE(workspace != nullptr, "avsr_linear: AVSR_PREC_F16 needs a workspace");
+  if (prec16(precision) && rows > 0 && n > 0) {
+    AVSR_REQUIRE(workspace != nullptr, "avsr_linear: %s needs a workspace",
+                 precision == AVSR_PREC_F16 ? "AVSR_PREC_F16" : "AVSR_PREC_BF16");
     AVSR_REQUIRE_BYTES(avsr_linear_workspace_bytes(rows, n, k, precision), workspace_bytes, "linear workspace");
     char* xh = reinterpret_cast<char*>(workspace);
     char* wh = xh + align_up((size_t)rows * k * 2, 256);
-    AVSR_TRY(copy_round(x, xh, (long)rows * k, OP_F16, st));
-    AVSR_TRY(copy_round(w, wh, (long)n * k, OP_F16, st));
+    AVSR_TRY(copy_round(x, xh, (long)rows * k, operand_kind(precision), st));
+    AVSR_TRY(copy_round(w, wh, (long)n * k, operand_kind(precision), st));
     xa = xh; wa = wh;
   }
   // note: in TF32 mode operands are used as given (the tensor core truncates fp32 -> tf32)
@@ -792,16 +788,14 @@ __global__ void split_heads_kernel(const float* __restrict__ src, const float* _
     const int c = (int)(i % (H * kHeadDim));
     const long r = i / (H * kHeadDim);
     const int b = (int)(r / T), t = (int)(r % T), h = c / kHeadDim, d = c % kHeadDim;
-    const float v = src[i] + (bias ? bias[c] : 0.f);
     const long o = transpose ? (((long)b * H + h) * kHeadDim + d) * Tp + t : (((long)b * H + h) * T + t) * kHeadDim + d;
-    if (kind == OP_F16) reinterpret_cast<__half*>(dst)[o] = to_half_sat(v);
-    else reinterpret_cast<float*>(dst)[o] = kind == OP_TF32 ? round_tf32(v) : v;
+    store_kind1(dst, o, kind, src[i] + (bias ? bias[c] : 0.f));
   }
 }
 
-__global__ void half_to_float_kernel(const __half* __restrict__ src, float* __restrict__ dst, long n) {
+__global__ void op_to_float_kernel(const void* __restrict__ src, float* __restrict__ dst, long n, int kind) {
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x)
-    dst[i] = __half2float(src[i]);
+    dst[i] = load_kind1(src, i, kind);
 }
 
 size_t avsr_attention_workspace_bytes(int B, int T, int H) {
@@ -829,13 +823,12 @@ int avsr_relpos_attention(const float* q, const float* k, const float* v, const 
   split_heads_kernel<<<blocks, 256, 0, st>>>(q, pos_bias_u, qu, B, T, H, Tp, 0, kind); AVSR_CHECK_LAUNCH();
   split_heads_kernel<<<blocks, 256, 0, st>>>(q, pos_bias_v, qv, B, T, H, Tp, 0, kind); AVSR_CHECK_LAUNCH();
   split_heads_kernel<<<blocks, 256, 0, st>>>(k, nullptr, kk, B, T, H, Tp, 0, kind); AVSR_CHECK_LAUNCH();
-  split_heads_kernel<<<blocks, 256, 0, st>>>(v, nullptr, vt, B, T, H, Tp, precision == AVSR_PREC_F16 ? 0 : 1, kind);
+  split_heads_kernel<<<blocks, 256, 0, st>>>(v, nullptr, vt, B, T, H, Tp, prec16(precision) ? 0 : 1, kind);
   AVSR_CHECK_LAUNCH();
   split_heads_kernel<<<blocks, 256, 0, st>>>(p, nullptr, pos, 1, R, H, R, 0, kind); AVSR_CHECK_LAUNCH();
-  if (precision == AVSR_PREC_F16) {
-    AVSR_TRY(attention_f16((const __half*)qu, (const __half*)qv, (const __half*)kk, (const __half*)vt, (const __half*)pos,
-                           lengths, (__half*)ctxh, B, T, H, R, st));
-    half_to_float_kernel<<<blocks, 256, 0, st>>>((const __half*)ctxh, ctx, (long)N * D);
+  if (prec16(precision)) {
+    AVSR_TRY(attention_op16(kind, qu, qv, kk, vt, pos, lengths, ctxh, B, T, H, R, st));
+    op_to_float_kernel<<<blocks, 256, 0, st>>>(ctxh, ctx, (long)N * D, kind);
     AVSR_CHECK_LAUNCH();
     return AVSR_OK;
   }
@@ -871,12 +864,12 @@ int avsr_pointwise_glu(const float* x, const float* w, const float* b, float* y,
   float* wi = reinterpret_cast<float*>(workspace);
   float* bi = wi + (size_t)2 * C * C;
   char* xh = reinterpret_cast<char*>(workspace) + align_up(((size_t)2 * C * C + 2 * C) * sizeof(float), 256);
-  const int kind = precision == AVSR_PREC_F16 ? OP_F16 : OP_F32;   // TF32: the tensor core truncates raw fp32
+  const int kind = prec16(precision) ? operand_kind(precision) : OP_F32;   // TF32: the tensor core truncates raw fp32
   glu_interleave_kernel<<<(unsigned)(2 * C), 256, 0, st>>>(w, b, wi, bi, C, kind);
   AVSR_CHECK_LAUNCH();
   const void* xa = x;
-  if (precision == AVSR_PREC_F16 && rows > 0) {
-    AVSR_TRY(copy_round(x, xh, (long)rows * C, OP_F16, st));
+  if (prec16(precision) && rows > 0) {
+    AVSR_TRY(copy_round(x, xh, (long)rows * C, kind, st));
     xa = xh;
   }
   EpiParams e{};

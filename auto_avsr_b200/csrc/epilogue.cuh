@@ -38,6 +38,16 @@ __device__ __forceinline__ void stage_write_f16(uint8_t* stg, int row_bytes, int
     *reinterpret_cast<uint4*>(row + 16 * j) = t;
   }
 }
+// lane writes its row: 64 values converted to bfloat16 (128 bytes)
+__device__ __forceinline__ void stage_write_bf16(uint8_t* stg, int row_bytes, int lane, const float* o) {
+  uint8_t* row = stg + lane * row_bytes;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const uint4 t = make_uint4(pack_bf162(o[8 * j], o[8 * j + 1]), pack_bf162(o[8 * j + 2], o[8 * j + 3]),
+                               pack_bf162(o[8 * j + 4], o[8 * j + 5]), pack_bf162(o[8 * j + 6], o[8 * j + 7]));
+    *reinterpret_cast<uint4*>(row + 16 * j) = t;
+  }
+}
 template <typename TOp> struct StageOp;
 template <> struct StageOp<float> {
   static constexpr int kCols = 32;   // operand columns per 128-byte row segment
@@ -49,6 +59,12 @@ template <> struct StageOp<__half> {
   static constexpr int kCols = 64;
   __device__ static void write(uint8_t* stg, int row_bytes, int lane, const float* o) {
     stage_write_f16(stg, row_bytes, lane, o);
+  }
+};
+template <> struct StageOp<__nv_bfloat16> {
+  static constexpr int kCols = 64;
+  __device__ static void write(uint8_t* stg, int row_bytes, int lane, const float* o) {
+    stage_write_bf16(stg, row_bytes, lane, o);
   }
 };
 // transposed read: iteration `it` (0..7) gives this lane the 16-byte piece (lane & 7) of row it*4 + (lane >> 3)

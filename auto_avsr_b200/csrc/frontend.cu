@@ -8,7 +8,7 @@
 //
 // conv_tc_kernel (sm_90a): 128 output pixels x BN channels per CTA, two warpgroups of 64 pixels each issue
 // wgmma.mma_async from a 4-stage ring of 128B-swizzled shared-memory tiles.  A K-block is 128 bytes of one filter tap
-// (64 f16 or 32 tf32 channels; every trunk C_in is a multiple of 64), so the A tile of a trunk conv is gathered with
+// (64 f16 / bf16 or 32 tf32 channels; every trunk C_in is a multiple of 64), so the A tile of a trunk conv is gathered with
 // 16-byte cp.async copies straight from the activation (zero-filled where the tap falls into the padding); tiles of
 // pixels cross frame boundaries.  The stems (C_in = 1) gather their fp32 input element by element (K = 245 -> 256
 // for video, 80 -> 128 for audio), convert it to the operand type and store it with the same swizzle.
@@ -39,11 +39,17 @@ __device__ __forceinline__ float silu_fast(float v) { return v * sigmoidf_fast(v
 template <typename TOp> __device__ __forceinline__ float op_ld(const TOp* p);
 template <> __device__ __forceinline__ float op_ld<float>(const float* p) { return *p; }
 template <> __device__ __forceinline__ float op_ld<__half>(const __half* p) { return __half2float(*p); }
+template <> __device__ __forceinline__ float op_ld<__nv_bfloat16>(const __nv_bfloat16* p) { return __bfloat162float(*p); }
 
 template <typename TOp>
 __device__ __forceinline__ float4 op_ld4(const TOp* p) {
   if constexpr (sizeof(TOp) == 4) {
     return *reinterpret_cast<const float4*>(p);
+  } else if constexpr (std::is_same<TOp, __nv_bfloat16>::value) {
+    const uint2 u = *reinterpret_cast<const uint2*>(p);
+    const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.x));
+    const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.y));
+    return make_float4(a.x, a.y, b.x, b.y);
   } else {
     const uint2 u = *reinterpret_cast<const uint2*>(p);
     const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
@@ -52,19 +58,16 @@ __device__ __forceinline__ float4 op_ld4(const TOp* p) {
   }
 }
 
-// kind: OP_F32 plain, OP_TF32 rounded fp32, OP_F16 half
+// kind: OP_F32 plain, OP_TF32 rounded fp32, OP_F16 half, OP_BF16 bfloat16
 __global__ void cvt_to_op_kernel(const float* __restrict__ x, void* __restrict__ y, long n, int kind) {
   pdl_wait();
-  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
-    const float v = x[i];
-    if (kind == OP_F16) reinterpret_cast<__half*>(y)[i] = to_half_sat(v);
-    else reinterpret_cast<float*>(y)[i] = kind == OP_TF32 ? round_tf32(v) : v;
-  }
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x)
+    store_kind1(y, i, kind, x[i]);
 }
 __global__ void cvt_from_op_kernel(const void* __restrict__ x, float* __restrict__ y, long n, int kind) {
   pdl_wait();
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x)
-    y[i] = kind == OP_F16 ? __half2float(reinterpret_cast<const __half*>(x)[i]) : reinterpret_cast<const float*>(x)[i];
+    y[i] = load_kind1(x, i, kind);
 }
 
 // torch conv weight (Cout, Cin, taps) -> (Cout, Kp) with k = tap * Cin + c, zero for k >= taps * Cin
@@ -79,8 +82,7 @@ __global__ void reorder_weight_kernel(const float* __restrict__ w, void* __restr
       const int tap = k / Cin, c = k - tap * Cin;
       v = w[((long)co * Cin + c) * taps + tap];
     }
-    if (kind == OP_F16) reinterpret_cast<__half*>(dst)[i] = to_half_sat(v);
-    else reinterpret_cast<float*>(dst)[i] = kind == OP_TF32 ? round_tf32(v) : v;
+    store_kind1(dst, i, kind, v);
   }
 }
 
@@ -185,6 +187,16 @@ template <> struct ConvOp<__half> {
     u.x = pack_half2_sat(v[0], v[1]); u.y = pack_half2_sat(v[2], v[3]);
     u.z = pack_half2_sat(v[4], v[5]); u.w = pack_half2_sat(v[6], v[7]);
     return u;
+  }
+};
+template <> struct ConvOp<__nv_bfloat16> {
+  static constexpr int KE = 64;
+  template <int BN>
+  __device__ static void mma(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+    if constexpr (BN == 64) wgmma_bf16_n64(d, a, b, acc); else wgmma_bf16_n128(d, a, b, acc);
+  }
+  __device__ static uint4 pack(const float* v) {   // 8 values
+    return make_uint4(pack_bf162(v[0], v[1]), pack_bf162(v[2], v[3]), pack_bf162(v[4], v[5]), pack_bf162(v[6], v[7]));
   }
 };
 
@@ -438,6 +450,10 @@ static int run_conv(int kind, bool stem, const void* x, const void* w, const flo
     return stem ? launch_conv_tc_bn<__half, true>(x, w, scale, shift, resid, y, g, act, st)
                 : launch_conv_tc_bn<__half, false>(x, w, scale, shift, resid, y, g, act, st);
   }
+  if (kind == OP_BF16) {
+    return stem ? launch_conv_tc_bn<__nv_bfloat16, true>(x, w, scale, shift, resid, y, g, act, st)
+                : launch_conv_tc_bn<__nv_bfloat16, false>(x, w, scale, shift, resid, y, g, act, st);
+  }
   return stem ? launch_conv_tc_bn<float, true>(x, w, scale, shift, resid, y, g, act, st)
               : launch_conv_tc_bn<float, false>(x, w, scale, shift, resid, y, g, act, st);
 }
@@ -631,6 +647,9 @@ static int frontend_forward_body(int modality, const void* prepared, const float
     if (kind == OP_F16)
       AVSR_LAUNCH(maxpool3x3s2_kernel<__half>, grid_1d(n), 256, 0, st, (const __half*)buf[0], (__half*)buf[1], P.N,
                   P.stem.Ho, P.stem.Wo, P.H0, P.W0, 64);
+    else if (kind == OP_BF16)
+      AVSR_LAUNCH(maxpool3x3s2_kernel<__nv_bfloat16>, grid_1d(n), 256, 0, st, (const __nv_bfloat16*)buf[0],
+                  (__nv_bfloat16*)buf[1], P.N, P.stem.Ho, P.stem.Wo, P.H0, P.W0, 64);
     else
       AVSR_LAUNCH(maxpool3x3s2_kernel<float>, grid_1d(n), 256, 0, st, (const float*)buf[0], (float*)buf[1], P.N,
                   P.stem.Ho, P.stem.Wo, P.H0, P.W0, 64);
@@ -668,6 +687,9 @@ static int frontend_forward_body(int modality, const void* prepared, const float
   const long n = P.groups * 512;
   if (kind == OP_F16)
     AVSR_LAUNCH(mean_rows_kernel<__half>, grid_1d(n), 256, 0, st, (const __half*)buf[cur], out, P.groups, Pn, 512);
+  else if (kind == OP_BF16)
+    AVSR_LAUNCH(mean_rows_kernel<__nv_bfloat16>, grid_1d(n), 256, 0, st, (const __nv_bfloat16*)buf[cur], out, P.groups,
+                Pn, 512);
   else
     AVSR_LAUNCH(mean_rows_kernel<float>, grid_1d(n), 256, 0, st, (const float*)buf[cur], out, P.groups, Pn, 512);
   return AVSR_OK;
@@ -955,8 +977,7 @@ __global__ void ft_dgrad_weight_kernel(const float* __restrict__ w, void* __rest
     const int ky = ry + py - s * (dy0 + ty), kx = rx + px - s * (dx0 + tx);
     float v = 0.f;
     if (ky >= 0 && ky < KH && kx >= 0 && kx < KW) v = w[(((long)co * Cin + ci) * KH + ky) * KW + kx];
-    if (kind == OP_F16) reinterpret_cast<__half*>(dst)[i] = to_half_sat(v);
-    else reinterpret_cast<float*>(dst)[i] = kind == OP_TF32 ? round_tf32(v) : v;
+    store_kind1(dst, i, kind, v);
   }
 }
 
@@ -1258,6 +1279,9 @@ static int run_conv_raw(int kind, bool stem, const void* x, const void* w, const
   if (kind == OP_F16)
     return stem ? launch_conv_tc_bn<__half, true, true>(x, w, nullptr, nullptr, nullptr, z, g, 0, st)
                 : launch_conv_tc_bn<__half, false, true>(x, w, nullptr, nullptr, nullptr, z, g, 0, st);
+  if (kind == OP_BF16)
+    return stem ? launch_conv_tc_bn<__nv_bfloat16, true, true>(x, w, nullptr, nullptr, nullptr, z, g, 0, st)
+                : launch_conv_tc_bn<__nv_bfloat16, false, true>(x, w, nullptr, nullptr, nullptr, z, g, 0, st);
   return stem ? launch_conv_tc_bn<float, true, true>(x, w, nullptr, nullptr, nullptr, z, g, 0, st)
               : launch_conv_tc_bn<float, false, true>(x, w, nullptr, nullptr, nullptr, z, g, 0, st);
 }

@@ -13,8 +13,8 @@
 //                   storage, coalesced global stores (epilogue.cuh).  Two ordering mbarriers alternate the
 //                   warpgroups, one for main loops and one for epilogues, so one warpgroup's epilogue runs while the
 //                   other's main loop issues wgmma, and only one epilogue at a time uses the shared fp32 tile
-// Operand storage (template TOp): float = TF32 (8 elements per MMA-K) or __half (16 per MMA-K; same 10-bit mantissa,
-// half the bytes, twice the rate).  Out-of-bounds rows of edge tiles are zero-filled by TMA and masked in the
+// Operand storage (template TOp): float = TF32 (8 elements per MMA-K), __half or __nv_bfloat16 (16 per MMA-K; half the
+// bytes, twice the rate).  Out-of-bounds rows of edge tiles are zero-filled by TMA and masked in the
 // epilogue.  The tile width is chosen per problem by a small cost model (bytes through L2 vs tensor-pipe time).
 #include <cstring>
 
@@ -44,18 +44,23 @@ static EncodeTiledFn encode_tiled_fn() {
   return fn;
 }
 
+static CUtensorMapDataType tmap_dtype(int kind) {
+  return kind == OP_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                        : (kind == OP_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32);
+}
+
 int make_tmap_2d(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
-                 int esz) {
+                 int kind) {
   EncodeTiledFn enc = encode_tiled_fn();
   if (!enc) { set_error("cuTensorMapEncodeTiled unavailable (no CUDA driver?)"); return AVSR_E_CUDA; }
-  AVSR_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0 && (ld * esz) % 16 == 0 && box_rows <= 256 &&
-                   (esz == 4 || esz == 2),
+  const int esz = (int)operand_bytes(kind);
+  AVSR_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0 && (ld * esz) % 16 == 0 && box_rows <= 256,
                "tensor map: base/stride must be 16-byte aligned (ld=%llu, esz=%d)", (unsigned long long)ld, esz);
   cuuint64_t gdim[2] = {cols, rows};
   cuuint64_t gstr[1] = {ld * (uint64_t)esz};
   cuuint32_t box[2] = {(cuuint32_t)(128 / esz), box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, esz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
+  CUresult r = enc(map, tmap_dtype(kind), 2,
                    const_cast<void*>(base), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(2d) failed: CUresult %d", (int)r); return AVSR_E_CUDA; }
@@ -63,17 +68,18 @@ int make_tmap_2d(CUtensorMap* map, const void* base, uint64_t rows, uint64_t col
 }
 
 int make_tmap_3d(CUtensorMap* map, const void* base, uint64_t planes, uint64_t rows, uint64_t cols, uint64_t ld_row,
-                 uint64_t ld_plane, uint32_t box_rows, int esz) {
+                 uint64_t ld_plane, uint32_t box_rows, int kind) {
   EncodeTiledFn enc = encode_tiled_fn();
   if (!enc) { set_error("cuTensorMapEncodeTiled unavailable (no CUDA driver?)"); return AVSR_E_CUDA; }
+  const int esz = (int)operand_bytes(kind);
   AVSR_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0 && (ld_row * esz) % 16 == 0 &&
-                   (ld_plane * esz) % 16 == 0 && box_rows <= 256 && (esz == 4 || esz == 2),
+                   (ld_plane * esz) % 16 == 0 && box_rows <= 256,
                "tensor map 3d: base/strides must be 16-byte aligned");
   cuuint64_t gdim[3] = {cols, rows, planes};
   cuuint64_t gstr[2] = {ld_row * (uint64_t)esz, ld_plane * (uint64_t)esz};
   cuuint32_t box[3] = {(cuuint32_t)(128 / esz), box_rows, 1};
   cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(map, esz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3,
+  CUresult r = enc(map, tmap_dtype(kind), 3,
                    const_cast<void*>(base), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(3d) failed: CUresult %d", (int)r); return AVSR_E_CUDA; }
@@ -113,6 +119,13 @@ template <> struct OpTraits<__half> {
   template <int BN>
   __device__ static void mma(float* d, uint64_t a, uint64_t b, uint32_t acc) {
     if constexpr (BN == 64) wgmma_f16_n64(d, a, b, acc); else wgmma_f16_n128(d, a, b, acc);
+  }
+};
+template <> struct OpTraits<__nv_bfloat16> {
+  static constexpr int kElemsPerBlock = 64;  // 128 bytes of bf16
+  template <int BN>
+  __device__ static void mma(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+    if constexpr (BN == 64) wgmma_bf16_n64(d, a, b, acc); else wgmma_bf16_n128(d, a, b, acc);
   }
 };
 
@@ -585,8 +598,8 @@ static int launch_tc(const void* A, const void* Bw, int M, int N, int K, int spl
   constexpr int CS = CM * CN;
   auto kernel = gemm_tc_kernel<MODE, BN, TOp, CM, CN>;
   CUtensorMap tmA, tmB;
-  AVSR_TRY(make_tmap_2d(&tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)K, TC_BM / CN, (int)sizeof(TOp)));
-  AVSR_TRY(make_tmap_2d(&tmB, Bw, (uint64_t)N, (uint64_t)K, (uint64_t)K, BN / CM, (int)sizeof(TOp)));
+  AVSR_TRY(make_tmap_2d(&tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)K, TC_BM / CN, op_kind_of<TOp>()));
+  AVSR_TRY(make_tmap_2d(&tmB, Bw, (uint64_t)N, (uint64_t)K, (uint64_t)K, BN / CM, op_kind_of<TOp>()));
   AVSR_SET_MAX_SMEM(kernel, Cfg::kSmem);
   const int tiles_m = cdiv(M, TC_BM), tiles_n = cdiv(N, BN);
   if (CS > 1 || splits > kMaxSplits || tiles_m * tiles_n > kSplitCounters) {   // caller's workspace contract
@@ -751,11 +764,12 @@ static int dispatch_mode(int mode, const void* A, const void* Bw, int M, int N, 
 
 int gemm_tc(int mode, int opk, const void* A, const void* Bw, int M, int N, int K, const EpiParams& ep,
             cudaStream_t st) {
-  AVSR_REQUIRE(opk == OP_TF32 || opk == OP_F16, "gemm_tc: operand kind %d", opk);
-  const int ke = opk == OP_F16 ? 64 : 32;
+  AVSR_REQUIRE(opk == OP_TF32 || op16(opk), "gemm_tc: operand kind %d", opk);
+  const int ke = op16(opk) ? 64 : 32;
   AVSR_REQUIRE(K >= ke && K % ke == 0, "gemm_tc: K=%d must be a multiple of %d", K, ke);
   if (M <= 0 || N <= 0) return AVSR_OK;
   if (opk == OP_F16) return dispatch_mode<__half>(mode, A, Bw, M, N, K, ep, st);
+  if (opk == OP_BF16) return dispatch_mode<__nv_bfloat16>(mode, A, Bw, M, N, K, ep, st);
   return dispatch_mode<float>(mode, A, Bw, M, N, K, ep, st);
 }
 

@@ -10,9 +10,11 @@ from typing import Dict, Optional, Tuple
 import torch
 
 from . import _cabi
-from ._cabi import EncoderConfig, LayerParams, LAYER_FIELDS, PREC_F16, PREC_FP32, PREC_TF32, check, lib
+from ._cabi import EncoderConfig, LayerParams, LAYER_FIELDS, PREC_BF16, PREC_F16, PREC_FP32, PREC_TF32, check, lib
 
-PRECISIONS = {"fp32": PREC_FP32, "tf32": PREC_TF32, "f16": PREC_F16}
+#: precision name -> AVSR_PREC_* code.  "bf16" has f16's bytes and tensor-core rate with fp32's exponent range (unit
+#: roundoff 2^-8 against f16's 2^-11): the mode for activations that outgrow f16's +-65504.
+PRECISIONS = {"fp32": PREC_FP32, "tf32": PREC_TF32, "f16": PREC_F16, "bf16": PREC_BF16}
 
 
 def default_precision() -> str:
@@ -90,7 +92,8 @@ class PlanCache:
 
 
 class SaturationError(OverflowError):
-    """The fp16 operand path left its range (+-65504) for these weights / inputs: use precision "tf32" or "fp32"."""
+    """The fp16 operand path left its range (+-65504) for these weights / inputs: use precision "bf16" (fp32's range
+    at f16's speed), "tf32" or "fp32"."""
 
 
 class EncoderEngine:
@@ -206,7 +209,8 @@ class EncoderEngine:
                     if n:
                         raise SaturationError(
                             f"{n} fp16 operand value(s) saturated at +-65504 (or NaN) in this forward: the f16 path "
-                            "is outside its range for these weights / inputs -- use precision='tf32' or 'fp32'")
+                            "is outside its range for these weights / inputs -- use precision='bf16' (fp32's range), 'tf32' or "
+                            "'fp32'")
                 elif taps is None:
                     check(lib.avsr_encoder_forward(C.byref(self.cfg), prepared.data_ptr(), xs.data_ptr(), _ptr(lengths),
                                                    B, T, out.data_ptr(), ws.data_ptr(), ws.numel(), prec, st))

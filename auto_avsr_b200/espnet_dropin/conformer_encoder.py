@@ -151,7 +151,7 @@ class ConformerEncoder(torch.nn.Module):
 
     ``forward(xs (B,T,d) f32, masks (B,1,T) bool | None) -> (xs (B,T,d), masks)``: one call into the C ABI
     (``avsr_plan_forward``: CUDA-graph replay of the whole 12-layer schedule).  Extra attributes:
-    ``precision`` ("f16" default | "tf32" | "fp32" CUDA-core reference path), ``use_graph`` / ``graph_after`` (a
+    ``precision`` ("f16" default | "bf16" | "tf32" | "fp32" CUDA-core reference path), ``use_graph`` / ``graph_after`` (a
     shape runs on direct launches until seen ``graph_after`` times, then from its CUDA graph), ``assume_frozen`` (skip
     the per-call parameter-version check), ``check_saturation`` (diagnostic forward that raises ``SaturationError``
     when an fp16 operand hit +-65504; env AVSR_B200_CHECK_SAT=1), ``check_mask`` (verify that ``masks`` is a prefix

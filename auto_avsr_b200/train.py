@@ -10,7 +10,8 @@ The rel-pos attention core has a (correctness-first, fp32 CUDA-core) backward to
 SyncBatchNorm (train.py:31) is honoured: the per-channel sums are all-reduced between the library's passes.
 Not built: dropout on attention probabilities (the reference trains with 0.0).
 
-Backward GEMMs run with TF32 operands (fp32 range: gradients do not fit fp16's) unless ``precision="fp32"``."""
+Backward GEMMs run with TF32 operands (fp32 range: gradients do not fit fp16's) unless ``precision="fp32"``; a "bf16"
+forward keeps the TF32 backward too."""
 from __future__ import annotations
 
 import ctypes as C

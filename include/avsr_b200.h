@@ -40,9 +40,12 @@ enum {
 enum {
   AVSR_PREC_FP32 = 0,  /* CUDA-core fp32 FMA kernels: the on-device exact reference path (slow) */
   AVSR_PREC_TF32 = 1,  /* wgmma .tf32: operands kept as fp32 rounded to TF32, fp32 accumulate */
-  AVSR_PREC_F16 = 2    /* wgmma .f16: operands stored as IEEE half (same 10-bit mantissa as TF32, saturating
+  AVSR_PREC_F16 = 2,   /* wgmma .f16: operands stored as IEEE half (same 10-bit mantissa as TF32, saturating
                           conversion), fp32 accumulate; residual stream, LayerNorm, softmax, conv stay fp32.
                           Half the operand bytes and twice the MMA rate of TF32: the product path. */
+  AVSR_PREC_BF16 = 16  /* wgmma .bf16: operands stored as bfloat16 (7-bit mantissa, fp32's 8-bit exponent, round to
+                          nearest even, no saturation), fp32 accumulate; the bytes and rate of AVSR_PREC_F16 with
+                          fp32's range.  Every *_bytes entry returns its AVSR_PREC_F16 value. */
 };
 
 /* Hyper-parameters hard-wired in E2E.__init__ (espnet/nets/pytorch_backend/e2e_asr_conformer.py:33-39):
@@ -106,7 +109,8 @@ int avsr_encoder_forward(const AvsrEncoderConfig *cfg, const void *prepared, con
                          size_t workspace_bytes, int precision, void *stream);
 
 /* Diagnostic variant of avsr_encoder_forward for AVSR_PREC_F16: fp16 operand stores saturate at +-65504
- * (cvt.rn.satfinite) where the fp32 reference would carry on.  This entry scans every operand tensor (LayerNorm
+ * (cvt.rn.satfinite) where the fp32 reference would carry on.  The other precisions cannot saturate (AVSR_PREC_BF16
+ * has fp32's range): for them this is the plain forward and *saturated stays 0.  This entry scans every operand tensor (LayerNorm
  * outputs, FFN hidden, q/k/v, rel-pos table, attention context, conv activations) right after its producer and
  * leaves in *saturated (DEVICE uint64, zeroed by the call) the number of elements that sit at the saturation value or
  * are NaN.  0 == the fp16 path stayed in range for these weights and inputs.  Direct launches, ~2x slower. */
@@ -137,15 +141,15 @@ int avsr_layernorm(const float *x, const float *gamma, const float *beta, float 
 
 /* torch.nn.Linear: y = x W^T + b, optionally ReLU (positionwise_feed_forward.py:30) and/or
  * y = resid + alpha*y (conformer_encoder.py:115,140,150,158).  x (rows,k); w (n,k); bias (n) or NULL;
- * resid (rows,n) or NULL (may alias y).  All tensors fp32; for AVSR_PREC_F16 x and w are first converted to
- * half into `workspace` (>= avsr_linear_workspace_bytes), for AVSR_PREC_TF32 the tensor core truncates them. */
+ * resid (rows,n) or NULL (may alias y).  All tensors fp32; for AVSR_PREC_F16 / BF16 x and w are first converted
+ * to half / bfloat16 into `workspace` (>= avsr_linear_workspace_bytes), for AVSR_PREC_TF32 the tensor core truncates them. */
 size_t avsr_linear_workspace_bytes(int rows, int n, int k, int precision);
 int avsr_linear(const float *x, const float *w, const float *bias, const float *resid, float alpha,
                 int relu, float *y, int rows, int n, int k, int precision, void *workspace,
                 size_t workspace_bytes, void *stream);
 
 /* A projection GEMM exactly as the encoder runs it: x and w ALREADY in `precision`'s operand storage (fp32 for
- * FP32/TF32, IEEE half for F16); y = [resid + alpha *] act(x W^T + b), stored as an operand (y_is_operand != 0,
+ * FP32/TF32, IEEE half for F16, bfloat16 for BF16); y = [resid + alpha *] act(x W^T + b), stored as an operand (y_is_operand != 0,
  * e.g. the FFN hidden) or as fp32 (the residual stream).  Used by bench.py / the tile sweep to time the dominant
  * kernel in isolation (roofline), not by the modules. */
 int avsr_linear_operands(const void *x_op, const void *w_op, const float *bias, const float *resid, float alpha,
@@ -455,7 +459,7 @@ int avsr_ctc_prefix_batch_score(const float *logp, const int32_t *lengths_dev, i
 
 /* ---- ResNet front-ends, inference (eval-mode BatchNorm): Conv3dResNet (frontend/resnet.py:176-233) and
  * Conv1dResNet (frontend/resnet1d.py:204-234) with relu_type "swish".  Activations are channels-last in the precision's
- * operand storage: (frames, H, W, C) for video, (utterances, L, C) for audio.  AVSR_PREC_TF32 and AVSR_PREC_F16 run the
+ * operand storage: (frames, H, W, C) for video, (utterances, L, C) for audio.  AVSR_PREC_TF32, F16 and BF16 run the
  * trunk convolutions and both stems as implicit GEMMs on wgmma; AVSR_PREC_FP32 runs a CUDA-core direct convolution
  * (the exact reference path). */
 enum { AVSR_FRONTEND_VIDEO = 0, AVSR_FRONTEND_AUDIO = 1 };
@@ -510,8 +514,8 @@ int avsr_conv_bn_act(const float *x, const float *w, const float *scale, const f
  * 1); 1 the video stem, x (N = B * T frames, H, W) with T frames per utterance, w (64, 1, 5, 7, 7); 2 the audio stem,
  * x (N, W) samples with W a multiple of 640, w (64, 1, 80).  C_in, C_out and KH, KW, stride are ignored for the stems.
  *
- * avsr_frontend_train_conv_fwd: z (output pixels, C_out) = conv(x, w) in `precision` (TF32 / F16 on wgmma, FP32 on CUDA
- * cores), and stats (3, C_out) fp64 = each channel's (count, mean, M2) over all output pixels, merged in a fixed order
+ * avsr_frontend_train_conv_fwd: z (output pixels, C_out) = conv(x, w) in `precision` (TF32 / F16 / BF16 on wgmma, FP32 on
+ * CUDA cores), and stats (3, C_out) fp64 = each channel's (count, mean, M2) over all output pixels, merged in a fixed order
  * with Chan's formula. */
 size_t avsr_frontend_train_conv_workspace_bytes(int stem, int N, int T, int H, int W, int C_in, int C_out, int KH,
                                                 int KW, int stride, int precision);
@@ -537,14 +541,14 @@ int avsr_frontend_train_bn_bwd_dx(const float *z, const float *dy, const float *
                                   const float *gamma, const float *beta, const float *resid, int act, const float *sums,
                                   float inv_count, float *dz, float *dres, long rows, int C, void *stream);
 /* Input gradient of a trunk conv: dx (N, H, W, C_in) from dz (N, Ho, Wo, C_out), one stride-1 implicit GEMM per parity
- * class of the input (TF32 / F16 on wgmma, FP32 on CUDA cores). */
+ * class of the input (TF32 / F16 / BF16 on wgmma, FP32 on CUDA cores). */
 size_t avsr_frontend_train_dgrad_workspace_bytes(int N, int H, int W, int C_in, int C_out, int KH, int KW, int stride,
                                                  int precision);
 int avsr_frontend_train_conv_dgrad(const float *dz, const float *w, float *dx, int N, int H, int W, int C_in, int C_out,
                                    int KH, int KW, int stride, void *workspace, size_t workspace_bytes, int precision,
                                    void *stream);
 /* Weight gradient dw (torch layout, like w) = sum over output pixels of dz x im2col(x): wgmma with TF32 operands
- * (AVSR_PREC_TF32 / AVSR_PREC_F16) or fp32 on CUDA cores (AVSR_PREC_FP32); the pixel axis is split across the SMs and
+ * (AVSR_PREC_TF32 / F16 / BF16) or fp32 on CUDA cores (AVSR_PREC_FP32); the pixel axis is split across the SMs and
  * the partials are summed in a fixed order. */
 size_t avsr_frontend_train_wgrad_workspace_bytes(int stem, int N, int T, int H, int W, int C_in, int C_out, int KH,
                                                  int KW, int stride);

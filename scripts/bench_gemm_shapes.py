@@ -27,7 +27,7 @@ sys.path.insert(0, %(root)r)
 from auto_avsr_b200 import _cabi
 from auto_avsr_b200.engine import PRECISIONS
 dev = torch.device("cuda:0"); prec = %(prec)r
-tdt = torch.float16 if prec == "f16" else torch.float32
+tdt = {"f16": torch.float16, "bf16": torch.bfloat16}.get(prec, torch.float32)
 res = {}
 for name, M, N, K, relu, opdest, resid in %(shapes)r:
     g = torch.Generator().manual_seed(7)
@@ -82,11 +82,11 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--lib", action="append", default=[], help="NAME=PATH of a libavsr_b200.so build")
     ap.add_argument("--tiles", nargs="*", default=["auto"])
-    ap.add_argument("--precision", default="f16", choices=["f16", "tf32"])
+    ap.add_argument("--precision", default="f16", choices=["f16", "bf16", "tf32"])
     args = ap.parse_args()
     libs = [tuple(s.split("=", 1)) for s in args.lib] or [("this", os.path.join(ROOT, "auto_avsr_b200", "csrc",
                                                                                    "libavsr_b200.so"))]
-    esz = 2 if args.precision == "f16" else 4
+    esz = 2 if args.precision in ("f16", "bf16") else 4
     rows = []
     for name, path in libs:
         for tile in args.tiles:

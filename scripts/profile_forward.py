@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """Per-kernel attribution of the encoder forward on the GPU, for one or more builds of the library.
 
-    python scripts/profile_forward.py [--lib NAME=PATH ...] [--shapes S2 S2r S3 S4] [--precision f16 tf32]
+    python scripts/profile_forward.py [--lib NAME=PATH ...] [--shapes S2 S2r S3 S4] [--precision f16 bf16 tf32]
                                       [--steps N] [--dump DIR]
 
 Each build runs in its own process (AVSR_B200_LIB selects it, as in scripts/bench_gemm_shapes.py).  For every shape and
@@ -27,7 +27,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ATTN = "attention_wg_kernel"   # the rel-pos attention kernel (csrc/attention_tc.cu)
-PEAK_TFLOPS = {"f16": 989.0, "tf32": 495.0}   # NVIDIA H100 SXM data sheet, dense, at a 700 W power limit
+PEAK_TFLOPS = {"f16": 989.0, "bf16": 989.0, "tf32": 495.0}   # NVIDIA H100 SXM data sheet, dense, at a 700 W power limit
 
 
 def attention_flops(lengths, heads=12):
@@ -123,7 +123,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--lib", action="append", default=[], help="NAME=PATH of a libavsr_b200.so build")
     ap.add_argument("--shapes", nargs="*", default=["S2", "S2r", "S3", "S4"])
-    ap.add_argument("--precision", nargs="*", default=["f16"], choices=["f16", "tf32"])
+    ap.add_argument("--precision", nargs="*", default=["f16"], choices=["f16", "bf16", "tf32"])
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--top", type=int, default=12, help="kernels listed per shape")
     ap.add_argument("--dump", metavar="DIR", default=None)
