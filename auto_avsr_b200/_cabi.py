@@ -128,6 +128,9 @@ SIGNATURES = {
     "avsr_colsum": (_I, [_P, _P, _I, _I, _P, _Z, _P]),
     "avsr_transpose": (_I, [_P, _P, _I, _I, C.c_long, _P]),
     "avsr_relu_bwd": (_I, [_P, _P, _P, C.c_long, _P]),
+    "avsr_pack_operand": (_I, [_P, _P, _I, _I, C.c_long, _I, _I, _P]),
+    "avsr_linear_bwd_bf16_workspace_bytes": (_Z, [_I, _I, _I]),
+    "avsr_linear_bwd_bf16": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _Z, _P]),
     "avsr_glu_fwd": (_I, [_P, _P, C.c_long, _I, _P]),
     "avsr_glu_bwd": (_I, [_P, _P, _P, C.c_long, _I, _P]),
     "avsr_dwconv_raw": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _Z, _P]),
@@ -137,6 +140,8 @@ SIGNATURES = {
     "avsr_dwconv_wgrad": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _Z, _P]),
     "avsr_relpos_attention_bwd_workspace_bytes": (_Z, [_I, _I, _I]),
     "avsr_relpos_attention_bwd": (_I, [_P] * 14 + [_I, _I, _I, _P, _Z, _P]),
+    "avsr_relpos_attention_bwd_tc_workspace_bytes": (_Z, [_I, _I, _I, _I]),
+    "avsr_relpos_attention_bwd_tc": (_I, [_P] * 14 + [_I, _I, _I, _I, _P, _Z, _P]),
     "avsr_ctc_loss_state_bytes": (_Z, [_I, _I, _I]),
     "avsr_ctc_loss_fwd": (_I, [_P, C.c_long, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _Z, _P]),
     "avsr_ctc_loss_bwd": (_I, [_P, C.c_long, _P, _P, _I, _I, _I, _I, _P, _P, _Z, _P, C.c_long, _P]),

@@ -448,6 +448,9 @@ int attention_simt(const float* qu, const float* qv, const float* kk, const floa
 int attention_tc(const float* qu, const float* qv, const float* kk, const float* vt, const float* pos,
                  const int32_t* lengths, float* ctx, int B, int T, int H, int Tp, int Rp, int round_out,
                  cudaStream_t st);
+// (B,T,H*64) fp32 [+ bias (H*64)] -> (B,H,T,64) in operand storage `kind`, or (B,H,64,Tp) when transpose != 0 (encoder.cu)
+int launch_split_heads(const float* src, const float* bias, void* dst, int B, int T, int H, int Tp, int transpose, int kind,
+                       cudaStream_t st);
 // 2-byte operands (attention_tc.cu), kind OP_F16 or OP_BF16: qu, qv, kk, vv all (B,H,T,64) (V in its natural
 // layout); ctx (B*T, H*64) in the same storage
 int attention_op16(int kind, const void* qu, const void* qv, const void* kk, const void* vv, const void* pos,

@@ -793,6 +793,17 @@ __global__ void split_heads_kernel(const float* __restrict__ src, const float* _
   }
 }
 
+}  // extern "C"
+
+int avsr::launch_split_heads(const float* src, const float* bias, void* dst, int B, int T, int H, int Tp, int transpose,
+                             int kind, cudaStream_t st) {
+  split_heads_kernel<<<132 * 4, 256, 0, st>>>(src, bias, dst, B, T, H, Tp, transpose, kind);
+  AVSR_CHECK_LAUNCH();
+  return AVSR_OK;
+}
+
+extern "C" {
+
 __global__ void op_to_float_kernel(const void* __restrict__ src, float* __restrict__ dst, long n, int kind) {
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x)
     dst[i] = load_kind1(src, i, kind);
@@ -820,12 +831,11 @@ int avsr_relpos_attention(const float* q, const float* k, const float* v, const 
         *pos = cv.take((size_t)R * D), *ctxh = cv.take(N * D);
   const int blocks = 132 * 4;
   if (Tp != T) AVSR_CUDA_TRY(cudaMemsetAsync(vt, 0, (size_t)B * D * Tp * sizeof(float), st));
-  split_heads_kernel<<<blocks, 256, 0, st>>>(q, pos_bias_u, qu, B, T, H, Tp, 0, kind); AVSR_CHECK_LAUNCH();
-  split_heads_kernel<<<blocks, 256, 0, st>>>(q, pos_bias_v, qv, B, T, H, Tp, 0, kind); AVSR_CHECK_LAUNCH();
-  split_heads_kernel<<<blocks, 256, 0, st>>>(k, nullptr, kk, B, T, H, Tp, 0, kind); AVSR_CHECK_LAUNCH();
-  split_heads_kernel<<<blocks, 256, 0, st>>>(v, nullptr, vt, B, T, H, Tp, prec16(precision) ? 0 : 1, kind);
-  AVSR_CHECK_LAUNCH();
-  split_heads_kernel<<<blocks, 256, 0, st>>>(p, nullptr, pos, 1, R, H, R, 0, kind); AVSR_CHECK_LAUNCH();
+  AVSR_TRY(launch_split_heads(q, pos_bias_u, qu, B, T, H, Tp, 0, kind, st));
+  AVSR_TRY(launch_split_heads(q, pos_bias_v, qv, B, T, H, Tp, 0, kind, st));
+  AVSR_TRY(launch_split_heads(k, nullptr, kk, B, T, H, Tp, 0, kind, st));
+  AVSR_TRY(launch_split_heads(v, nullptr, vt, B, T, H, Tp, prec16(precision) ? 0 : 1, kind, st));
+  AVSR_TRY(launch_split_heads(p, nullptr, pos, 1, R, H, R, 0, kind, st));
   if (prec16(precision)) {
     AVSR_TRY(attention_op16(kind, qu, qv, kk, vt, pos, lengths, ctxh, B, T, H, R, st));
     op_to_float_kernel<<<blocks, 256, 0, st>>>(ctxh, ctx, (long)N * D, kind);

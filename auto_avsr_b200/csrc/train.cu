@@ -127,6 +127,34 @@ __global__ void transpose_kernel(const float* __restrict__ src, float* __restric
   }
 }
 
+// ------------------------------------------------------------------ fp32 -> bf16 GEMM operands with zero padding
+// transposed: (rows x cols) -> (cols x ld_dst), dst[c][r]; tiles of 32 x 32 through shared memory, the padding columns
+// [rows, ld_dst) written as zeros
+__global__ void pack_bf16_t_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, int rows, int cols,
+                                   long ld_dst) {
+  __shared__ float tile[32][33];
+  const int c0 = blockIdx.y * 32, r0 = blockIdx.x * 32;
+  for (int j = threadIdx.y; j < 32; j += 8) {
+    const int r = r0 + j, c = c0 + threadIdx.x;
+    tile[j][threadIdx.x] = (r < rows && c < cols) ? src[(long)r * cols + c] : 0.f;
+  }
+  __syncthreads();
+  for (int j = threadIdx.y; j < 32; j += 8) {
+    const int c = c0 + j, r = r0 + threadIdx.x;
+    if (c < cols && r < ld_dst) dst[(long)c * ld_dst + r] = __float2bfloat16_rn(tile[threadIdx.x][j]);
+  }
+}
+// not transposed: (rows x cols) -> (rows x ld_dst), the padding columns [cols, ld_dst) written as zeros
+__global__ void pack_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, int rows, int cols,
+                                 long ld_dst) {
+  const long total = (long)rows * ld_dst;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const long r = i / ld_dst;
+    const int c = (int)(i - r * ld_dst);
+    dst[i] = __float2bfloat16_rn(c < cols ? src[r * cols + c] : 0.f);
+  }
+}
+
 // ------------------------------------------------------------------ ReLU backward: dx = dy * (y > 0)
 __global__ void relu_bwd_kernel(const float4* __restrict__ y, const float4* __restrict__ dy, float4* __restrict__ dx, long n4) {
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n4; i += (long)gridDim.x * blockDim.x) {
@@ -334,6 +362,54 @@ int avsr_transpose(const float* src, float* dst, int rows, int cols, long ld_dst
   if (rows <= 0 || cols <= 0) return AVSR_OK;
   transpose_kernel<<<dim3(cdiv(cols, 32), cdiv(rows, 32)), dim3(32, 8), 0, reinterpret_cast<cudaStream_t>(stream)>>>(src, dst, rows, cols, ld_dst);
   AVSR_CHECK_LAUNCH();
+  return AVSR_OK;
+}
+
+int avsr_pack_operand(const float* src, void* dst, int rows, int cols, long ld_dst, int transpose, int precision,
+                      void* stream) {
+  AVSR_REQUIRE(src && dst, "NULL argument");
+  AVSR_REQUIRE(precision == AVSR_PREC_BF16, "pack_operand: precision %d is not built; AVSR_PREC_BF16 only", precision);
+  AVSR_REQUIRE(rows >= 0 && cols >= 0 && ld_dst >= (transpose ? rows : cols), "pack_operand: bad rows=%d cols=%d ld=%ld",
+               rows, cols, ld_dst);
+  if (rows <= 0 || cols <= 0) return AVSR_OK;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(dst);
+  if (transpose)
+    pack_bf16_t_kernel<<<dim3((unsigned)((ld_dst + 31) / 32), cdiv(cols, 32)), dim3(32, 8), 0, st>>>(src, d, rows, cols,
+                                                                                                        ld_dst);
+  else
+    pack_bf16_kernel<<<132 * 4, 256, 0, st>>>(src, d, rows, cols, ld_dst);
+  AVSR_CHECK_LAUNCH();
+  return AVSR_OK;
+}
+
+static size_t pad64(int v) { return ((size_t)v + 63) / 64 * 64; }
+
+size_t avsr_linear_bwd_bf16_workspace_bytes(int rows, int n, int k) {
+  if (rows <= 0 || n <= 0 || k <= 0) return 256;
+  return align_up((size_t)rows * pad64(n) * 2, 256) + align_up((size_t)k * pad64(n) * 2, 256) +
+         align_up((size_t)n * pad64(rows) * 2, 256) + align_up((size_t)k * pad64(rows) * 2, 256);
+}
+
+int avsr_linear_bwd_bf16(const float* dy, const float* x, const float* w, float* dx, float* dw, int rows, int n, int k,
+                         void* workspace, size_t workspace_bytes, void* stream) {
+  AVSR_REQUIRE(dy && workspace && (dx || dw) && (!dx || w) && (!dw || x), "NULL argument");
+  AVSR_REQUIRE(rows > 0 && n > 0 && k > 0, "linear_bwd_bf16: bad rows=%d n=%d k=%d", rows, n, k);
+  AVSR_REQUIRE_BYTES(avsr_linear_bwd_bf16_workspace_bytes(rows, n, k), workspace_bytes, "linear_bwd_bf16 workspace");
+  const long np = (long)pad64(n), rp = (long)pad64(rows);
+  Carver cv{reinterpret_cast<char*>(workspace)};
+  __nv_bfloat16 *dy_op = cv.take<__nv_bfloat16>((size_t)rows * np), *wt_op = cv.take<__nv_bfloat16>((size_t)k * np),
+                *dyt_op = cv.take<__nv_bfloat16>((size_t)n * rp), *xt_op = cv.take<__nv_bfloat16>((size_t)k * rp);
+  if (dx) {   // dX (rows, k) = dY W = dY (W^T)^T: K = n
+    AVSR_TRY(avsr_pack_operand(dy, dy_op, rows, n, np, 0, AVSR_PREC_BF16, stream));
+    AVSR_TRY(avsr_pack_operand(w, wt_op, n, k, np, 1, AVSR_PREC_BF16, stream));
+    AVSR_TRY(avsr_linear_operands(dy_op, wt_op, nullptr, nullptr, 1.0f, dx, rows, k, (int)np, 0, 0, AVSR_PREC_BF16, stream));
+  }
+  if (dw) {   // dW (n, k) = dY^T X = dY^T (X^T)^T: K = rows
+    AVSR_TRY(avsr_pack_operand(dy, dyt_op, rows, n, rp, 1, AVSR_PREC_BF16, stream));
+    AVSR_TRY(avsr_pack_operand(x, xt_op, rows, k, rp, 1, AVSR_PREC_BF16, stream));
+    AVSR_TRY(avsr_linear_operands(dyt_op, xt_op, nullptr, nullptr, 1.0f, dw, n, k, (int)rp, 0, 0, AVSR_PREC_BF16, stream));
+  }
   return AVSR_OK;
 }
 

@@ -255,6 +255,9 @@ def source_attention_train(m, x, memory, mem_lengths, precision: str):
 
 def decoder_layer_train(layer, x, tgt_lengths, memory, mem_lengths, precision: str):
     """DecoderLayer.forward (transformer_decoder.py:65-128): pre-norm, concat_after=False, no cache."""
+    if getattr(layer.feed_forward, "backward_precision", None) is not None:
+        raise ValueError("feed_forward.backward_precision is set on a decoder layer: the bf16 backward is an encoder "
+                         "option; the decoder trains with the default backward")
     h = LayerNormFn.apply(x, layer.norm1.weight, layer.norm1.bias)
     x = x + layer.dropout(self_attention_train(layer.self_attn, h, tgt_lengths, precision))
     h = LayerNormFn.apply(x, layer.norm2.weight, layer.norm2.bias)

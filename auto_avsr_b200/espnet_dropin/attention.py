@@ -55,6 +55,7 @@ class RelPositionMultiHeadedAttention(nn.Module):
         torch.nn.init.xavier_uniform_(self.pos_bias_u)
         torch.nn.init.xavier_uniform_(self.pos_bias_v)
         self.precision: Optional[str] = None
+        self.backward_precision: Optional[str] = None     # None (default backward) | "bf16"; see train.py
 
     def forward(self, query, key, value, pos_emb, mask, residual: Optional[torch.Tensor] = None):
         """query (B,T,d); key/value must be the same tensor (self-attention) or None; pos_emb (1,2T-1,d);
@@ -67,8 +68,8 @@ class RelPositionMultiHeadedAttention(nn.Module):
         prec = self.precision or default_precision()
         B, T, _ = query.shape
         if self.training:                       # forward + backward in libavsr_b200 (auto_avsr_b200/train.py)
-            from ..train import attention_train
-            y = attention_train(self, query, pos_emb, mask, prec)
+            from ..train import attention_train, module_backward_precision
+            y = attention_train(self, query, pos_emb, mask, prec, module_backward_precision(self))
             return y if residual is None else residual + y
         q = ops.linear(query, self.linear_q.weight, self.linear_q.bias, precision=prec)
         k = ops.linear(query, self.linear_k.weight, self.linear_k.bias, precision=prec)

@@ -5,12 +5,13 @@ reference (espnet/nets/pytorch_backend/encoder/conformer_encoder.py:19,38,186), 
 (e2e_asr_conformer.py:33-39), ``lightning.py`` and the released checkpoints keep working unchanged;
 only ``forward`` differs: on a CUDA tensor it runs the hand-written sm_90a kernels of libavsr_b200.so.
 
-Scope: inference forward (``eval()``: one fused C-ABI call, outputs carry no autograd graph) plus the FIRST SLICE of
-training (SURVEY.md section 8f item 2): ``LayerNorm``, ``PositionwiseFeedForward`` and ``ConvolutionModule`` run forward
-AND backward in libavsr_b200 (auto_avsr_b200/train.py: batch-statistics BatchNorm incl. running-stat update, dgrad /
-wgrad as tensor-core GEMMs, gradients on the original Parameters).  The rel-pos attention backward is not built yet, so
-``RelPositionMultiHeadedAttention`` / ``EncoderLayer`` / ``ConformerEncoder`` still raise ``NotImplementedError`` in
-``train()`` instead of silently falling back to PyTorch.  CPU tensors raise too: there is no CPU path in this package.
+Scope: inference forward (``eval()``: one fused C-ABI call, outputs carry no autograd graph) and training
+(SURVEY.md section 8f item 2): in ``train()`` every module -- ``LayerNorm``, ``PositionwiseFeedForward``,
+``ConvolutionModule``, ``RelPositionMultiHeadedAttention`` (the rel-pos attention core included), ``EncoderLayer`` and
+``ConformerEncoder`` -- runs forward AND backward in libavsr_b200 (auto_avsr_b200/train.py: batch-statistics BatchNorm
+incl. running-stat update, dgrad / wgrad as tensor-core GEMMs, gradients on the original Parameters).  Attention
+dropout > 0 raises ``NotImplementedError`` instead of silently falling back to PyTorch.  CPU tensors raise too: there is
+no CPU path in this package.
 """
 from __future__ import annotations
 
@@ -51,6 +52,7 @@ class ConvolutionModule(torch.nn.Module):
         self.pointwise_cov2 = torch.nn.Conv1d(channels, channels, 1, bias=bias)
         self.activation = torch.nn.SiLU(inplace=True)
         self.precision: Optional[str] = None
+        self.backward_precision: Optional[str] = None     # None (default backward) | "bf16"; see train.py
 
     def forward(self, x, residual: Optional[torch.Tensor] = None):
         """x (B, T, C) -> (B, T, C); ``residual`` (extension) is added in the last GEMM's epilogue."""
@@ -60,8 +62,8 @@ class ConvolutionModule(torch.nn.Module):
             # (eval mode = the inference kernels below; their outputs carry no autograd graph)
             if not x.is_cuda:
                 raise RuntimeError("ConvolutionModule: CPU tensor; auto_avsr_b200 has no CPU fallback")
-            from ..train import conv_module_train
-            y = conv_module_train(self, x, prec)
+            from ..train import conv_module_train, module_backward_precision
+            y = conv_module_train(self, x, prec, module_backward_precision(self))
             return y if residual is None else residual + y
         C = self.pointwise_cov2.weight.size(0)
         g = ops.pointwise_glu(x, self.pointwise_cov1.weight, self.pointwise_cov1.bias, prec)
@@ -151,7 +153,9 @@ class ConformerEncoder(torch.nn.Module):
 
     ``forward(xs (B,T,d) f32, masks (B,1,T) bool | None) -> (xs (B,T,d), masks)``: one call into the C ABI
     (``avsr_plan_forward``: CUDA-graph replay of the whole 12-layer schedule).  Extra attributes:
-    ``precision`` ("f16" default | "bf16" | "tf32" | "fp32" CUDA-core reference path), ``use_graph`` / ``graph_after`` (a
+    ``precision`` ("f16" default | "bf16" | "tf32" | "fp32" CUDA-core reference path), ``backward_precision`` (training
+    only: None = the default backward, TF32 GEMMs and the fp32 attention backward; "bf16" = bf16 backward GEMMs and the
+    tensor-core attention backward; env AVSR_B200_BWD_PRECISION), ``use_graph`` / ``graph_after`` (a
     shape runs on direct launches until seen ``graph_after`` times, then from its CUDA graph), ``assume_frozen`` (skip
     the per-call parameter-version check), ``check_saturation`` (diagnostic forward that raises ``SaturationError``
     when an fp16 operand hit +-65504; env AVSR_B200_CHECK_SAT=1), ``check_mask`` (verify that ``masks`` is a prefix
@@ -183,6 +187,7 @@ class ConformerEncoder(torch.nn.Module):
                                 and not zero_triu and attention_dim == attention_heads * 64)
         self._cfg = (attention_dim, attention_heads, linear_units, num_blocks, cnn_module_kernel)
         self.precision: Optional[str] = None
+        self.backward_precision: Optional[str] = None
         self.use_graph = True
         self.graph_after: Optional[int] = None      # None: EncoderEngine.GRAPH_AFTER (3); 1: capture at first sight
         self.assume_frozen = False
@@ -235,9 +240,13 @@ class ConformerEncoder(torch.nn.Module):
         if self.training:
             # training (SURVEY.md 8f #2): module by module under autograd, every module's forward AND backward in
             # libavsr_b200 (auto_avsr_b200/train.py); MultiSequential draws the reference's CPU uniforms itself
+            from ..train import resolve_backward_precision
+            backward = resolve_backward_precision(self.backward_precision)
             for m in self.modules():
                 if hasattr(m, "precision") and m is not self and m.precision is None:
                     m.precision = precision
+                if hasattr(m, "backward_precision") and m is not self:
+                    m._inherited_backward_precision = backward   # this forward's value; a module's own setting wins
             xs, masks_ = self.embed(xs), masks
             xs, masks_ = self.encoders(xs, masks_)
             if isinstance(xs, tuple):

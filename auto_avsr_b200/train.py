@@ -11,17 +11,20 @@ SyncBatchNorm (train.py:31) is honoured: the per-channel sums are all-reduced be
 Not built: dropout on attention probabilities (the reference trains with 0.0).
 
 Backward GEMMs run with TF32 operands (fp32 range: gradients do not fit fp16's) unless ``precision="fp32"``; a "bf16"
-forward keeps the TF32 backward too."""
+forward keeps the TF32 backward too.  The encoder modules take an opt-in ``backward_precision="bf16"`` (env
+AVSR_B200_BWD_PRECISION): every backward GEMM then gets bf16 operands (fp32's exponent range, an 8-bit mantissa) and the
+attention core's backward runs on the tensor cores (avsr_relpos_attention_bwd_tc)."""
 from __future__ import annotations
 
 import ctypes as C
+import os
 from typing import Optional
 
 import torch
 
 from . import ops
 from ._cabi import check, lib
-from .engine import _ptr, _stream_handle, require_cuda
+from .engine import PRECISIONS, _ptr, _stream_handle, require_cuda
 
 _WS = {}
 
@@ -40,6 +43,28 @@ def _c(t: torch.Tensor) -> torch.Tensor:
 
 def bwd_precision(precision: str) -> str:
     return "fp32" if precision == "fp32" else "tf32"
+
+
+BACKWARD_PRECISIONS = (None, "bf16")
+
+
+def resolve_backward_precision(value: Optional[str]) -> Optional[str]:
+    """A module's ``backward_precision``: ``value``, else env AVSR_B200_BWD_PRECISION, else None (the default backward,
+    ``bwd_precision``).  "bf16" is the only other choice: an f16 backward is not offered, gradients overflow its range."""
+    if value is None:
+        value = os.environ.get("AVSR_B200_BWD_PRECISION") or None
+    if value not in BACKWARD_PRECISIONS:
+        raise ValueError(f"backward_precision={value!r}: expected None (default backward) or 'bf16'; f16 is not "
+                         "offered (gradients overflow its 65504 range)")
+    return value
+
+
+def module_backward_precision(m) -> Optional[str]:
+    """``m.backward_precision`` if set, else what the enclosing ConformerEncoder passed down for this forward."""
+    v = getattr(m, "backward_precision", None)
+    if v is None:
+        v = getattr(m, "_inherited_backward_precision", None)
+    return resolve_backward_precision(v)
 
 
 # ------------------------------------------------------------------------------------------------ raw ops
@@ -79,6 +104,21 @@ def transpose_padded(x2d, pad_to: int = 32):
     return out
 
 
+def linear_bwd_bf16(dy2, x2, w2, want_dx: bool, want_dw: bool):
+    """avsr_linear_bwd_bf16: dX = dY W and dW = dY^T X on bf16 operands (transposed, padded to 64 along K and converted
+    in one pass each inside the library), one call for both -> (dx (rows, k) | None, dw (n, k) | None)."""
+    dy2, x2, w2 = _c(dy2), _c(x2), _c(w2)
+    rows, n = dy2.shape
+    k = w2.size(1)
+    dx = torch.empty(rows, k, dtype=torch.float32, device=dy2.device) if want_dx else None
+    dw = torch.empty(n, k, dtype=torch.float32, device=dy2.device) if want_dw else None
+    ws = _workspace(dy2.device, int(lib.avsr_linear_bwd_bf16_workspace_bytes(rows, n, k)))
+    with torch.cuda.device(dy2.device):
+        check(lib.avsr_linear_bwd_bf16(dy2.data_ptr(), x2.data_ptr(), w2.data_ptr(), _ptr(dx), _ptr(dw), rows, n, k,
+                                       ws.data_ptr(), ws.numel(), _stream_handle(dy2.device)))
+    return dx, dw
+
+
 def relu_bwd(y, dy):
     y, dy = _c(y), _c(dy)
     dx = torch.empty_like(dy)
@@ -110,11 +150,12 @@ class LinearFn(torch.autograd.Function):
     db = column sums of dY."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, relu: bool, precision: str):
+    def forward(ctx, x, weight, bias, relu: bool, precision: str, backward: Optional[str] = None):
         require_cuda(x, "Linear input")
         w2 = weight.reshape(weight.size(0), -1)          # Conv1d(k=1) weights carry a trailing 1
         y = ops.linear(x, w2, bias, relu=relu, precision=precision)
         ctx.relu, ctx.precision, ctx.wshape = relu, precision, weight.shape
+        ctx.backward = backward
         ctx.save_for_backward(x, w2, y if relu else None)
         ctx.has_bias = bias is not None
         return y
@@ -122,13 +163,21 @@ class LinearFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         x, w2, y = ctx.saved_tensors
-        prec = bwd_precision(ctx.precision)
+        prec = ctx.backward or bwd_precision(ctx.precision)
         dy = _c(dy)
         if ctx.relu:
             dy = relu_bwd(y, dy)
         n, k = w2.shape
         dy2, x2 = dy.reshape(-1, n), _c(x).reshape(-1, k)
         dx = dw = db = None
+        if prec == "bf16":
+            if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
+                dx, dw = linear_bwd_bf16(dy2, x2, w2, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+                dx = None if dx is None else dx.reshape(x.shape)
+                dw = None if dw is None else dw.reshape(ctx.wshape)
+            if ctx.has_bias and ctx.needs_input_grad[2]:
+                db = colsum(dy2)
+            return dx, dw, db, None, None, None
         if ctx.needs_input_grad[0]:
             wt = transpose_padded(w2, 32)                               # (k, n_padded): dX = dY W = dY (W^T)^T
             dyp = dy2
@@ -141,7 +190,7 @@ class LinearFn(torch.autograd.Function):
             dw = ops.linear(dyt, xt, None, precision=prec).reshape(ctx.wshape)
         if ctx.has_bias and ctx.needs_input_grad[2]:
             db = colsum(dy2)
-        return dx, dw, db, None, None
+        return dx, dw, db, None, None, None
 
 
 class GluFn(torch.autograd.Function):
@@ -274,14 +323,15 @@ class DwConvBnSiluFn(torch.autograd.Function):
 class AttentionCoreFn(torch.autograd.Function):
     """ctx = softmax(((q+u) k^T + rel_shift((q+v) p^T)) / 8, key mask) v  (attention.py:174-189 + :59-82) on projected
     q, k, v (B,T,H*64), p (2T-1,H*64).  Forward = the fused attention kernel of the module's precision; backward =
-    avsr_relpos_attention_bwd (fp32, scores recomputed)."""
+    avsr_relpos_attention_bwd (fp32, scores recomputed), or with ``backward="bf16"`` avsr_relpos_attention_bwd_tc."""
 
     @staticmethod
-    def forward(ctx_, q, k, v, p, u, vb, lengths, n_heads: int, precision: str):
+    def forward(ctx_, q, k, v, p, u, vb, lengths, n_heads: int, precision: str, backward: Optional[str] = None):
         require_cuda(q, "attention input")
         out = ops.relpos_attention(q, k, v, p, u, vb, lengths, n_heads, precision=precision)
         ctx_.save_for_backward(q, k, v, p, u, vb, out, lengths if lengths is not None else torch.empty(0, device=q.device))
         ctx_.n_heads, ctx_.masked = n_heads, lengths is not None
+        ctx_.backward = backward
         return out
 
     @staticmethod
@@ -289,26 +339,34 @@ class AttentionCoreFn(torch.autograd.Function):
         q, k, v, p, u, vb, out, lengths = ctx_.saved_tensors
         D = q.size(-1)
         dq_k, dq_p, dk, dv, dp = relpos_attention_bwd(q, k, v, p, u, vb, lengths if ctx_.masked else None, out, dctx,
-                                                      ctx_.n_heads)
+                                                      ctx_.n_heads, precision=ctx_.backward or "fp32")
         du = colsum(dq_k.reshape(-1, D)).reshape(u.shape)        # d pos_bias_u = sum over (b, t) of the k part of dq
         dvb = colsum(dq_p.reshape(-1, D)).reshape(vb.shape)
-        return dq_k + dq_p, dk, dv, dp, du, dvb, None, None, None
+        return dq_k + dq_p, dk, dv, dp, du, dvb, None, None, None, None
 
 
-def relpos_attention_bwd(q, k, v, p, u, vb, lengths, out, dctx, n_heads: int):
-    """avsr_relpos_attention_bwd -> (dq_k, dq_p, dk, dv, dp): the two parts of dq (through the content scores and through
-    the rel-pos scores), the key / value gradients (B, T, H*64) and the pos-table gradient (2T-1, H*64)."""
+def relpos_attention_bwd(q, k, v, p, u, vb, lengths, out, dctx, n_heads: int, precision: str = "fp32"):
+    """avsr_relpos_attention_bwd ("fp32") or avsr_relpos_attention_bwd_tc ("bf16") -> (dq_k, dq_p, dk, dv, dp): the two
+    parts of dq (through the content scores and through the rel-pos scores), the key / value gradients (B, T, H*64) and
+    the pos-table gradient (2T-1, H*64)."""
+    if precision not in ("fp32", "bf16"):
+        raise ValueError(f"relpos_attention_bwd: precision {precision!r}: 'fp32' or 'bf16'")
     q, k, v, p, u, vb, out, dctx = (_c(t) for t in (q, k, v, p, u, vb, out, dctx))
     B, T, D = q.shape
     dq_k, dq_p, dk, dv = (torch.empty_like(q) for _ in range(4))
     dp = torch.empty_like(p)
     ln = lengths.to(torch.int32).contiguous() if lengths is not None else None
-    ws = _workspace(q.device, int(lib.avsr_relpos_attention_bwd_workspace_bytes(B, T, n_heads)))
+    args = (q.data_ptr(), k.data_ptr(), v.data_ptr(), p.data_ptr(), u.data_ptr(), vb.data_ptr(), _ptr(ln),
+            out.data_ptr(), dctx.data_ptr(), dq_k.data_ptr(), dq_p.data_ptr(), dk.data_ptr(), dv.data_ptr(),
+            dp.data_ptr(), B, T, n_heads)
     with torch.cuda.device(q.device):
-        check(lib.avsr_relpos_attention_bwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), p.data_ptr(), u.data_ptr(),
-                                            vb.data_ptr(), _ptr(ln), out.data_ptr(), dctx.data_ptr(), dq_k.data_ptr(),
-                                            dq_p.data_ptr(), dk.data_ptr(), dv.data_ptr(), dp.data_ptr(), B, T, n_heads,
-                                            ws.data_ptr(), ws.numel(), _stream_handle(q.device)))
+        if precision == "fp32":
+            ws = _workspace(q.device, int(lib.avsr_relpos_attention_bwd_workspace_bytes(B, T, n_heads)))
+            check(lib.avsr_relpos_attention_bwd(*args, ws.data_ptr(), ws.numel(), _stream_handle(q.device)))
+        else:
+            prec = PRECISIONS["bf16"]
+            ws = _workspace(q.device, int(lib.avsr_relpos_attention_bwd_tc_workspace_bytes(B, T, n_heads, prec)))
+            check(lib.avsr_relpos_attention_bwd_tc(*args, prec, ws.data_ptr(), ws.numel(), _stream_handle(q.device)))
     return dq_k, dq_p, dk, dv, dp
 
 
@@ -365,14 +423,14 @@ class CtcLossFn(torch.autograd.Function):
 
 
 # ------------------------------------------------------------------------------------------------ module forwards (train)
-def feed_forward_train(m, x, precision: str):
+def feed_forward_train(m, x, precision: str, backward: Optional[str] = None):
     """PositionwiseFeedForward.forward in train mode: w_2(dropout(relu(w_1 x)))."""
-    h = LinearFn.apply(x, m.w_1.weight, m.w_1.bias, True, precision)
+    h = LinearFn.apply(x, m.w_1.weight, m.w_1.bias, True, precision, backward)
     h = m.dropout(h)
-    return LinearFn.apply(h, m.w_2.weight, m.w_2.bias, False, precision)
+    return LinearFn.apply(h, m.w_2.weight, m.w_2.bias, False, precision, backward)
 
 
-def conv_module_train(m, x, precision: str):
+def conv_module_train(m, x, precision: str, backward: Optional[str] = None):
     """ConvolutionModule.forward in train mode on (B, T, C): pointwise_cov1 -> GLU -> depthwise + BatchNorm(batch stats)
     + SiLU -> pointwise_cov2.  ``m.norm`` stays a real BatchNorm1d: its running statistics and num_batches_tracked are
     updated like torch's (momentum None = cumulative average is not supported here)."""
@@ -388,27 +446,27 @@ def conv_module_train(m, x, precision: str):
         raise NotImplementedError(f"conv_module.norm is {type(bn).__name__}: BatchNorm1d / SyncBatchNorm only")
     if bn.momentum is None:
         raise NotImplementedError("BatchNorm1d(momentum=None) (cumulative moving average) is not supported")
-    h = LinearFn.apply(x, m.pointwise_cov1.weight, m.pointwise_cov1.bias, False, precision)
+    h = LinearFn.apply(x, m.pointwise_cov1.weight, m.pointwise_cov1.bias, False, precision, backward)
     g = GluFn.apply(h)
     track = bn.track_running_stats and bn.running_mean is not None
     y = DwConvBnSiluFn.apply(g, m.depthwise_conv.weight, m.depthwise_conv.bias, bn.weight, bn.bias,
                              bn.running_mean if track else None, bn.running_var if track else None, bn.momentum, bn.eps, group)
     if track and bn.num_batches_tracked is not None:
         bn.num_batches_tracked.add_(1)
-    return LinearFn.apply(y, m.pointwise_cov2.weight, m.pointwise_cov2.bias, False, precision)
+    return LinearFn.apply(y, m.pointwise_cov2.weight, m.pointwise_cov2.bias, False, precision, backward)
 
 
-def attention_train(m, x, pos_emb, mask, precision: str):
+def attention_train(m, x, pos_emb, mask, precision: str, backward: Optional[str] = None):
     """RelPositionMultiHeadedAttention.forward (self-attention) in train mode -> (B, T, d)."""
     from .espnet_dropin.attention import mask_to_lengths
     if m.dropout.p > 0:
         raise NotImplementedError("dropout on the attention probabilities (attention_dropout_rate > 0) is not implemented "
                                   "in the fused kernel; auto_avsr trains with 0.0 (e2e_asr_conformer.py:33-39)")
     B, T, D = x.shape
-    q = LinearFn.apply(x, m.linear_q.weight, m.linear_q.bias, False, precision)
-    k = LinearFn.apply(x, m.linear_k.weight, m.linear_k.bias, False, precision)
-    v = LinearFn.apply(x, m.linear_v.weight, m.linear_v.bias, False, precision)
-    p = LinearFn.apply(pos_emb.reshape(2 * T - 1, D), m.linear_pos.weight, None, False, precision)
+    q = LinearFn.apply(x, m.linear_q.weight, m.linear_q.bias, False, precision, backward)
+    k = LinearFn.apply(x, m.linear_k.weight, m.linear_k.bias, False, precision, backward)
+    v = LinearFn.apply(x, m.linear_v.weight, m.linear_v.bias, False, precision, backward)
+    p = LinearFn.apply(pos_emb.reshape(2 * T - 1, D), m.linear_pos.weight, None, False, precision, backward)
     lengths = None if mask is None else mask_to_lengths(mask, B, T)
-    ctx = AttentionCoreFn.apply(q, k, v, p, m.pos_bias_u, m.pos_bias_v, lengths, m.h, precision)
-    return LinearFn.apply(ctx, m.linear_out.weight, m.linear_out.bias, False, precision)
+    ctx = AttentionCoreFn.apply(q, k, v, p, m.pos_bias_u, m.pos_bias_v, lengths, m.h, precision, backward)
+    return LinearFn.apply(ctx, m.linear_out.weight, m.linear_out.bias, False, precision, backward)

@@ -253,6 +253,18 @@ int avsr_layernorm_bwd(const float *x, const float *gamma, const float *dy, floa
 int avsr_colsum(const float *y, float *out, int rows, int cols, void *workspace, size_t workspace_bytes, void *stream);
 /* dst (cols, ld_dst >= rows) = src (rows, cols)^T; columns [rows, ld_dst) of dst are left untouched (pre-zeroed padding) */
 int avsr_transpose(const float *src, float *dst, int rows, int cols, long ld_dst, void *stream);
+/* fp32 (rows, cols) -> a bf16 GEMM operand (precision must be AVSR_PREC_BF16): transposed, dst (cols, ld_dst >= rows)
+ * with dst[c][r] = src[r][c]; else dst (rows, ld_dst >= cols).  The padding columns are written as zeros.  The bf16
+ * backward's dgrad / wgrad operands, transposed, padded and converted in one pass for avsr_linear_operands. */
+int avsr_pack_operand(const float *src, void *dst, int rows, int cols, long ld_dst, int transpose, int precision,
+                      void *stream);
+/* Both GEMMs of a Linear's backward with bf16 operands (fp32 accumulation) in one call: dx (rows, k) = dy w and
+ * dw (n, k) = dy^T x, for dy (rows, n), x (rows, k), w (n, k), all fp32.  dx or dw may be NULL (not wanted).  The
+ * operands are packed with avsr_pack_operand into the workspace (>= avsr_linear_bwd_bf16_workspace_bytes), then
+ * avsr_linear_operands runs on them. */
+size_t avsr_linear_bwd_bf16_workspace_bytes(int rows, int n, int k);
+int avsr_linear_bwd_bf16(const float *dy, const float *x, const float *w, float *dx, float *dw, int rows, int n, int k,
+                         void *workspace, size_t workspace_bytes, void *stream);
 /* dx = dy * (y > 0) */
 int avsr_relu_bwd(const float *y, const float *dy, float *dx, long n, void *stream);
 /* F.glu over channels (conformer_encoder.py:32): in (rows, 2C) -> y (rows, C); and its backward din (rows, 2C) */
@@ -289,6 +301,19 @@ int avsr_relpos_attention_bwd(const float *q, const float *k, const float *v, co
                               const float *pos_bias_v, const int32_t *lengths, const float *ctx, const float *dctx,
                               float *dq_k, float *dq_p, float *dk, float *dv, float *dp, int B, int T, int H,
                               void *workspace, size_t workspace_bytes, void *stream);
+
+/* The same backward on the tensor cores (wgmma), replacing the same reference lines
+ * (transformer/attention.py:174-189 + :59-82): the arguments and outputs of avsr_relpos_attention_bwd, plus
+ * `precision`, which must be AVSR_PREC_BF16 (bf16 operands, fp32 accumulation; any other value is an error naming it).
+ * q+u, q+v, k, v, dctx and p are converted to bf16 head-major copies in the workspace; Delta is computed in fp32 from
+ * ctx and dctx; the backward computes its own row log-sum-exp from the bf16 operands.  Scores are recomputed (nothing
+ * of size T^2 is stored), no atomics, every sum in a fixed order: repeated calls are bit-identical.
+ * avsr_relpos_attention_bwd_tc_workspace_bytes returns 0 for a precision other than AVSR_PREC_BF16. */
+size_t avsr_relpos_attention_bwd_tc_workspace_bytes(int B, int T, int H, int precision);
+int avsr_relpos_attention_bwd_tc(const float *q, const float *k, const float *v, const float *p, const float *pos_bias_u,
+                                 const float *pos_bias_v, const int32_t *lengths, const float *ctx, const float *dctx,
+                                 float *dq_k, float *dq_p, float *dk, float *dv, float *dp, int B, int T, int H,
+                                 int precision, void *workspace, size_t workspace_bytes, void *stream);
 
 /* CTC loss of the head (espnet/nets/pytorch_backend/ctc.py:32-65: CTC.forward -> loss_fn):
  * torch.nn.CTCLoss(reduction="none", zero_infinity=True), blank 0, on log_softmax of the logits, per utterance.
