@@ -305,6 +305,9 @@ struct EpiParams {
   void* qv;
   void* kk;
   void* vt;
+  // Bw is a prepared weight that no kernel of the current PDL chain writes: gemm_tc may load it before
+  // griddepcontrol.wait (gemm_tc.cu, "static-operand prologue").  Only the encoder forward sets it; not for EPI_VT.
+  int b_static;
 };
 
 // ---------------------------------------------------------------- phase trace (diagnostic build only)

@@ -220,6 +220,13 @@ static EpiParams epi_resid(int M, int N, const float* bias, float* x, float alph
   return e;
 }
 
+// the weight operand is a prepared buffer that nothing in the forward's PDL chain writes: the GEMM may load it before
+// its dependency wait (gemm_tc.cu, "static-operand prologue").  Only the encoder forward and its head use this.
+static EpiParams static_b(EpiParams e) {
+  e.b_static = 1;
+  return e;
+}
+
 static int run_gemm(int prec, int mode, const void* A, const void* Bw, int M, int N, int K, const EpiParams& e,
                     cudaStream_t st) {
   if (prec == AVSR_PREC_FP32)
@@ -243,7 +250,7 @@ static int compute_pos(const AvsrEncoderConfig& c, const Prepared& P, const Work
   AVSR_TRY(launch_sinusoid(W.pe, T, D, operand_kind(prec), ps));
   EpiParams e{};
   e.M = W.Rp; e.N = L * D; e.out = W.pos; e.H = H; e.Rp = W.Rp; e.round_out = prec != AVSR_PREC_FP32;
-  return run_gemm(prec, EPI_POS, W.pe, P.pos_w_all, W.Rp, L * D, D, e, ps);
+  return run_gemm(prec, EPI_POS, W.pe, P.pos_w_all, W.Rp, L * D, D, static_b(e), ps);
 }
 
 // pos_external: the caller computes the pos tables (compute_pos) and records aux->join; this body only waits for it
@@ -284,9 +291,9 @@ static int forward_body(const AvsrEncoderConfig& c, const Prepared& P, const Wor
     // (for l > 0 the norm_ff_macaron output was produced together with the previous layer's norm_final)
     if (l == 0) AVSR_TRY(launch_layernorm(W.x, w.ln_ffm_w, w.ln_ffm_b, W.xn, N, D, opk, st));
     AVSR_TRY(chk(W.xn, (size_t)N * D));
-    AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.xn, w.ffm_w1, N, F, D, epi_linear(N, F, w.ffm_b1, W.hid, nullptr, 0.f, 1, opr), st));
+    AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.xn, w.ffm_w1, N, F, D, static_b(epi_linear(N, F, w.ffm_b1, W.hid, nullptr, 0.f, 1, opr)), st));
     AVSR_TRY(chk(W.hid, (size_t)N * F));
-    AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.hid, w.ffm_w2, N, D, F, epi_resid(N, D, w.ffm_b2, W.x, 0.5f, W.splitk, W.counters), st));
+    AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.hid, w.ffm_w2, N, D, F, static_b(epi_resid(N, D, w.ffm_b2, W.x, 0.5f, W.splitk, W.counters)), st));
     AVSR_TRY(tap(0));
     // (2) rel-pos MHA: x += out(attn(LN(x)))                                  conformer_encoder.py:119-142
     AVSR_TRY(launch_layernorm(W.x, w.ln_mha_w, w.ln_mha_b, W.xn, N, D, opk, st));
@@ -298,10 +305,10 @@ static int forward_body(const AvsrEncoderConfig& c, const Prepared& P, const Wor
       if (prec16(prec)) {
         // one QKV projection; V keeps the (B,H,T,64) layout (the P.V MMA reads it as an MN-major operand)
         e.N = 3 * D;
-        AVSR_TRY(run_gemm(prec, EPI_QK, W.xn, w.qk_w, N, 3 * D, D, e, st));
+        AVSR_TRY(run_gemm(prec, EPI_QK, W.xn, w.qk_w, N, 3 * D, D, static_b(e), st));
       } else {
         e.N = 2 * D;
-        AVSR_TRY(run_gemm(prec, EPI_QK, W.xn, w.qk_w, N, 2 * D, D, e, st));
+        AVSR_TRY(run_gemm(prec, EPI_QK, W.xn, w.qk_w, N, 2 * D, D, static_b(e), st));
         EpiParams v{};
         v.M = D; v.N = N; v.bias = w.v_b; v.T = T; v.H = H; v.Tp = W.Tp; v.vt = W.vt; v.round_out = opr;
         AVSR_TRY(run_gemm(prec, EPI_VT, op_offset(w.qk_w, (size_t)2 * D * D, prec), W.xn, D, N, D, v, st));
@@ -321,7 +328,7 @@ static int forward_body(const AvsrEncoderConfig& c, const Prepared& P, const Wor
         AVSR_TRY(attention_simt(W.qu, W.qv, W.kk, W.vt, (const float*)pos_l, lengths, W.ctx, B, T, H, W.Tp, W.Rp, 0, st));
     }
     AVSR_TRY(chk(W.ctx, (size_t)N * D));
-    AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.ctx, w.out_w, N, D, D, epi_resid(N, D, w.out_b, W.x, 1.0f, W.splitk, W.counters), st));
+    AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.ctx, w.out_w, N, D, D, static_b(epi_resid(N, D, w.out_b, W.x, 1.0f, W.splitk, W.counters)), st));
     AVSR_TRY(tap(1));
     // (3) conv module: x += pw2(silu(bn(dw(glu(pw1 LN(x))))))                 conformer_encoder.py:145-151, :30-35
     AVSR_TRY(launch_layernorm(W.x, w.ln_conv_w, w.ln_conv_b, W.xn, N, D, opk, st));
@@ -329,18 +336,18 @@ static int forward_body(const AvsrEncoderConfig& c, const Prepared& P, const Wor
     {
       EpiParams e{};
       e.M = N; e.N = 2 * D; e.bias = w.pw1_b; e.out = W.glu; e.ldo = D;
-      AVSR_TRY(run_gemm(prec, EPI_GLU, W.xn, w.pw1_w, N, 2 * D, D, e, st));
+      AVSR_TRY(run_gemm(prec, EPI_GLU, W.xn, w.pw1_w, N, 2 * D, D, static_b(e), st));
     }
     AVSR_TRY(launch_dwconv_bn_silu(W.glu, w.dw_wt, w.dw_scale, w.dw_shift, W.dw, B, T, D, c.cnn_kernel, opk, st));
     AVSR_TRY(chk(W.dw, (size_t)N * D));
-    AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.dw, w.pw2_w, N, D, D, epi_resid(N, D, w.pw2_b, W.x, 1.0f, W.splitk, W.counters), st));
+    AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.dw, w.pw2_w, N, D, D, static_b(epi_resid(N, D, w.pw2_b, W.x, 1.0f, W.splitk, W.counters)), st));
     AVSR_TRY(tap(2));
     // (4) FFN: x += 0.5 * w2(relu(w1 LN(x)))                                  conformer_encoder.py:154-159
     AVSR_TRY(launch_layernorm(W.x, w.ln_ff_w, w.ln_ff_b, W.xn, N, D, opk, st));
     AVSR_TRY(chk(W.xn, (size_t)N * D));
-    AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.xn, w.ff_w1, N, F, D, epi_linear(N, F, w.ff_b1, W.hid, nullptr, 0.f, 1, opr), st));
+    AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.xn, w.ff_w1, N, F, D, static_b(epi_linear(N, F, w.ff_b1, W.hid, nullptr, 0.f, 1, opr)), st));
     AVSR_TRY(chk(W.hid, (size_t)N * F));
-    AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.hid, w.ff_w2, N, D, F, epi_resid(N, D, w.ff_b2, W.x, 0.5f, W.splitk, W.counters), st));
+    AVSR_TRY(run_gemm(prec, EPI_LINEAR, W.hid, w.ff_w2, N, D, F, static_b(epi_resid(N, D, w.ff_b2, W.x, 0.5f, W.splitk, W.counters)), st));
     AVSR_TRY(tap(3));
     // (5) x = LN_final(x)                                                     conformer_encoder.py:161-162
     //     fused with the next layer's norm_ff_macaron: one pass writes x (fp32) and xn (operand)
@@ -430,10 +437,13 @@ static HeadWorkspace layout_head_workspace(const AvsrEncoderConfig& c, int B, in
 }
 
 // hs_op (rows, d_model) in operand storage -> logp (rows, odim) fp32 log-probabilities [+ arg max]
+// `b_static`: the head forward's ctc_lo (EpiParams::b_static)
 static int ctc_logprobs(const AvsrEncoderConfig& c, const HeadPrep& H, const void* hs_op, int rows, int odim, float* logits,
-                        float* logp, int32_t* argmax, int prec, cudaStream_t st) {
+                        float* logp, int32_t* argmax, int prec, cudaStream_t st, bool b_static = false) {
   const int D = c.d_model;
-  AVSR_TRY(run_gemm(prec, EPI_LINEAR, hs_op, H.ctc_w, rows, H.npad, D, epi_linear(rows, H.npad, H.ctc_b, logits, nullptr, 0.f, 0, 0), st));
+  EpiParams e = epi_linear(rows, H.npad, H.ctc_b, logits, nullptr, 0.f, 0, 0);
+  e.b_static = b_static;
+  AVSR_TRY(run_gemm(prec, EPI_LINEAR, hs_op, H.ctc_w, rows, H.npad, D, e, st));
   return launch_log_softmax_rows(logits, H.npad, logp, odim, argmax, rows, odim, st);
 }
 
@@ -447,14 +457,15 @@ static int head_forward_body(const AvsrEncoderConfig& c, const Prepared& P, cons
   // (1) proj_encoder with the embed scale folded in, straight into the residual stream: x = sqrt(d) * (f Wp^T + bp)
   const void* fx = feats;
   if (precision != AVSR_PREC_FP32) { AVSR_TRY(copy_round(feats, HW.fx, (long)N * idim, operand_kind(precision), st)); fx = HW.fx; }
-  AVSR_TRY(run_gemm(precision, EPI_LINEAR, fx, H.proj_ws, N, D, idim, epi_linear(N, D, H.proj_bs, W.x, nullptr, 0.f, 0, 0), st));
+  // (copy_round is launched without PDL, so the prepared head weights are complete before this GEMM starts)
+  AVSR_TRY(run_gemm(precision, EPI_LINEAR, fx, H.proj_ws, N, D, idim, static_b(epi_linear(N, D, H.proj_bs, W.x, nullptr, 0.f, 0, 0)), st));
   // (2) the 12 layers
   AVSR_TRY(forward_body(c, P, W, B, T, lengths, nullptr, precision, st, aux));
   // (3) after_norm: fp32 features for the caller (attention decoder / beam search) + the operand of ctc_lo in one pass
   float* feat_out = enc_out ? enc_out : W.x;
   AVSR_TRY(launch_layernorm_dual(W.x, P.after_w, P.after_b, feat_out, W.xn, N, D, operand_kind(precision), st));
   // (4) ctc_lo + log_softmax: GEMM into fp32 logits, then the row-wise log-softmax / arg-max kernel
-  return ctc_logprobs(c, H, W.xn, N, odim, HW.logits, logp, argmax, precision, st);
+  return ctc_logprobs(c, H, W.xn, N, odim, HW.logits, logp, argmax, precision, st, true);
 }
 
 }  // namespace avsr

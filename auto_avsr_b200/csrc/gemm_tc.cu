@@ -178,7 +178,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   };
 
   pdl_launch_dependents();
-  AVSR_TSPAN_OPEN(400 + MODE, (unsigned)BN);
+  // trace record: kernel 400 + MODE, aux = N | K << 16 (the GEMM's shape names its kind in the encoder's schedule)
+  AVSR_TSPAN_OPEN(400 + MODE, (unsigned)ep.N | ((unsigned)K << 16));
+#ifdef AVSR_TRACE
+  __shared__ unsigned long long* s_trec;   // the record, for marks by threads other than thread 0
+  if (threadIdx.x == 0) s_trec = _tsp;
+#define TC_STAMP(slot) ::avsr::trace_stamp(s_trec, slot)
+#else
+#define TC_STAMP(slot) do { } while (0)
+#endif
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
@@ -189,12 +197,37 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
   __syncthreads();
   if constexpr (CS > 1) cluster_sync();   // peers' barriers are initialised before any multicast or remote arrive
-  pdl_wait();   // everything above overlapped the previous kernel's tail; from here on we touch its outputs
-  AVSR_TSPAN_DEP();
-
+  // Static-operand prologue (ep.b_static): Bw is a prepared weight that no kernel of this PDL chain writes, so it may be
+  // read before griddepcontrol.wait.  Why that holds: with PDL, kernel k + 2 can run this section before kernel k has
+  // finished, so only buffers that nothing in the chain writes may be read here.  The encoder forward is the only
+  // caller that sets the flag; its weights are written by avsr_prepare_weights / the training refresh, which end
+  // before the chain starts (the forward's first operation is a memset, the plan's body a graph launch, and the head's
+  // proj GEMM follows a kernel launched without PDL, each a full dependency on the stream's earlier work).
+  //   warp 0: arms `full` of the first min(S, k-blocks of its pieces) stages with the whole stage's bytes and issues
+  //           their Bw boxes; their A boxes follow the wait (the barrier protocol is unchanged);
+  //   warp 1: prefetches this CTA's share of the whole weight into L2, k-block-major (the order the CTAs consume it),
+  //           so the k-blocks past the ring's first fill do not wait on HBM either.
+  const bool pre = CS == 1 && MODE != EPI_VT && ep.b_static != 0;
+  // Everything before each warp's pdl_wait() overlaps the previous kernel's tail; after it the warp touches that
+  // kernel's outputs.  Warps 1-3 never touch them.
   if (warp < 4) {
     setmaxnreg_dec<40>();
     if (warp == 0) {
+      int pre_its = 0;                              // ring iterations whose Bw box the prologue issued
+      if (pre) {
+        for (int j = 0; j < npieces && pre_its < S; ++j) {
+          const TcPiece w = piece_at(j);
+          for (int kb = w.kb0; kb < w.kb1 && pre_its < S; ++kb, ++pre_its) {
+            if (elect_one_sync()) {
+              mbar_expect_tx(full_bar(pre_its), Cfg::kStageBytes);
+              tma_load_2d(base + pre_its * Cfg::kStageBytes + Cfg::kABytes, &tmB, kb * KE, w.tn * BN, full_bar(pre_its));
+            }
+          }
+        }
+        if (lane == 0) TC_STAMP(0);                 // the prologue's loads are issued
+      }
+      pdl_wait();
+      AVSR_TSPAN_DEP();
       // TMA producer: warp-uniform loop, only the instruction issue is guarded by elect.sync
       const int cm = crank % CM, cn = crank / CM;
       uint16_t a_mask = 0, b_mask = 0;              // peers sharing this CTA's A rows / Bw rows
@@ -207,21 +240,29 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         for (int kb = w.kb0; kb < w.kb1; ++kb, ++it) {
           const int s = it % S;
           const uint32_t ph = (it / S) & 1;
-          mbar_wait(empty_bar(s), ph ^ 1);
+          const bool b_done = it < pre_its;           // armed and Bw issued by the prologue (a fresh stage)
+          if (!b_done) mbar_wait(empty_bar(s), ph ^ 1);
           if (elect_one_sync()) {
-            mbar_expect_tx(full_bar(s), Cfg::kStageBytes);   // own slices + the peers' multicast slices
+            if (!b_done) mbar_expect_tx(full_bar(s), Cfg::kStageBytes);   // own slices + the peers' multicast slices
             const uint32_t a_dst = base + s * Cfg::kStageBytes;
             if constexpr (CN == 1) tma_load_2d(a_dst, &tmA, kb * KE, m0, full_bar(s));
             else tma_load_2d_mc(a_dst + cn * (TC_BM / CN) * 128, &tmA, kb * KE, m0 + cn * (TC_BM / CN), full_bar(s), a_mask);
-            if constexpr (CM == 1) tma_load_2d(a_dst + Cfg::kABytes, &tmB, kb * KE, n0, full_bar(s));
-            else tma_load_2d_mc(a_dst + Cfg::kABytes + cm * (BN / CM) * 128, &tmB, kb * KE, n0 + cm * (BN / CM),
-                                full_bar(s), b_mask);
+            if (!b_done) {
+              if constexpr (CM == 1) tma_load_2d(a_dst + Cfg::kABytes, &tmB, kb * KE, n0, full_bar(s));
+              else tma_load_2d_mc(a_dst + Cfg::kABytes + cm * (BN / CM) * 128, &tmB, kb * KE, n0 + cm * (BN / CM),
+                                  full_bar(s), b_mask);
+            }
           }
         }
       }
+      if (lane == 0) TC_STAMP(2);                   // every load of the CTA is issued
+    } else if (warp == 1 && pre && lane == 0) {
+      for (int i = blockIdx.x; i < tiles_n * nkb; i += gridDim.x)
+        tma_prefetch_l2_2d(&tmB, (i / tiles_n) * KE, (i % tiles_n) * BN);
     }
   } else {
     setmaxnreg_inc<232>();
+    pdl_wait();
     const int wg = (warp - 4) >> 2;              // consumer warpgroup: the CTA's items with index parity wg
     const int q = warp & 3;                      // 32-row slab of the tile this warp drains (all BN columns)
     constexpr int RB = LD * 4;                               // accumulator row stride in bytes
@@ -267,6 +308,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     for (int kb = kb0; kb < kb1; ++kb, ++it) {
       const int s = it % S;
       mbar_wait(full_bar(s), (it / S) & 1);
+      if (idx == 0 && kb == kb0 && q == 0 && lane == 0) TC_STAMP(1);   // the CTA's first stage landed
       const uint32_t a_addr = base + s * Cfg::kStageBytes;
       const uint64_t a_desc0 = wgmma_desc_sw128(a_addr);
       const uint64_t a_desc1 = wgmma_desc_sw128(a_addr + 64 * 128);
@@ -285,6 +327,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     pass_turn(0);                                  // every k-block is issued: the other main loop may start
     wgmma_wait<0>();
     wgmma_fence_regs<BN>(acc);
+    if (idx == npieces - 1 && q == 0 && lane == 0) TC_STAMP(3);       // the CTA's last main loop retired
     release((it - 1) % S);
     mbar_wait(order_bar(1, wg), par);              // the other warpgroup's epilogue is done with s_acc / s_vec
     if (!w.valid) { pass_turn(1); continue; }      // past the matrix edge: took part in the loads, stores nothing
@@ -563,6 +606,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   __syncthreads();
   if constexpr (CS > 1) cluster_sync();   // no CTA leaves while a peer may still arrive on or load into its memory
   AVSR_TSPAN_CLOSE();
+#undef TC_STAMP
 }
 
 AVSR_TRACE_DEFINE_BIND(trace_bind_gemm_tc)
@@ -768,9 +812,12 @@ int gemm_tc(int mode, int opk, const void* A, const void* Bw, int M, int N, int 
   const int ke = op16(opk) ? 64 : 32;
   AVSR_REQUIRE(K >= ke && K % ke == 0, "gemm_tc: K=%d must be a multiple of %d", K, ke);
   if (M <= 0 || N <= 0) return AVSR_OK;
-  if (opk == OP_F16) return dispatch_mode<__half>(mode, A, Bw, M, N, K, ep, st);
-  if (opk == OP_BF16) return dispatch_mode<__nv_bfloat16>(mode, A, Bw, M, N, K, ep, st);
-  return dispatch_mode<float>(mode, A, Bw, M, N, K, ep, st);
+  // AVSR_B200_PROLOGUE=0 turns the static-operand prologue off (read per call, so one process can A/B both paths)
+  EpiParams e = ep;
+  if (const char* pro = getenv("AVSR_B200_PROLOGUE")) { if (pro[0] == '0') e.b_static = 0; }
+  if (opk == OP_F16) return dispatch_mode<__half>(mode, A, Bw, M, N, K, e, st);
+  if (opk == OP_BF16) return dispatch_mode<__nv_bfloat16>(mode, A, Bw, M, N, K, e, st);
+  return dispatch_mode<float>(mode, A, Bw, M, N, K, e, st);
 }
 
 }  // namespace avsr

@@ -76,6 +76,14 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, 
       : "memory");
 }
 
+// 2-D tiled prefetch of one box into L2 (no shared memory, no completion): a later load of the box hits in L2
+__device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* m, int c0, int c1) {
+  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];"
+               :
+               : "l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1)
+               : "memory");
+}
+
 // 2-D tiled load multicast to the CTAs of the cluster in `cta_mask`: the box lands at the same shared offset `dst` in
 // each of them, and its bytes are credited to the mbarrier at offset `bar` in each of them.
 __device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* m, int c0, int c1, uint32_t bar,
