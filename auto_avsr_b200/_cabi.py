@@ -13,7 +13,7 @@ LIB_PATH = os.environ.get("AVSR_B200_LIB") or os.path.join(_HERE, "csrc", "libav
 
 OK, E_INVALID, E_CUDA, E_WORKSPACE = 0, 1, 2, 3
 PREC_FP32, PREC_TF32, PREC_F16, PREC_BF16 = 0, 1, 2, 16
-ABI_VERSION = 10
+ABI_VERSION = 11
 
 
 class AvsrError(RuntimeError):
@@ -134,10 +134,13 @@ SIGNATURES = {
     "avsr_glu_fwd": (_I, [_P, _P, C.c_long, _I, _P]),
     "avsr_glu_bwd": (_I, [_P, _P, _P, C.c_long, _I, _P]),
     "avsr_dwconv_raw": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _Z, _P]),
-    "avsr_chan_sums": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _P, _Z, _P]),
-    "avsr_bn_silu_fwd": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _P]),
-    "avsr_bn_silu_bwd_dx": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _F, _P, _I, _I, _P]),
     "avsr_dwconv_wgrad": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _Z, _P]),
+    "avsr_bn_train_workspace_bytes": (_Z, [C.c_long, _I]),
+    "avsr_bn_train_stats": (_I, [_P, C.c_long, _I, _P, _P, _Z, _P]),
+    "avsr_bn_train_finalize": (_I, [_P, _I, _I, C.c_double, C.c_double, _P, _P, _P, _P, _P]),
+    "avsr_bn_train_act_fwd": (_I, [_P, _P, _P, _P, _P, _P, _I, _P, C.c_long, _I, _P]),
+    "avsr_bn_train_bwd_sums": (_I, [_P] * 7 + [_I, _P, C.c_long, _I, _P, _Z, _P]),
+    "avsr_bn_train_bwd_dx": (_I, [_P] * 7 + [_I, _P, _F, _P, _P, C.c_long, _I, _P]),
     "avsr_relpos_attention_bwd_workspace_bytes": (_Z, [_I, _I, _I]),
     "avsr_relpos_attention_bwd": (_I, [_P] * 14 + [_I, _I, _I, _P, _Z, _P]),
     "avsr_relpos_attention_bwd_tc_workspace_bytes": (_Z, [_I, _I, _I, _I]),
@@ -191,11 +194,6 @@ SIGNATURES = {
     "avsr_conv_bn_act": (_I, [_P, _P, _P, _P, _P, _I, _P] + [_I] * 8 + [_P, _Z, _I, _P]),
     "avsr_frontend_train_conv_workspace_bytes": (_Z, [_I] * 11),
     "avsr_frontend_train_conv_fwd": (_I, [_P, _P, _P, _P] + [_I] * 10 + [_P, _Z, _I, _P]),
-    "avsr_frontend_train_bn_finalize": (_I, [_P, _I, _I, C.c_double, C.c_double, _P, _P, _P, _P, _P]),
-    "avsr_frontend_train_bn_act_fwd": (_I, [_P, _P, _P, _P, _P, _P, _I, _P, C.c_long, _I, _P]),
-    "avsr_frontend_train_bn_bwd_workspace_bytes": (_Z, [C.c_long, _I]),
-    "avsr_frontend_train_bn_bwd_sums": (_I, [_P] * 7 + [_I, _P, C.c_long, _I, _P, _Z, _P]),
-    "avsr_frontend_train_bn_bwd_dx": (_I, [_P] * 7 + [_I, _P, _F, _P, _P, C.c_long, _I, _P]),
     "avsr_frontend_train_dgrad_workspace_bytes": (_Z, [_I] * 9),
     "avsr_frontend_train_conv_dgrad": (_I, [_P, _P, _P] + [_I] * 8 + [_P, _Z, _I, _P]),
     "avsr_frontend_train_wgrad_workspace_bytes": (_Z, [_I] * 10),

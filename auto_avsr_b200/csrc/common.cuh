@@ -441,6 +441,10 @@ int launch_sinusoid(void* pe, int T, int d, int out_kind, cudaStream_t st);
 int launch_dwconv_bn_silu(const float* x, const float* wt /*(K,C)*/, const float* scale, const float* shift, void* y,
                           int B, int T, int C, int K, int out_kind, cudaStream_t st);
 
+// train.cu: each channel's (count, mean, M2) over z (rows >= 1, C) -> stats (3, C) fp64, through the fp64 partials
+// `part` (256-byte aligned, avsr_bn_train_workspace_bytes(rows, C) - 256 bytes)
+int launch_bn_stats(const float* z, long rows, int C, double* part, double* stats, cudaStream_t st);
+
 // head.cu
 int launch_log_softmax_rows(const float* x, long ldx, float* y, long ldy, int32_t* best, int rows, int n, cudaStream_t st);
 

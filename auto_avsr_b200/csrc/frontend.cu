@@ -778,8 +778,8 @@ extern "C" int avsr_conv_bn_act(const float* x, const float* w, const float* sca
 // The front-end's training path is a chain of library calls that auto_avsr_b200/frontend_train.py drives per conv unit
 // (conv -> BatchNorm -> [+ residual] -> [SiLU]).  Activations cross the boundary as fp32 channels-last tensors.
 //  - forward conv: the inference implicit GEMM (conv_tc_kernel, RAW epilogue: the fp32 accumulator) or, in fp32, the
-//    direct kernel with scale 1 and shift 0; then per-tile (count, mean, M2) of every channel and a fixed-order merge
-//    with Chan's formula in fp64 (no one-pass variance);
+//    direct kernel with scale 1 and shift 0; then the batch statistics of every channel (launch_bn_stats, train.cu,
+//    which also holds the BatchNorm's normalise and backward: the avsr_bn_train_* entries);
 //  - dgrad: stride 1 is the same implicit GEMM over dZ with the 180-degree-rotated weight; stride 2 splits the input
 //    gradient into its parity classes, each a stride-1 implicit GEMM with a 1- or 2-tap sub-filter per axis (no MAC on
 //    inserted zeros), scattered to the class's pixels;
@@ -787,163 +787,10 @@ extern "C" int avsr_conv_bn_act(const float* x, const float* w, const float* sca
 //  - max-pool with a recorded winner (first maximum in scan order, NaN wins: torch's rule) and a gather backward.
 namespace avsr {
 
-constexpr int FT_ROWS = 256;      // rows per statistics tile
-
 __global__ void fill_f32_kernel(float* p, int n, float v) {
   pdl_wait();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) p[i] = v;
-}
-
-// per-tile (count, mean, M2) of each channel of z (rows, C): part[tile][3][C], two passes over the tile in fp32
-__global__ void __launch_bounds__(128) ft_stats_partial_kernel(const float* __restrict__ z, double* __restrict__ part,
-                                                                long rows, int C) {
-  pdl_wait();
-  const int c = blockIdx.y * 128 + threadIdx.x;
-  if (c >= C) return;
-  const long r0 = (long)blockIdx.x * FT_ROWS, r1 = min(rows, r0 + FT_ROWS);
-  const int n = (int)(r1 - r0);
-  float s = 0.f;
-  for (long r = r0; r < r1; ++r) s += z[r * C + c];
-  const float mean = s / (float)n;
-  float q = 0.f;
-  for (long r = r0; r < r1; ++r) { const float d = z[r * C + c] - mean; q = fmaf(d, d, q); }
-  double* p = part + (long)blockIdx.x * 3 * C;
-  p[c] = n; p[C + c] = mean; p[2 * C + c] = q;
-}
-
-__device__ __forceinline__ void chan_merge(double& n, double& m, double& q, double nb, double mb, double qb) {
-  if (nb == 0.0) return;
-  const double nn = n + nb, d = mb - m;
-  m += d * (nb / nn);
-  q += qb + d * d * (n * nb / nn);
-  n = nn;
-}
-
-// one CTA per channel: thread t merges tiles t, t + 256, ... in order, then a fixed tree; out[3][C]
-__global__ void __launch_bounds__(256) ft_stats_merge_kernel(const double* __restrict__ part, int tiles, int C,
-                                                             double* __restrict__ out) {
-  pdl_wait();
-  __shared__ double sn[256], sm[256], sq[256];
-  const int c = blockIdx.x, t = threadIdx.x;
-  double n = 0, m = 0, q = 0;
-  for (int i = t; i < tiles; i += 256) {
-    const double* p = part + (long)i * 3 * C;
-    chan_merge(n, m, q, p[c], p[C + c], p[2 * C + c]);
-  }
-  sn[t] = n; sm[t] = m; sq[t] = q;
-  __syncthreads();
-  for (int h = 128; h > 0; h >>= 1) {
-    if (t < h) {
-      double a = sn[t], b = sm[t], e = sq[t];
-      chan_merge(a, b, e, sn[t + h], sm[t + h], sq[t + h]);
-      sn[t] = a; sm[t] = b; sq[t] = e;
-    }
-    __syncthreads();
-  }
-  if (t == 0) { out[c] = sn[0]; out[C + c] = sm[0]; out[2 * C + c] = sq[0]; }
-}
-
-// merge R ranks' (count, mean, M2) in rank order; mean, 1/sqrt(var + eps) with the biased variance; running statistics
-// (when given) move by `factor` toward the mean and the unbiased variance
-__global__ void ft_bn_finalize_kernel(const double* __restrict__ st, int R, int C, double eps, double factor,
-                                      float* __restrict__ running_mean, float* __restrict__ running_var,
-                                      float* __restrict__ mean, float* __restrict__ invstd) {
-  pdl_wait();
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  double n = 0, m = 0, q = 0;
-  for (int r = 0; r < R; ++r) chan_merge(n, m, q, st[(long)r * 3 * C + c], st[(long)r * 3 * C + C + c],
-                                         st[(long)r * 3 * C + 2 * C + c]);
-  const double var = n > 0 ? q / n : 0.0;
-  mean[c] = (float)m;
-  invstd[c] = (float)(1.0 / sqrt(var + eps));
-  if (running_mean) {
-    const double unb = n > 1 ? q / (n - 1) : var;
-    running_mean[c] = (float)((1.0 - factor) * running_mean[c] + factor * m);
-    running_var[c] = (float)((1.0 - factor) * running_var[c] + factor * unb);
-  }
-}
-
-__device__ __forceinline__ float ft_act_pre(float z, float m, float is, float g, float b) { return (z - m) * is * g + b; }
-__device__ __forceinline__ float silu_grad_acc(float h, float dy) {
-  const float s = sigmoidf_acc(h);
-  return dy * s * (1.0f + h * (1.0f - s));
-}
-
-// y = [SiLU]((z - mean) * invstd * gamma + beta [+ resid])
-__global__ void ft_bn_act_fwd_kernel(const float* __restrict__ z, const float* __restrict__ mean,
-                                     const float* __restrict__ invstd, const float* __restrict__ gamma,
-                                     const float* __restrict__ beta, const float* __restrict__ resid, int act,
-                                     float* __restrict__ y, long n, int C) {
-  pdl_wait();
-  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
-    const int c = (int)(i % C);
-    float h = ft_act_pre(z[i], mean[c], invstd[c], gamma[c], beta[c]);
-    if (resid) h += resid[i];
-    y[i] = act ? h * sigmoidf_acc(h) : h;
-  }
-}
-
-// ds = dL/d(BN output): dy, through SiLU when act; per-tile [sum ds, sum ds * x_hat]: part[tile][2][C] (fp64)
-__global__ void __launch_bounds__(128) ft_bn_bwd_partial_kernel(const float* __restrict__ z, const float* __restrict__ dy,
-                                                                 const float* __restrict__ mean,
-                                                                 const float* __restrict__ invstd,
-                                                                 const float* __restrict__ gamma,
-                                                                 const float* __restrict__ beta,
-                                                                 const float* __restrict__ resid, int act,
-                                                                 double* __restrict__ part, long rows, int C) {
-  pdl_wait();
-  const int c = blockIdx.y * 128 + threadIdx.x;
-  if (c >= C) return;
-  const long r0 = (long)blockIdx.x * FT_ROWS, r1 = min(rows, r0 + FT_ROWS);
-  const float m = mean[c], is = invstd[c], g = gamma[c], b = beta[c];
-  float s = 0.f, q = 0.f;
-  for (long r = r0; r < r1; ++r) {
-    const long i = r * C + c;
-    const float xh = (z[i] - m) * is;
-    float ds = dy[i];
-    if (act) ds = silu_grad_acc(xh * g + b + (resid ? resid[i] : 0.f), ds);
-    s += ds;
-    q = fmaf(ds, xh, q);
-  }
-  part[(long)blockIdx.x * 2 * C + c] = s;
-  part[(long)blockIdx.x * 2 * C + C + c] = q;
-}
-
-// out[j] = sum_t part[t][j] in fp64, one CTA per column j: strided per-thread sums, then a fixed tree
-__global__ void __launch_bounds__(256) ft_sum_merge_kernel(const double* __restrict__ part, int tiles, int width,
-                                                           float* __restrict__ out) {
-  pdl_wait();
-  __shared__ double sh[256];
-  const int j = blockIdx.x, t = threadIdx.x;
-  double s = 0;
-  for (int i = t; i < tiles; i += 256) s += part[(long)i * width + j];
-  sh[t] = s;
-  __syncthreads();
-  for (int h = 128; h > 0; h >>= 1) {
-    if (t < h) sh[t] += sh[t + h];
-    __syncthreads();
-  }
-  if (t == 0) out[j] = (float)sh[0];
-}
-
-// dz = gamma * invstd * (ds - (sum ds + x_hat * sum ds x_hat) / count); dres (when given) = ds
-__global__ void ft_bn_bwd_dx_kernel(const float* __restrict__ z, const float* __restrict__ dy,
-                                    const float* __restrict__ mean, const float* __restrict__ invstd,
-                                    const float* __restrict__ gamma, const float* __restrict__ beta,
-                                    const float* __restrict__ resid, int act, const float* __restrict__ sums,
-                                    float inv_count, float* __restrict__ dz, float* __restrict__ dres, long n, int C) {
-  pdl_wait();
-  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
-    const int c = (int)(i % C);
-    const float g = gamma[c], is = invstd[c];
-    const float xh = (z[i] - mean[c]) * is;
-    float ds = dy[i];
-    if (act) ds = silu_grad_acc(xh * g + beta[c] + (resid ? resid[i] : 0.f), ds);
-    if (dres) dres[i] = ds;
-    dz[i] = g * is * (ds - inv_count * (sums[c] + xh * sums[C + c]));
-  }
 }
 
 // ---------------------------------------------------------------- dgrad sub-filters
@@ -1256,8 +1103,6 @@ static bool ft_geom(int stem, int N, int T, int H, int W, int Cin, int Cout, int
   return true;
 }
 
-static size_t ft_tiles(long rows) { return (size_t)((rows + FT_ROWS - 1) / FT_ROWS); }
-
 struct FtConvWs { size_t xop, wop, unit, part, total; };
 static FtConvWs ft_conv_ws(const ConvGeom& g, int stem, int kind) {
   const size_t esz = operand_bytes(kind);
@@ -1265,7 +1110,7 @@ static FtConvWs ft_conv_ws(const ConvGeom& g, int stem, int kind) {
   w.xop = stem ? 0 : align_up((size_t)g.N * g.H * g.W * g.Cin * esz, 256);
   w.wop = align_up((size_t)g.Cout * g.Kp * esz, 256);
   w.unit = align_up(2 * (size_t)g.Cout * 4, 256);
-  w.part = align_up(ft_tiles(conv_rows(g)) * 3 * g.Cout * 8, 256);
+  w.part = avsr_bn_train_workspace_bytes(conv_rows(g), g.Cout);
   w.total = w.xop + w.wop + w.unit + w.part + 256;
   return w;
 }
@@ -1355,67 +1200,7 @@ extern "C" int avsr_frontend_train_conv_fwd(const float* x, const float* w, floa
     xin = xo;
   }
   AVSR_TRY(run_conv_raw(kind, stem != 0, xin, wo, ones, ones + g.Cout, z, g, st));
-  const int tiles = (int)ft_tiles(M);
-  AVSR_LAUNCH(ft_stats_partial_kernel, dim3(tiles, cdiv(g.Cout, 128)), 128, 0, st, (const float*)z, part, M, g.Cout);
-  AVSR_LAUNCH(ft_stats_merge_kernel, g.Cout, 256, 0, st, (const double*)part, tiles, g.Cout, stats);
-  return AVSR_OK;
-}
-
-extern "C" int avsr_frontend_train_bn_finalize(const double* stats, int ranks, int C, double eps, double factor,
-                                               float* running_mean, float* running_var, float* mean, float* invstd,
-                                               void* stream) {
-  AVSR_REQUIRE(ranks >= 1 && C >= 1 && eps >= 0.0 && factor >= 0.0 && factor <= 1.0,
-               "frontend train bn: bad ranks=%d C=%d eps or factor", ranks, C);
-  AVSR_REQUIRE(stats && mean && invstd && (running_mean != nullptr) == (running_var != nullptr), "NULL argument");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  AVSR_LAUNCH(ft_bn_finalize_kernel, cdiv(C, 128), 128, 0, st, stats, ranks, C, eps, factor, running_mean, running_var,
-              mean, invstd);
-  return AVSR_OK;
-}
-
-extern "C" int avsr_frontend_train_bn_act_fwd(const float* z, const float* mean, const float* invstd,
-                                              const float* gamma, const float* beta, const float* resid, int act,
-                                              float* y, long rows, int C, void* stream) {
-  AVSR_REQUIRE(rows >= 0 && C >= 1, "frontend train bn: bad rows=%ld C=%d", rows, C);
-  AVSR_REQUIRE(z && mean && invstd && gamma && beta && y, "NULL argument");
-  if (rows == 0) return AVSR_OK;
-  AVSR_LAUNCH(ft_bn_act_fwd_kernel, grid_1d(rows * C), 256, 0, reinterpret_cast<cudaStream_t>(stream), z, mean,
-              invstd, gamma, beta, resid, act, y, rows * C, C);
-  return AVSR_OK;
-}
-
-extern "C" size_t avsr_frontend_train_bn_bwd_workspace_bytes(long rows, int C) {
-  if (rows < 0 || C < 1) return 0;
-  return align_up(ft_tiles(rows) * 2 * C * 8, 256) + 256;
-}
-
-extern "C" int avsr_frontend_train_bn_bwd_sums(const float* z, const float* dy, const float* mean, const float* invstd,
-                                               const float* gamma, const float* beta, const float* resid, int act,
-                                               float* sums, long rows, int C, void* workspace, size_t workspace_bytes,
-                                               void* stream) {
-  AVSR_REQUIRE(rows >= 1 && C >= 1, "frontend train bn: bad rows=%ld C=%d", rows, C);
-  AVSR_REQUIRE(z && dy && mean && invstd && gamma && beta && sums && workspace, "NULL argument");
-  AVSR_REQUIRE_BYTES(avsr_frontend_train_bn_bwd_workspace_bytes(rows, C), workspace_bytes,
-                     "frontend train bn backward workspace");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  double* part = reinterpret_cast<double*>(align_up(reinterpret_cast<uintptr_t>(workspace), 256));
-  const int tiles = (int)ft_tiles(rows);
-  AVSR_LAUNCH(ft_bn_bwd_partial_kernel, dim3(tiles, cdiv(C, 128)), 128, 0, st, z, dy, mean, invstd, gamma, beta, resid,
-              act, part, rows, C);
-  AVSR_LAUNCH(ft_sum_merge_kernel, 2 * C, 256, 0, st, (const double*)part, tiles, 2 * C, sums);
-  return AVSR_OK;
-}
-
-extern "C" int avsr_frontend_train_bn_bwd_dx(const float* z, const float* dy, const float* mean, const float* invstd,
-                                             const float* gamma, const float* beta, const float* resid, int act,
-                                             const float* sums, float inv_count, float* dz, float* dres, long rows,
-                                             int C, void* stream) {
-  AVSR_REQUIRE(rows >= 0 && C >= 1, "frontend train bn: bad rows=%ld C=%d", rows, C);
-  AVSR_REQUIRE(z && dy && mean && invstd && gamma && beta && sums && dz, "NULL argument");
-  if (rows == 0) return AVSR_OK;
-  AVSR_LAUNCH(ft_bn_bwd_dx_kernel, grid_1d(rows * C), 256, 0, reinterpret_cast<cudaStream_t>(stream), z, dy, mean,
-              invstd, gamma, beta, resid, act, sums, inv_count, dz, dres, rows * C, C);
-  return AVSR_OK;
+  return launch_bn_stats(z, M, g.Cout, part, stats, st);
 }
 
 extern "C" size_t avsr_frontend_train_dgrad_workspace_bytes(int N, int H, int W, int C_in, int C_out, int KH, int KW,

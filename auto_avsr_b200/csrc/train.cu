@@ -1,7 +1,8 @@
 // Training slice of the encoder path (SURVEY.md 8f #2, first slice): backward of the HBM-bound kernels and the pieces a
 // Linear's backward needs around the tensor-core GEMMs -- LayerNorm backward, bias gradients (column sums), fp32
-// transpose (so that dgrad / wgrad are the SAME wgmma GEMMs on transposed operands), ReLU backward, and the
-// depthwise-conv + BatchNorm(batch statistics) + SiLU block forward / backward incl. the running-statistics update.
+// transpose (so that dgrad / wgrad are the SAME wgmma GEMMs on transposed operands), ReLU backward, the depthwise
+// conv's forward / backward, and the batch-statistics BatchNorm [+ SiLU] of the conformer conv module and the front-end
+// convolutions, forward / backward incl. the running-statistics update.
 // Reference: lightning.py:86-94 (training_step), conformer_encoder.py:26,30-35 (BatchNorm1d in train mode sees ALL B*T
 // frames incl. padding), layer_norm.py:21, positionwise_feed_forward.py:28-30.  fp32 math; every cross-row reduction is
 // a two-stage (per-CTA partials, fixed-order finish) sum: results do not depend on scheduling.
@@ -184,69 +185,179 @@ __global__ void glu_bwd_kernel(const float* __restrict__ in, const float* __rest
   }
 }
 
-// ------------------------------------------------------------------ BatchNorm (batch statistics) + SiLU
-// per-channel partial sums of v - shift and (v - shift)^2 over a block of rows: part[blk][2][C] (shift NULL: 0).  With
-// shift = a provisional mean the sums are centred, so the variance does not come from the difference of two large sums.
-__global__ void __launch_bounds__(256) chan_stats_partial_kernel(const float* __restrict__ v, const float* __restrict__ shift,
-                                                                 float* __restrict__ part, int rows, int C, int rows_per_cta) {
-  const int r0 = blockIdx.x * rows_per_cta, r1 = min(rows, r0 + rows_per_cta);
-  for (int c = threadIdx.x; c < C; c += 256) {
-    const float m = shift ? shift[c] : 0.f;
-    float s = 0.f, q = 0.f;
-    for (int r = r0; r < r1; ++r) { const float t = v[(long)r * C + c] - m; s += t; q += t * t; }
-    part[((long)blockIdx.x * 2) * C + c] = s;
-    part[((long)blockIdx.x * 2 + 1) * C + c] = q;
+// ------------------------------------------------------------------ BatchNorm with batch statistics (training)
+// The conformer conv module's BatchNorm1d and the front-end convolutions' BatchNorm2d share these kernels.  Statistics:
+// per-tile (count, mean, M2) of every channel, merged in a fixed order with Chan's formula in fp64 (no one-pass
+// variance).  Normalise [+ residual] [+ SiLU]; the backward's per-tile [sum ds, sum ds * x_hat] are summed in fp64.
+// A tile is bn_tile_rows() rows of 128 channels.
+
+// rows per tile: 256, halved (down to 32) while the grid would hold fewer than two CTAs per SM
+static int bn_tile_rows(long rows, int C) {
+  int h = 256;
+  while (h > 32 && (rows + h - 1) / h * cdiv(C, 128) < 2 * 132) h >>= 1;
+  return h;
+}
+
+// per-tile (count, mean, M2) of each channel of z (rows, C): part[tile][3][C].  Both passes sum z - (the tile's first
+// row) in fp32, so a channel whose mean lies many standard deviations from 0 keeps its mean and variance.
+__global__ void __launch_bounds__(128) bn_stats_partial_kernel(const float* __restrict__ z, double* __restrict__ part,
+                                                               long rows, int C, int tile_rows) {
+  pdl_wait();
+  const int c = blockIdx.y * 128 + threadIdx.x;
+  if (c >= C) return;
+  const long r0 = (long)blockIdx.x * tile_rows, r1 = min(rows, r0 + tile_rows);
+  const int n = (int)(r1 - r0);
+  const float z0 = z[r0 * C + c];
+  float s = 0.f;
+  for (long r = r0; r < r1; ++r) s += z[r * C + c] - z0;
+  const float dm = s / (float)n;
+  float q = 0.f;
+  for (long r = r0; r < r1; ++r) { const float d = (z[r * C + c] - z0) - dm; q = fmaf(d, d, q); }
+  double* p = part + (long)blockIdx.x * 3 * C;
+  p[c] = n; p[C + c] = (double)z0 + (double)dm; p[2 * C + c] = q;
+}
+
+__device__ __forceinline__ void chan_merge(double& n, double& m, double& q, double nb, double mb, double qb) {
+  if (nb == 0.0) return;
+  const double nn = n + nb, d = mb - m;
+  m += d * (nb / nn);
+  q += qb + d * d * (n * nb / nn);
+  n = nn;
+}
+
+// one CTA per channel: thread t merges tiles t, t + 256, ... in order, then a fixed tree; out[3][C]
+__global__ void __launch_bounds__(256) bn_stats_merge_kernel(const double* __restrict__ part, int tiles, int C,
+                                                             double* __restrict__ out) {
+  pdl_wait();
+  __shared__ double sn[256], sm[256], sq[256];
+  const int c = blockIdx.x, t = threadIdx.x;
+  double n = 0, m = 0, q = 0;
+  for (int i = t; i < tiles; i += 256) {
+    const double* p = part + (long)i * 3 * C;
+    chan_merge(n, m, q, p[c], p[C + c], p[2 * C + c]);
   }
-}
-// y = silu((v - mean) * invstd * gamma + beta)
-__global__ void bn_silu_fwd_kernel(const float4* __restrict__ v, const float* __restrict__ mean, const float* __restrict__ invstd,
-                                   const float* __restrict__ gamma, const float* __restrict__ beta, float4* __restrict__ y,
-                                   long n4, int C4) {
-  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n4; i += (long)gridDim.x * blockDim.x) {
-    const int c = (int)(i % C4);
-    const float4 a = v[i], m = reinterpret_cast<const float4*>(mean)[c], s = reinterpret_cast<const float4*>(invstd)[c];
-    const float4 g = reinterpret_cast<const float4*>(gamma)[c], b = reinterpret_cast<const float4*>(beta)[c];
-    float4 h = make_float4((a.x - m.x) * s.x * g.x + b.x, (a.y - m.y) * s.y * g.y + b.y, (a.z - m.z) * s.z * g.z + b.z,
-                           (a.w - m.w) * s.w * g.w + b.w);
-    y[i] = make_float4(h.x * sigmoidf_acc(h.x), h.y * sigmoidf_acc(h.y), h.z * sigmoidf_acc(h.z), h.w * sigmoidf_acc(h.w));
-  }
-}
-// ds = dL/dh of y = silu(h): dy * sig(h) * (1 + h * (1 - sig(h)))
-__device__ __forceinline__ float silu_grad(float h, float dy) {
-  const float s = sigmoidf_acc(h);
-  return dy * s * (1.0f + h * (1.0f - s));
-}
-// per-channel partial sums of ds and ds * x_hat (h recomputed from the saved conv output): part[blk][2][C]
-__global__ void __launch_bounds__(256) bn_bwd_partial_kernel(const float* __restrict__ v, const float* __restrict__ dy,
-                                                             const float* __restrict__ mean, const float* __restrict__ invstd,
-                                                             const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                             float* __restrict__ part, int rows, int C, int rows_per_cta) {
-  const int r0 = blockIdx.x * rows_per_cta, r1 = min(rows, r0 + rows_per_cta);
-  for (int c = threadIdx.x; c < C; c += 256) {
-    const float m = mean[c], is = invstd[c], g = gamma[c], b = beta[c];
-    float s = 0.f, q = 0.f;
-    for (int r = r0; r < r1; ++r) {
-      const float xh = (v[(long)r * C + c] - m) * is;
-      const float ds = silu_grad(xh * g + b, dy[(long)r * C + c]);
-      s += ds; q += ds * xh;
+  sn[t] = n; sm[t] = m; sq[t] = q;
+  __syncthreads();
+  for (int h = 128; h > 0; h >>= 1) {
+    if (t < h) {
+      double a = sn[t], b = sm[t], e = sq[t];
+      chan_merge(a, b, e, sn[t + h], sm[t + h], sq[t + h]);
+      sn[t] = a; sm[t] = b; sq[t] = e;
     }
-    part[((long)blockIdx.x * 2) * C + c] = s;
-    part[((long)blockIdx.x * 2 + 1) * C + c] = q;
+    __syncthreads();
   }
+  if (t == 0) { out[c] = sn[0]; out[C + c] = sm[0]; out[2 * C + c] = sq[0]; }
 }
-// dconv = gamma * invstd / N * (N * ds - dbeta - x_hat * dgamma)
-__global__ void bn_bwd_dx_kernel(const float* __restrict__ v, const float* __restrict__ dy, const float* __restrict__ mean,
-                                 const float* __restrict__ invstd, const float* __restrict__ gamma, const float* __restrict__ beta,
-                                 const float* __restrict__ dgamma, const float* __restrict__ dbeta, float* __restrict__ dv, long n,
-                                 int C, float inv_rows) {
-  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
-    const int c = (int)(i % C);
-    const float xh = (v[i] - mean[c]) * invstd[c];
-    const float ds = silu_grad(xh * gamma[c] + beta[c], dy[i]);
-    dv[i] = gamma[c] * invstd[c] * (ds - inv_rows * (dbeta[c] + xh * dgamma[c]));
+
+// merge R ranks' (count, mean, M2) in rank order; mean, 1/sqrt(var + eps) with the biased variance; running statistics
+// (when given) move by `factor` toward the mean and the unbiased variance
+__global__ void bn_finalize_kernel(const double* __restrict__ st, int R, int C, double eps, double factor,
+                                   float* __restrict__ running_mean, float* __restrict__ running_var,
+                                   float* __restrict__ mean, float* __restrict__ invstd) {
+  pdl_wait();
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  double n = 0, m = 0, q = 0;
+  for (int r = 0; r < R; ++r) chan_merge(n, m, q, st[(long)r * 3 * C + c], st[(long)r * 3 * C + C + c],
+                                         st[(long)r * 3 * C + 2 * C + c]);
+  const double var = n > 0 ? q / n : 0.0;
+  mean[c] = (float)m;
+  invstd[c] = (float)(1.0 / sqrt(var + eps));
+  if (running_mean) {
+    const double unb = n > 1 ? q / (n - 1) : var;
+    running_mean[c] = (float)((1.0 - factor) * running_mean[c] + factor * m);
+    running_var[c] = (float)((1.0 - factor) * running_var[c] + factor * unb);
   }
 }
 
+// ds = dL/dh of y = silu(h): dy * sig(h) * (1 + h * (1 - sig(h)))
+__device__ __forceinline__ float silu_grad_acc(float h, float dy) {
+  const float s = sigmoidf_acc(h);
+  return dy * s * (1.0f + h * (1.0f - s));
+}
+
+// y = [SiLU]((z - mean) * invstd * gamma + beta [+ resid])
+__global__ void bn_act_fwd_kernel(const float* __restrict__ z, const float* __restrict__ mean,
+                                  const float* __restrict__ invstd, const float* __restrict__ gamma,
+                                  const float* __restrict__ beta, const float* __restrict__ resid, int act,
+                                  float* __restrict__ y, long n, int C) {
+  pdl_wait();
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    float h = (z[i] - mean[c]) * invstd[c] * gamma[c] + beta[c];
+    if (resid) h += resid[i];
+    y[i] = act ? h * sigmoidf_acc(h) : h;
+  }
+}
+
+// ds = dL/d(BN output): dy, through SiLU when act; per-tile [sum ds, sum ds * x_hat]: part[tile][2][C] (fp64)
+__global__ void __launch_bounds__(128) bn_bwd_partial_kernel(const float* __restrict__ z, const float* __restrict__ dy,
+                                                             const float* __restrict__ mean,
+                                                             const float* __restrict__ invstd,
+                                                             const float* __restrict__ gamma,
+                                                             const float* __restrict__ beta,
+                                                             const float* __restrict__ resid, int act,
+                                                             double* __restrict__ part, long rows, int C,
+                                                             int tile_rows) {
+  pdl_wait();
+  const int c = blockIdx.y * 128 + threadIdx.x;
+  if (c >= C) return;
+  const long r0 = (long)blockIdx.x * tile_rows, r1 = min(rows, r0 + tile_rows);
+  const float m = mean[c], is = invstd[c], g = gamma[c], b = beta[c];
+  float s = 0.f, q = 0.f;
+  for (long r = r0; r < r1; ++r) {
+    const long i = r * C + c;
+    const float xh = (z[i] - m) * is;
+    float ds = dy[i];
+    if (act) ds = silu_grad_acc(xh * g + b + (resid ? resid[i] : 0.f), ds);
+    s += ds;
+    q = fmaf(ds, xh, q);
+  }
+  part[(long)blockIdx.x * 2 * C + c] = s;
+  part[(long)blockIdx.x * 2 * C + C + c] = q;
+}
+
+// out[j] = sum_t part[t][j] in fp64, one CTA per column j: strided per-thread sums, then a fixed tree
+__global__ void __launch_bounds__(256) bn_sum_merge_kernel(const double* __restrict__ part, int tiles, int width,
+                                                           float* __restrict__ out) {
+  pdl_wait();
+  __shared__ double sh[256];
+  const int j = blockIdx.x, t = threadIdx.x;
+  double s = 0;
+  for (int i = t; i < tiles; i += 256) s += part[(long)i * width + j];
+  sh[t] = s;
+  __syncthreads();
+  for (int h = 128; h > 0; h >>= 1) {
+    if (t < h) sh[t] += sh[t + h];
+    __syncthreads();
+  }
+  if (t == 0) out[j] = (float)sh[0];
+}
+
+// dz = gamma * invstd * (ds - (sum ds + x_hat * sum ds x_hat) / count); dres (when given) = ds
+__global__ void bn_bwd_dx_kernel(const float* __restrict__ z, const float* __restrict__ dy,
+                                 const float* __restrict__ mean, const float* __restrict__ invstd,
+                                 const float* __restrict__ gamma, const float* __restrict__ beta,
+                                 const float* __restrict__ resid, int act, const float* __restrict__ sums,
+                                 float inv_count, float* __restrict__ dz, float* __restrict__ dres, long n, int C) {
+  pdl_wait();
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    const float g = gamma[c], is = invstd[c];
+    const float xh = (z[i] - mean[c]) * is;
+    float ds = dy[i];
+    if (act) ds = silu_grad_acc(xh * g + beta[c] + (resid ? resid[i] : 0.f), ds);
+    if (dres) dres[i] = ds;
+    dz[i] = g * is * (ds - inv_count * (sums[c] + xh * sums[C + c]));
+  }
+}
+
+int launch_bn_stats(const float* z, long rows, int C, double* part, double* stats, cudaStream_t st) {
+  const int h = bn_tile_rows(rows, C), tiles = (int)((rows + h - 1) / h);
+  AVSR_LAUNCH(bn_stats_partial_kernel, dim3(tiles, cdiv(C, 128)), 128, 0, st, z, part, rows, C, h);
+  AVSR_LAUNCH(bn_stats_merge_kernel, C, 256, 0, st, (const double*)part, tiles, C, stats);
+  return AVSR_OK;
+}
 // ------------------------------------------------------------------ depthwise conv backward: tap / bias gradients
 // dw[c][k] = sum_{b,t} x[b, t+k-half, c] * dconv[b,t,c] ; db[c] = sum dconv.  part[blk][K+1][C], one CTA per block of
 // (utterance, frame range); threads over channels (coalesced along C).
@@ -438,9 +549,7 @@ int avsr_glu_bwd(const float* in, const float* dy, float* din, long rows, int C,
   return AVSR_OK;
 }
 
-// ---- depthwise conv + BatchNorm (training) + SiLU, in the pieces a (Sync)BatchNorm needs: the per-channel sums leave the
-// library between the pieces so that the host can all-reduce them over the ranks (torch.nn.SyncBatchNorm semantics,
-// train.py:31) before the statistics are finalised.
+// ---- depthwise conv of the conformer conv module (its training BatchNorm is the avsr_bn_train_* below)
 
 // y = depthwise_conv(x) + b (raw fp32; flip != 0: taps reversed along k and b may be NULL -- the input gradient)
 int avsr_dwconv_raw(const float* x, const float* w, const float* b, float* y, int B, int T, int C, int K, int flip,
@@ -460,50 +569,6 @@ int avsr_dwconv_raw(const float* x, const float* w, const float* b, float* y, in
   return launch_dwconv_bn_silu(x, wt, ones, b ? b : zeros, y, B, T, C, K, /*out_kind=*/-1, st);
 }
 
-// sums (2, C): dy == NULL -> [sum v, sum v^2] over the rows, or with mean given the centred [sum (v - mean),
-// sum (v - mean)^2] (the second pass of the batch statistics); else the BatchNorm+SiLU backward sums [sum ds, sum ds*x_hat]
-// with h = x_hat * gamma + beta, ds = dL/dh of y = silu(h)
-int avsr_chan_sums(const float* v, const float* dy, const float* mean, const float* invstd, const float* gamma,
-                   const float* beta, float* sums, int rows, int C, void* workspace, size_t workspace_bytes, void* stream) {
-  AVSR_REQUIRE(v && sums && workspace && C > 0, "NULL / bad argument");
-  AVSR_REQUIRE(!dy || (mean && invstd && gamma && beta), "chan_sums: the backward sums need mean / invstd / gamma / beta");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (rows <= 0) { AVSR_CUDA_TRY(cudaMemsetAsync(sums, 0, 2 * C * sizeof(float), st)); return AVSR_OK; }
-  const int rpc = cdiv(rows, kRedBlocks), nb = cdiv(rows, rpc);
-  AVSR_REQUIRE_BYTES((size_t)nb * 2 * C * sizeof(float), workspace_bytes, "chan_sums workspace");
-  float* part = reinterpret_cast<float*>(workspace);
-  if (dy) bn_bwd_partial_kernel<<<nb, 256, 0, st>>>(v, dy, mean, invstd, gamma, beta, part, rows, C, rpc);
-  else chan_stats_partial_kernel<<<nb, 256, 0, st>>>(v, mean, part, rows, C, rpc);
-  AVSR_CHECK_LAUNCH();
-  reduce_partials_kernel<<<cdiv(2 * C, 256), 256, 0, st>>>(part, sums, nb, 2 * C);
-  AVSR_CHECK_LAUNCH();
-  return AVSR_OK;
-}
-
-// y = silu((v - mean) * invstd * gamma + beta)
-int avsr_bn_silu_fwd(const float* v, const float* mean, const float* invstd, const float* gamma, const float* beta, float* y,
-                     int rows, int C, void* stream) {
-  AVSR_REQUIRE(v && mean && invstd && gamma && beta && y && C > 0 && C % 4 == 0, "NULL / bad argument");
-  if (rows <= 0) return AVSR_OK;
-  bn_silu_fwd_kernel<<<grid_for((long)rows * C / 4), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const float4*>(v), mean, invstd, gamma, beta, reinterpret_cast<float4*>(y), (long)rows * C / 4, C / 4);
-  AVSR_CHECK_LAUNCH();
-  return AVSR_OK;
-}
-
-// dv = gamma * invstd * (ds - inv_count * (sum_ds + x_hat * sum_dsx)): sum_ds / sum_dsx (C) and inv_count are GLOBAL
-// (over all ranks' rows under SyncBatchNorm)
-int avsr_bn_silu_bwd_dx(const float* v, const float* dy, const float* mean, const float* invstd, const float* gamma,
-                        const float* beta, const float* sum_ds, const float* sum_dsx, float inv_count, float* dv, int rows,
-                        int C, void* stream) {
-  AVSR_REQUIRE(v && dy && mean && invstd && gamma && beta && sum_ds && sum_dsx && dv && C > 0, "NULL / bad argument");
-  if (rows <= 0) return AVSR_OK;
-  bn_bwd_dx_kernel<<<grid_for((long)rows * C), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      v, dy, mean, invstd, gamma, beta, sum_dsx, sum_ds, dv, (long)rows * C, C, inv_count);
-  AVSR_CHECK_LAUNCH();
-  return AVSR_OK;
-}
-
 // dw (C,1,K), db (C) of the depthwise conv from its input x and its output gradient dconv
 int avsr_dwconv_wgrad(const float* x, const float* dconv, float* dw, float* db, int B, int T, int C, int K, void* workspace,
                       size_t workspace_bytes, void* stream) {
@@ -521,6 +586,77 @@ int avsr_dwconv_wgrad(const float* x, const float* dconv, float* dw, float* db, 
   AVSR_CHECK_LAUNCH();
   dwconv_wgrad_finish_kernel<<<cdiv((K + 1) * C, 256), 256, 0, st>>>(partw, dw, db, nbw, C, K);
   AVSR_CHECK_LAUNCH();
+  return AVSR_OK;
+}
+
+// ---- BatchNorm with batch statistics, in the pieces a (Sync)BatchNorm needs: the per-rank statistics and the backward
+// sums leave the library between the pieces, so that the host can gather / all-reduce them over the ranks
+// (torch.nn.SyncBatchNorm semantics, train.py:31) before they are used.
+
+size_t avsr_bn_train_workspace_bytes(long rows, int C) {
+  if (rows < 0 || C < 1) return 0;
+  const int h = bn_tile_rows(rows, C);
+  return align_up((size_t)((rows + h - 1) / h) * 3 * C * sizeof(double), 256) + 256;
+}
+
+int avsr_bn_train_stats(const float* z, long rows, int C, double* stats, void* workspace, size_t workspace_bytes,
+                        void* stream) {
+  AVSR_REQUIRE(rows >= 0 && C >= 1, "bn_train: bad rows=%ld C=%d", rows, C);
+  AVSR_REQUIRE(stats && workspace, "NULL argument");
+  AVSR_REQUIRE_BYTES(avsr_bn_train_workspace_bytes(rows, C), workspace_bytes, "bn_train workspace");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (rows == 0) {               // no rows (z may be NULL): count 0, which the rank merge skips
+    AVSR_CUDA_TRY(cudaMemsetAsync(stats, 0, 3 * (size_t)C * sizeof(double), st));
+    return AVSR_OK;
+  }
+  AVSR_REQUIRE(z, "NULL argument");
+  double* part = reinterpret_cast<double*>(align_up(reinterpret_cast<uintptr_t>(workspace), 256));
+  return launch_bn_stats(z, rows, C, part, stats, st);
+}
+
+int avsr_bn_train_finalize(const double* stats, int ranks, int C, double eps, double factor, float* running_mean,
+                           float* running_var, float* mean, float* invstd, void* stream) {
+  AVSR_REQUIRE(ranks >= 1 && C >= 1 && eps >= 0.0 && factor >= 0.0 && factor <= 1.0,
+               "bn_train: bad ranks=%d C=%d eps or factor", ranks, C);
+  AVSR_REQUIRE(stats && mean && invstd && (running_mean != nullptr) == (running_var != nullptr), "NULL argument");
+  AVSR_LAUNCH(bn_finalize_kernel, cdiv(C, 128), 128, 0, reinterpret_cast<cudaStream_t>(stream), stats, ranks, C, eps,
+              factor, running_mean, running_var, mean, invstd);
+  return AVSR_OK;
+}
+
+int avsr_bn_train_act_fwd(const float* z, const float* mean, const float* invstd, const float* gamma, const float* beta,
+                          const float* resid, int act, float* y, long rows, int C, void* stream) {
+  AVSR_REQUIRE(rows >= 0 && C >= 1, "bn_train: bad rows=%ld C=%d", rows, C);
+  AVSR_REQUIRE(z && mean && invstd && gamma && beta && y, "NULL argument");
+  if (rows == 0) return AVSR_OK;
+  AVSR_LAUNCH(bn_act_fwd_kernel, grid_for(rows * C, 256, 8192), 256, 0, reinterpret_cast<cudaStream_t>(stream), z, mean,
+              invstd, gamma, beta, resid, act, y, rows * C, C);
+  return AVSR_OK;
+}
+
+int avsr_bn_train_bwd_sums(const float* z, const float* dy, const float* mean, const float* invstd, const float* gamma,
+                           const float* beta, const float* resid, int act, float* sums, long rows, int C,
+                           void* workspace, size_t workspace_bytes, void* stream) {
+  AVSR_REQUIRE(rows >= 1 && C >= 1, "bn_train: bad rows=%ld C=%d", rows, C);
+  AVSR_REQUIRE(z && dy && mean && invstd && gamma && beta && sums && workspace, "NULL argument");
+  AVSR_REQUIRE_BYTES(avsr_bn_train_workspace_bytes(rows, C), workspace_bytes, "bn_train backward workspace");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  double* part = reinterpret_cast<double*>(align_up(reinterpret_cast<uintptr_t>(workspace), 256));
+  const int h = bn_tile_rows(rows, C), tiles = (int)((rows + h - 1) / h);
+  AVSR_LAUNCH(bn_bwd_partial_kernel, dim3(tiles, cdiv(C, 128)), 128, 0, st, z, dy, mean, invstd, gamma, beta, resid,
+              act, part, rows, C, h);
+  AVSR_LAUNCH(bn_sum_merge_kernel, 2 * C, 256, 0, st, (const double*)part, tiles, 2 * C, sums);
+  return AVSR_OK;
+}
+
+int avsr_bn_train_bwd_dx(const float* z, const float* dy, const float* mean, const float* invstd, const float* gamma,
+                         const float* beta, const float* resid, int act, const float* sums, float inv_count, float* dz,
+                         float* dres, long rows, int C, void* stream) {
+  AVSR_REQUIRE(rows >= 0 && C >= 1, "bn_train: bad rows=%ld C=%d", rows, C);
+  AVSR_REQUIRE(z && dy && mean && invstd && gamma && beta && sums && dz, "NULL argument");
+  if (rows == 0) return AVSR_OK;
+  AVSR_LAUNCH(bn_bwd_dx_kernel, grid_for(rows * C, 256, 8192), 256, 0, reinterpret_cast<cudaStream_t>(stream), z, dy,
+              mean, invstd, gamma, beta, resid, act, sums, inv_count, dz, dres, rows * C, C);
   return AVSR_OK;
 }
 

@@ -6,13 +6,14 @@ Gradients land on the original ``Parameter``s (20 conv weights, 20 BatchNorm wei
 the two gradients that reach a BasicBlock's input) and the collectives; every unit's forward and backward arithmetic
 runs in the library.
 
-BatchNorm follows torch's training semantics exactly: statistics over every position the module normalises (padded
-frames and samples included), the biased variance to normalise, the unbiased one for ``running_var``,
-``num_batches_tracked`` incremented (``momentum=None`` is the cumulative average), and under ``torch.no_grad()`` the
-batch statistics are still used and the running statistics still updated.  The statistics are per-tile
-(count, mean, M2) merged with Chan's formula in fp64, never a one-pass sum of squares.  ``SyncBatchNorm`` with a group
-of more than one rank all-gathers the per-rank (count, mean, M2) and merges them in rank order, and all-reduces
-[sum ds, sum ds * x_hat] in backward; d gamma / d beta stay local sums (DDP averages them).
+BatchNorm is the step the conformer conv module uses too (``train.bn_train_forward`` / ``bn_train_backward``), fed
+with the statistics the conv computes: torch's training semantics exactly -- statistics over every position the module
+normalises (padded frames and samples included), the biased variance to normalise, the unbiased one for
+``running_var``, ``num_batches_tracked`` incremented (``momentum=None`` is the cumulative average), and under
+``torch.no_grad()`` the batch statistics are still used and the running statistics still updated.  The statistics are
+per-tile (count, mean, M2) merged with Chan's formula in fp64, never a one-pass sum of squares.  ``SyncBatchNorm`` with
+a group of more than one rank all-gathers the per-rank (count, mean, M2) and merges them in rank order, and
+all-reduces [sum ds, sum ds * x_hat] in backward; d gamma / d beta stay local sums (DDP averages them).
 
 Forward convolutions run in the module's precision; dgrad and wgrad on wgmma with TF32 operands unless
 ``precision="fp32"`` (gradients do not fit fp16's range), which runs both on CUDA cores in fp32."""
@@ -24,18 +25,7 @@ import torch
 
 from ._cabi import check, lib
 from .engine import PRECISIONS, _ptr, _stream_handle, default_precision
-from .train import _c, _workspace, bwd_precision
-
-
-def _sync_group(bn):
-    """The process group a SyncBatchNorm slot reduces over, or None for a plain BatchNorm / one rank."""
-    if not isinstance(bn, torch.nn.SyncBatchNorm):
-        return None
-    import torch.distributed as dist
-    if not (dist.is_available() and dist.is_initialized()):
-        return None
-    group = bn.process_group if bn.process_group is not None else dist.group.WORLD
-    return None if dist.get_world_size(group) == 1 else group
+from .train import _c, _sync_group, _workspace, bn_train_backward, bn_train_forward, bwd_precision
 
 
 class _Spec:
@@ -74,8 +64,6 @@ class ConvBnActFn(torch.autograd.Function):
         x, weight, gamma, beta = _c(x), _c(weight), _c(gamma), _c(beta)
         resid = _c(resid) if resid is not None else None
         dev, C = x.device, spec.Cout
-        if group is None and spec.rows <= 1:
-            raise ValueError(f"Expected more than 1 value per channel when training, got {spec.rows} (BatchNorm)")
         p = PRECISIONS[precision]
         z = torch.empty(spec.rows, C, dtype=torch.float32, device=dev)
         stats = torch.empty(3, C, dtype=torch.float64, device=dev)
@@ -83,55 +71,18 @@ class ConvBnActFn(torch.autograd.Function):
         with torch.cuda.device(dev):
             check(lib.avsr_frontend_train_conv_fwd(x.data_ptr(), weight.data_ptr(), z.data_ptr(), stats.data_ptr(),
                                                    *spec.args(), ws.data_ptr(), ws.numel(), p, _stream_handle(dev)))
-        ranks = 1
-        if group is not None:
-            import torch.distributed as dist
-            parts = [torch.empty_like(stats) for _ in range(dist.get_world_size(group))]
-            dist.all_gather(parts, stats, group=group)
-            stats, ranks = torch.stack(parts), len(parts)
-        count = float(stats.view(ranks, 3, C)[:, 0, 0].sum().item()) if ranks > 1 else float(spec.rows)
-        if count <= 1:
-            raise ValueError(f"Expected more than 1 value per channel when training, got {int(count)} (BatchNorm)")
-        # torch's _BatchNorm.forward: count this batch, then the averaging factor
-        bn.num_batches_tracked.add_(1)
-        factor = bn.momentum if bn.momentum is not None else 1.0 / float(bn.num_batches_tracked.item())
-        mean = torch.empty(C, dtype=torch.float32, device=dev)
-        invstd = torch.empty_like(mean)
-        y = torch.empty(spec.N, spec.Ho, spec.Wo, C, dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            check(lib.avsr_frontend_train_bn_finalize(stats.data_ptr(), ranks, C, float(bn.eps), float(factor),
-                                                      bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
-                                                      mean.data_ptr(), invstd.data_ptr(), _stream_handle(dev)))
-            check(lib.avsr_frontend_train_bn_act_fwd(z.data_ptr(), mean.data_ptr(), invstd.data_ptr(), gamma.data_ptr(),
-                                                     beta.data_ptr(), _ptr(resid), int(act), y.data_ptr(), spec.rows, C,
-                                                     _stream_handle(dev)))
+        y, mean, invstd, count = bn_train_forward(z, gamma, beta, bn, group, resid, act, stats)
         ctx.save_for_backward(x, resid, weight, z, mean, invstd, gamma, beta)
         ctx.spec, ctx.act, ctx.precision, ctx.group, ctx.count = spec, act, precision, group, count
-        return y
+        return y.view(spec.N, spec.Ho, spec.Wo, C)
 
     @staticmethod
     def backward(ctx, dy):
         x, resid, weight, z, mean, invstd, gamma, beta = ctx.saved_tensors
         spec, dev, C = ctx.spec, x.device, ctx.spec.Cout
-        dy = _c(dy)
-        sums = torch.empty(2, C, dtype=torch.float32, device=dev)
-        ws = _workspace(dev, int(lib.avsr_frontend_train_bn_bwd_workspace_bytes(spec.rows, C)))
-        with torch.cuda.device(dev):
-            check(lib.avsr_frontend_train_bn_bwd_sums(z.data_ptr(), dy.data_ptr(), mean.data_ptr(), invstd.data_ptr(),
-                                                      gamma.data_ptr(), beta.data_ptr(), _ptr(resid), int(ctx.act),
-                                                      sums.data_ptr(), spec.rows, C, ws.data_ptr(), ws.numel(),
-                                                      _stream_handle(dev)))
-        dbeta, dgamma = sums[0].clone(), sums[1].clone()       # local sums: DDP averages the parameter gradients
-        if ctx.group is not None:
-            import torch.distributed as dist
-            dist.all_reduce(sums, group=ctx.group)
-        dz = torch.empty_like(z)
-        dres = torch.empty_like(z) if resid is not None and ctx.needs_input_grad[1] else None
-        with torch.cuda.device(dev):
-            check(lib.avsr_frontend_train_bn_bwd_dx(z.data_ptr(), dy.data_ptr(), mean.data_ptr(), invstd.data_ptr(),
-                                                    gamma.data_ptr(), beta.data_ptr(), _ptr(resid), int(ctx.act),
-                                                    sums.data_ptr(), 1.0 / ctx.count, dz.data_ptr(), _ptr(dres),
-                                                    spec.rows, C, _stream_handle(dev)))
+        dz, dres, dgamma, dbeta = bn_train_backward(z, _c(dy).view(-1, C), mean, invstd, gamma, beta, ctx.count,
+                                                    ctx.group, resid, ctx.act,
+                                                    resid is not None and ctx.needs_input_grad[1])
         pb = PRECISIONS[bwd_precision(ctx.precision)]
         dw = torch.empty_like(weight)
         ws = _workspace(dev, int(lib.avsr_frontend_train_wgrad_workspace_bytes(*spec.args())))

@@ -1,13 +1,16 @@
 """Training slice of the encoder path (SURVEY.md 8f #2, first slice): ``torch.autograd.Function``s whose forward AND
 backward run in libavsr_b200 -- LayerNorm, Linear (+ReLU) with dgrad / wgrad as the same wgmma GEMMs on transposed
-operands, GLU, and the depthwise-conv + BatchNorm(batch statistics) + SiLU block.  Gradients land on the original
-``nn.Parameter``s (autograd accumulates what ``backward`` returns), so DDP hooks, ``clip_grad_norm_`` and AdamW
-(lightning.py:49, train.py:37-41) see them unchanged.  torch supplies device memory, the autograd tape, dropout masks
-and the residual adds; no module falls back to PyTorch arithmetic for its own forward or backward.
+operands, GLU, the depthwise conv, and the batch-statistics BatchNorm step (``bn_train_forward`` /
+``bn_train_backward``) that the conformer conv module and the ResNet front-ends (frontend_train.py) share: per-tile
+(count, mean, M2) merged with Chan's formula in fp64, running statistics as torch keeps them.  Gradients land on the
+original ``nn.Parameter``s (autograd accumulates what ``backward`` returns), so DDP hooks, ``clip_grad_norm_`` and
+AdamW (lightning.py:49, train.py:37-41) see them unchanged.  torch supplies device memory, the autograd tape, dropout
+masks and the residual adds; no module falls back to PyTorch arithmetic for its own forward or backward.
 
 The rel-pos attention core has a (correctness-first, fp32 CUDA-core) backward too, so a whole ``EncoderLayer`` /
 ``ConformerEncoder`` runs ``train()``: the reference's layer schedule with its dropouts (conformer_encoder.py:96-170).
-SyncBatchNorm (train.py:31) is honoured: the per-channel sums are all-reduced between the library's passes.
+SyncBatchNorm (train.py:31) is honoured: the per-rank (count, mean, M2) are all-gathered and merged in rank order, and
+[sum ds, sum ds * x_hat] all-reduced in backward.
 Not built: dropout on attention probabilities (the reference trains with 0.0).
 
 Backward GEMMs run with TF32 operands (fp32 range: gradients do not fit fp16's) unless ``precision="fp32"``; a "bf16"
@@ -220,19 +223,6 @@ class GluFn(torch.autograd.Function):
         return dx
 
 
-def _chan_sums(v, dy=None, mean=None, invstd=None, gamma=None, beta=None):
-    """(2, C): [sum v, sum v^2] over all rows, with ``mean`` alone the centred [sum (v - mean), sum (v - mean)^2], or
-    (dy given) the BatchNorm+SiLU backward sums [sum ds, sum ds * x_hat]."""
-    Cc = v.size(-1)
-    rows = v.numel() // Cc
-    out = torch.empty(2, Cc, dtype=torch.float32, device=v.device)
-    ws = _workspace(v.device, 132 * 2 * Cc * 4 + 1024)
-    with torch.cuda.device(v.device):
-        check(lib.avsr_chan_sums(v.data_ptr(), _ptr(dy), _ptr(mean), _ptr(invstd), _ptr(gamma), _ptr(beta), out.data_ptr(),
-                                 rows, Cc, ws.data_ptr(), ws.numel(), _stream_handle(v.device)))
-    return out
-
-
 def _dwconv_raw(x, w, b, flip: bool):
     B, T, Cc = x.shape
     K = w.size(-1)
@@ -244,80 +234,116 @@ def _dwconv_raw(x, w, b, flip: bool):
     return y
 
 
+def _sync_group(bn):
+    """The process group a SyncBatchNorm slot reduces over, or None for a plain BatchNorm / one rank."""
+    if not isinstance(bn, torch.nn.SyncBatchNorm):
+        return None
+    import torch.distributed as dist
+    if not (dist.is_available() and dist.is_initialized()):
+        return None
+    group = bn.process_group if bn.process_group is not None else dist.group.WORLD
+    return None if dist.get_world_size(group) == 1 else group
+
+
+def bn_train_forward(z, gamma, beta, bn, group, resid=None, act: bool = True, stats=None):
+    """BatchNorm in training on z (rows, C) fp32 [+ resid] [-> SiLU] -> (y (rows, C), mean, invstd, count).
+
+    ``stats`` is z's (3, C) fp64 (count, mean, M2) when the caller already has it (the front-end's conv produces it),
+    else avsr_bn_train_stats computes it.  Under a SyncBatchNorm ``group`` the ranks' statistics are all-gathered and
+    merged in rank order, so ``count`` is the global row count.  ``bn``'s running statistics and num_batches_tracked
+    move as torch's _BatchNorm.forward moves them (``momentum=None``: the cumulative average)."""
+    rows, C = z.shape
+    dev = z.device
+    if stats is None:
+        stats = torch.empty(3, C, dtype=torch.float64, device=dev)
+        ws = _workspace(dev, int(lib.avsr_bn_train_workspace_bytes(rows, C)))
+        with torch.cuda.device(dev):
+            check(lib.avsr_bn_train_stats(z.data_ptr(), rows, C, stats.data_ptr(), ws.data_ptr(), ws.numel(),
+                                          _stream_handle(dev)))
+    ranks = 1
+    if group is not None:
+        import torch.distributed as dist
+        parts = [torch.empty_like(stats) for _ in range(dist.get_world_size(group))]
+        dist.all_gather(parts, stats, group=group)
+        stats, ranks = torch.stack(parts), len(parts)
+    count = float(stats.view(ranks, 3, C)[:, 0, 0].sum().item()) if ranks > 1 else float(rows)
+    if count <= 1:
+        raise ValueError(f"Expected more than 1 value per channel when training, got {int(count)} (BatchNorm)")
+    track = bn.track_running_stats and bn.running_mean is not None
+    factor = 0.0
+    if track:   # torch's _BatchNorm.forward: count this batch, then the averaging factor
+        bn.num_batches_tracked.add_(1)
+        factor = bn.momentum if bn.momentum is not None else 1.0 / float(bn.num_batches_tracked.item())
+    mean = torch.empty(C, dtype=torch.float32, device=dev)
+    invstd = torch.empty_like(mean)
+    y = torch.empty_like(z)
+    with torch.cuda.device(dev):
+        check(lib.avsr_bn_train_finalize(stats.data_ptr(), ranks, C, float(bn.eps), float(factor),
+                                         _ptr(bn.running_mean if track else None),
+                                         _ptr(bn.running_var if track else None), mean.data_ptr(), invstd.data_ptr(),
+                                         _stream_handle(dev)))
+        check(lib.avsr_bn_train_act_fwd(z.data_ptr(), mean.data_ptr(), invstd.data_ptr(), gamma.data_ptr(),
+                                        beta.data_ptr(), _ptr(resid), int(act), y.data_ptr(), rows, C,
+                                        _stream_handle(dev)))
+    return y, mean, invstd, count
+
+
+def bn_train_backward(z, dy, mean, invstd, gamma, beta, count: float, group, resid=None, act: bool = True,
+                      want_dres: bool = False):
+    """Backward of ``bn_train_forward`` -> (dz, dres | None, dgamma, dbeta).  d gamma / d beta are this rank's sums (DDP
+    averages the parameter gradients); under a ``group`` dz uses the sums all-reduced over the ranks."""
+    rows, C = z.shape
+    dev = z.device
+    sums = torch.empty(2, C, dtype=torch.float32, device=dev)
+    ws = _workspace(dev, int(lib.avsr_bn_train_workspace_bytes(rows, C)))
+    with torch.cuda.device(dev):
+        check(lib.avsr_bn_train_bwd_sums(z.data_ptr(), dy.data_ptr(), mean.data_ptr(), invstd.data_ptr(),
+                                         gamma.data_ptr(), beta.data_ptr(), _ptr(resid), int(act), sums.data_ptr(),
+                                         rows, C, ws.data_ptr(), ws.numel(), _stream_handle(dev)))
+    dbeta, dgamma = sums[0].clone(), sums[1].clone()
+    if group is not None:
+        import torch.distributed as dist
+        dist.all_reduce(sums, group=group)
+    dz = torch.empty_like(z)
+    dres = torch.empty_like(z) if want_dres else None
+    with torch.cuda.device(dev):
+        check(lib.avsr_bn_train_bwd_dx(z.data_ptr(), dy.data_ptr(), mean.data_ptr(), invstd.data_ptr(),
+                                       gamma.data_ptr(), beta.data_ptr(), _ptr(resid), int(act), sums.data_ptr(),
+                                       1.0 / count, dz.data_ptr(), _ptr(dres), rows, C, _stream_handle(dev)))
+    return dz, dres, dgamma, dbeta
+
+
 class DwConvBnSiluFn(torch.autograd.Function):
-    """depthwise Conv1d + BatchNorm1d / SyncBatchNorm (training: batch statistics over all B*T frames -- of ALL ranks of
-    ``group`` when given --, running stats updated in place) + SiLU on (B, T, C) (conformer_encoder.py:33-34).
-
-    The heavy passes (conv, per-channel sums, normalise + SiLU, their backward, tap gradients) run in libavsr_b200; the
-    C-length statistics vectors are finalised here between them, which is where SyncBatchNorm's all-reduce goes
-    (forward: a packed [sum, count] message, then the centred sums; backward: [sum ds, sum ds*x_hat];
-    torch/_functions.py:49-159).
-
-    The batch statistics take two passes over the conv output: ``sum v`` gives a provisional mean m1, then the centred
-    sums S = sum (v - m1) and Q = sum (v - m1)^2 give mean = m1 + S/n and var = Q/n - (S/n)^2.  The one-pass
-    ``sum v^2 / n - mean^2`` cancels in fp32 once a channel's mean is a few times its standard deviation (the conv bias
-    alone can put it there), which the centred sums do not."""
+    """depthwise Conv1d + BatchNorm1d / SyncBatchNorm ``bn`` in training + SiLU on (B, T, C)
+    (conformer_encoder.py:33-34): batch statistics over all B*T frames (of all ranks of ``group`` when given), ``bn``'s
+    running statistics updated in place.  The conv and its tap gradients run in libavsr_b200 around
+    ``bn_train_forward`` / ``bn_train_backward``."""
 
     @staticmethod
-    def forward(ctx, x, w, b, bn_w, bn_b, running_mean, running_var, momentum: float, eps: float, group):
+    def forward(ctx, x, w, b, bn_w, bn_b, bn, group):
         require_cuda(x, "conv module input")
         x, w, b, bn_w, bn_b = _c(x), _c(w), _c(b), _c(bn_w), _c(bn_b)
-        B, T, Cc = x.shape
         conv = _dwconv_raw(x, w, b, False)
-        s1 = _chan_sums(conv)[0]
-        n = float(B * T)
-        if group is not None:
-            packed = torch.cat([s1, torch.full((1,), n, dtype=torch.float32, device=x.device)])
-            torch.distributed.all_reduce(packed, group=group)
-            s1, n = packed[:-1], float(packed[-1].item())                      # global row count (one host sync)
-        m1 = (s1.double() / n).float().contiguous()                            # provisional mean
-        cs = _chan_sums(conv, mean=m1)                                         # [sum (v - m1), sum (v - m1)^2]
-        if group is not None:
-            torch.distributed.all_reduce(cs, group=group)
-        cs64 = cs.double()
-        dm = cs64[0] / n
-        mean = m1.double() + dm
-        var = (cs64[1] / n - dm * dm).clamp_min_(0.0)
-        invstd = torch.rsqrt(var + eps)
-        if running_mean is not None:
-            with torch.no_grad():
-                unbiased = var * (n / max(n - 1.0, 1.0))
-                running_mean.mul_(1.0 - momentum).add_(mean.to(running_mean.dtype), alpha=momentum)
-                running_var.mul_(1.0 - momentum).add_(unbiased.to(running_var.dtype), alpha=momentum)
-        mean, invstd = mean.float().contiguous(), invstd.float().contiguous()
-        y = torch.empty_like(x)
-        with torch.cuda.device(x.device):
-            check(lib.avsr_bn_silu_fwd(conv.data_ptr(), mean.data_ptr(), invstd.data_ptr(), bn_w.data_ptr(), bn_b.data_ptr(),
-                                       y.data_ptr(), B * T, Cc, _stream_handle(x.device)))
+        y, mean, invstd, count = bn_train_forward(conv.view(-1, x.size(-1)), bn_w, bn_b, bn, group)
         ctx.save_for_backward(x, w, conv, mean, invstd, bn_w, bn_b)
-        ctx.group, ctx.inv_count = group, 1.0 / n
-        ctx.mark_non_differentiable(*[t for t in (running_mean, running_var) if t is not None])
-        return y
+        ctx.group, ctx.count = group, count
+        return y.view(x.shape)
 
     @staticmethod
     def backward(ctx, dy):
         x, w, conv, mean, invstd, bn_w, bn_b = ctx.saved_tensors
-        dy = _c(dy)
         B, T, Cc = x.shape
         K = w.size(-1)
-        local = _chan_sums(conv, dy, mean, invstd, bn_w, bn_b)            # [sum ds, sum ds * x_hat] of THIS rank
-        dbt, dg = local[0].clone(), local[1].clone()                       # d beta, d gamma: local sums (DDP averages them)
-        glob = local
-        if ctx.group is not None:
-            glob = local.clone()
-            torch.distributed.all_reduce(glob, group=ctx.group)
-        dconv = torch.empty_like(x)
-        with torch.cuda.device(x.device):
-            check(lib.avsr_bn_silu_bwd_dx(conv.data_ptr(), dy.data_ptr(), mean.data_ptr(), invstd.data_ptr(), bn_w.data_ptr(),
-                                          bn_b.data_ptr(), glob[0].contiguous().data_ptr(), glob[1].contiguous().data_ptr(),
-                                          float(ctx.inv_count), dconv.data_ptr(), B * T, Cc, _stream_handle(x.device)))
+        dconv, _, dg, dbt = bn_train_backward(conv.view(-1, Cc), _c(dy).view(-1, Cc), mean, invstd, bn_w, bn_b,
+                                              ctx.count, ctx.group)
+        dconv = dconv.view(x.shape)
         dx = _dwconv_raw(dconv, w, None, True)                             # correlation with the flipped taps
         dw, db = torch.empty_like(w), torch.empty(Cc, device=x.device)
         ws = _workspace(x.device, int(lib.avsr_train_workspace_bytes(B * T, Cc, K)))
         with torch.cuda.device(x.device):
             check(lib.avsr_dwconv_wgrad(x.data_ptr(), dconv.data_ptr(), dw.data_ptr(), db.data_ptr(), B, T, Cc, K, ws.data_ptr(),
                                         ws.numel(), _stream_handle(x.device)))
-        return dx, dw, db, dg, dbt, None, None, None, None, None
+        return dx, dw, db, dg, dbt, None, None
 
 
 class AttentionCoreFn(torch.autograd.Function):
@@ -432,27 +458,14 @@ def feed_forward_train(m, x, precision: str, backward: Optional[str] = None):
 
 def conv_module_train(m, x, precision: str, backward: Optional[str] = None):
     """ConvolutionModule.forward in train mode on (B, T, C): pointwise_cov1 -> GLU -> depthwise + BatchNorm(batch stats)
-    + SiLU -> pointwise_cov2.  ``m.norm`` stays a real BatchNorm1d: its running statistics and num_batches_tracked are
-    updated like torch's (momentum None = cumulative average is not supported here)."""
+    + SiLU -> pointwise_cov2.  ``m.norm`` stays a real BatchNorm1d / SyncBatchNorm: its running statistics and
+    num_batches_tracked are updated like torch's."""
     bn = m.norm
-    group = None
-    if isinstance(bn, torch.nn.SyncBatchNorm):        # what Lightning's sync_batchnorm=True (train.py:31) turns `norm` into
-        import torch.distributed as dist
-        if dist.is_available() and dist.is_initialized():
-            group = bn.process_group if bn.process_group is not None else dist.group.WORLD
-            if dist.get_world_size(group) == 1:
-                group = None
-    elif type(bn) is not torch.nn.BatchNorm1d:
+    if not isinstance(bn, torch.nn.SyncBatchNorm) and type(bn) is not torch.nn.BatchNorm1d:
         raise NotImplementedError(f"conv_module.norm is {type(bn).__name__}: BatchNorm1d / SyncBatchNorm only")
-    if bn.momentum is None:
-        raise NotImplementedError("BatchNorm1d(momentum=None) (cumulative moving average) is not supported")
     h = LinearFn.apply(x, m.pointwise_cov1.weight, m.pointwise_cov1.bias, False, precision, backward)
     g = GluFn.apply(h)
-    track = bn.track_running_stats and bn.running_mean is not None
-    y = DwConvBnSiluFn.apply(g, m.depthwise_conv.weight, m.depthwise_conv.bias, bn.weight, bn.bias,
-                             bn.running_mean if track else None, bn.running_var if track else None, bn.momentum, bn.eps, group)
-    if track and bn.num_batches_tracked is not None:
-        bn.num_batches_tracked.add_(1)
+    y = DwConvBnSiluFn.apply(g, m.depthwise_conv.weight, m.depthwise_conv.bias, bn.weight, bn.bias, bn, _sync_group(bn))
     return LinearFn.apply(y, m.pointwise_cov2.weight, m.pointwise_cov2.bias, False, precision, backward)
 
 

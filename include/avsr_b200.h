@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define AVSR_ABI_VERSION 10
+#define AVSR_ABI_VERSION 11
 
 enum {
   AVSR_OK = 0,
@@ -270,26 +270,43 @@ int avsr_relu_bwd(const float *y, const float *dy, float *dx, long n, void *stre
 /* F.glu over channels (conformer_encoder.py:32): in (rows, 2C) -> y (rows, C); and its backward din (rows, 2C) */
 int avsr_glu_fwd(const float *in, float *y, long rows, int C, void *stream);
 int avsr_glu_bwd(const float *in, const float *dy, float *din, long rows, int C, void *stream);
-/* depthwise Conv1d(C,C,K,groups=C) -> BatchNorm1d in TRAINING mode -> SiLU (conformer_encoder.py:33-34) in the pieces a
- * (Sync)BatchNorm needs: the per-channel sums leave the library so that the host can all-reduce them over the ranks
- * (train.py:31 sync_batchnorm=True) before it finalises mean / invstd / the running statistics.
+/* depthwise Conv1d(C,C,K,groups=C) of the conformer conv module (conformer_encoder.py:33), its training BatchNorm1d
+ * being the avsr_bn_train_* entries below.
  *   avsr_dwconv_raw      y = conv(x) + b, raw fp32 (flip != 0: taps reversed, b may be NULL = the input gradient)
- *   avsr_chan_sums       sums (2,C): [sum v, sum v^2] (dy, mean NULL), the centred [sum (v-mean), sum (v-mean)^2]
- *                        (dy NULL, mean given) or the backward sums [sum ds, sum ds*x_hat] (dy given)
- *   avsr_bn_silu_fwd     y = silu((v - mean) * invstd * gamma + beta)
- *   avsr_bn_silu_bwd_dx  dv from dy with the GLOBAL sums and 1 / (global row count)
  *   avsr_dwconv_wgrad    dw (C,1,K), db (C) */
 int avsr_dwconv_raw(const float *x, const float *w, const float *b, float *y, int B, int T, int C, int K, int flip,
                     void *workspace, size_t workspace_bytes, void *stream);
-int avsr_chan_sums(const float *v, const float *dy, const float *mean, const float *invstd, const float *gamma,
-                   const float *beta, float *sums, int rows, int C, void *workspace, size_t workspace_bytes, void *stream);
-int avsr_bn_silu_fwd(const float *v, const float *mean, const float *invstd, const float *gamma, const float *beta,
-                     float *y, int rows, int C, void *stream);
-int avsr_bn_silu_bwd_dx(const float *v, const float *dy, const float *mean, const float *invstd, const float *gamma,
-                        const float *beta, const float *sum_ds, const float *sum_dsx, float inv_count, float *dv, int rows,
-                        int C, void *stream);
 int avsr_dwconv_wgrad(const float *x, const float *dconv, float *dw, float *db, int B, int T, int C, int K,
                       void *workspace, size_t workspace_bytes, void *stream);
+
+/* ---- BatchNorm with batch statistics (training), shared by the conformer conv module and the ResNet front-ends, in
+ * the pieces a (Sync)BatchNorm needs: the statistics and the backward sums leave the library between the pieces, so
+ * that the host can gather / all-reduce them over the ranks (train.py:31 sync_batchnorm=True).  z, y, dy, resid, dz,
+ * dres are DEVICE fp32 (rows, C); the workspace is >= avsr_bn_train_workspace_bytes(rows, C).
+ *   avsr_bn_train_stats     stats (3, C) fp64 = each channel's (count, mean, M2) over the rows: per-tile two-pass sums,
+ *                           merged in a fixed order with Chan's formula.  avsr_frontend_train_conv_fwd computes the
+ *                           same for its output.
+ *   avsr_bn_train_finalize  stats (ranks, 3, C), merged in rank order -> mean, invstd = 1 / sqrt(biased var + eps) (C
+ *                           fp32).  When running_mean / running_var are given they become (1 - factor) * old + factor *
+ *                           (mean, unbiased var).
+ *   avsr_bn_train_act_fwd   y = [SiLU]((z - mean) * invstd * gamma + beta [+ resid]); resid may be NULL
+ *   avsr_bn_train_bwd_sums  sums (2, C) = [sum ds, sum ds * x_hat] with ds = dL/d(BatchNorm output) (dy through the
+ *                           SiLU when act), summed in a fixed order
+ *   avsr_bn_train_bwd_dx    dz = gamma * invstd * (ds - inv_count * (sums[0] + x_hat * sums[1])) and, when dres is
+ *                           given, dres = ds (the residual's gradient); sums and inv_count over all ranks */
+size_t avsr_bn_train_workspace_bytes(long rows, int C);
+int avsr_bn_train_stats(const float *z, long rows, int C, double *stats, void *workspace, size_t workspace_bytes,
+                        void *stream);
+int avsr_bn_train_finalize(const double *stats, int ranks, int C, double eps, double factor, float *running_mean,
+                           float *running_var, float *mean, float *invstd, void *stream);
+int avsr_bn_train_act_fwd(const float *z, const float *mean, const float *invstd, const float *gamma, const float *beta,
+                          const float *resid, int act, float *y, long rows, int C, void *stream);
+int avsr_bn_train_bwd_sums(const float *z, const float *dy, const float *mean, const float *invstd, const float *gamma,
+                           const float *beta, const float *resid, int act, float *sums, long rows, int C,
+                           void *workspace, size_t workspace_bytes, void *stream);
+int avsr_bn_train_bwd_dx(const float *z, const float *dy, const float *mean, const float *invstd, const float *gamma,
+                         const float *beta, const float *resid, int act, const float *sums, float inv_count, float *dz,
+                         float *dres, long rows, int C, void *stream);
 
 /* Backward of the rel-pos attention core (avsr_relpos_attention; transformer/attention.py:174-189 + :59-82), fp32:
  * from q, k, v (B,T,H*64: the projected tensors, biases included), p (2T-1, H*64), pos_bias_u / v (H,64), lengths, the
@@ -541,30 +558,12 @@ int avsr_conv_bn_act(const float *x, const float *w, const float *scale, const f
  *
  * avsr_frontend_train_conv_fwd: z (output pixels, C_out) = conv(x, w) in `precision` (TF32 / F16 / BF16 on wgmma, FP32 on
  * CUDA cores), and stats (3, C_out) fp64 = each channel's (count, mean, M2) over all output pixels, merged in a fixed order
- * with Chan's formula. */
+ * with Chan's formula (the avsr_bn_train_stats of z).  BatchNorm then runs on the avsr_bn_train_* entries. */
 size_t avsr_frontend_train_conv_workspace_bytes(int stem, int N, int T, int H, int W, int C_in, int C_out, int KH,
                                                 int KW, int stride, int precision);
 int avsr_frontend_train_conv_fwd(const float *x, const float *w, float *z, double *stats, int stem, int N, int T, int H,
                                  int W, int C_in, int C_out, int KH, int KW, int stride, void *workspace,
                                  size_t workspace_bytes, int precision, void *stream);
-/* stats: (ranks, 3, C) fp64, merged in rank order -> mean, invstd = 1 / sqrt(biased var + eps) (C fp32).  When
- * running_mean / running_var are given they become (1 - factor) * old + factor * (mean, unbiased var). */
-int avsr_frontend_train_bn_finalize(const double *stats, int ranks, int C, double eps, double factor,
-                                    float *running_mean, float *running_var, float *mean, float *invstd, void *stream);
-/* y = [SiLU]((z - mean) * invstd * gamma + beta [+ resid]), (rows, C); resid may be NULL */
-int avsr_frontend_train_bn_act_fwd(const float *z, const float *mean, const float *invstd, const float *gamma,
-                                   const float *beta, const float *resid, int act, float *y, long rows, int C,
-                                   void *stream);
-/* Backward of bn_act_fwd.  bwd_sums: sums (2, C) = [sum ds, sum ds * x_hat] with ds = dL/d(BatchNorm output) (dy through
- * the SiLU when act), summed in a fixed order.  bwd_dx: dz = gamma * invstd * (ds - inv_count * (sums[0] + x_hat *
- * sums[1])) and, when dres is given, dres = ds (the residual's gradient). */
-size_t avsr_frontend_train_bn_bwd_workspace_bytes(long rows, int C);
-int avsr_frontend_train_bn_bwd_sums(const float *z, const float *dy, const float *mean, const float *invstd,
-                                    const float *gamma, const float *beta, const float *resid, int act, float *sums,
-                                    long rows, int C, void *workspace, size_t workspace_bytes, void *stream);
-int avsr_frontend_train_bn_bwd_dx(const float *z, const float *dy, const float *mean, const float *invstd,
-                                  const float *gamma, const float *beta, const float *resid, int act, const float *sums,
-                                  float inv_count, float *dz, float *dres, long rows, int C, void *stream);
 /* Input gradient of a trunk conv: dx (N, H, W, C_in) from dz (N, Ho, Wo, C_out), one stride-1 implicit GEMM per parity
  * class of the input (TF32 / F16 / BF16 on wgmma, FP32 on CUDA cores). */
 size_t avsr_frontend_train_dgrad_workspace_bytes(int N, int H, int W, int C_in, int C_out, int KH, int KW, int stride,

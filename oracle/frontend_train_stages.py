@@ -22,7 +22,17 @@ Tensor = torch.Tensor
 
 WG_T = 64            # wgrad tile: 64 C_out x 64 k columns
 WGT_PB = 32          # pixels per wgrad K-block: a split is a multiple of it
-FT_ROWS = 256        # rows per BatchNorm statistics tile
+FT_ROWS = 256        # rows per BatchNorm statistics tile, at most (stats_tile_rows)
+
+
+def stats_tile_rows(rows: int, C: int) -> int:
+    """Rows per BatchNorm statistics tile (csrc/train.cu bn_tile_rows): FT_ROWS, halved down to 32 while the grid of
+    tiles x ceil(C / 128) CTAs would hold fewer than two per SM of 132."""
+    h = FT_ROWS
+    while h > 32 and -(-rows // h) * -(-C // 128) < 2 * 132:
+        h //= 2
+    return h
+
 
 DEFECTS: Dict[str, str] = {
     "wgrad_drop_split": "dW without the partial of one full-size pixel split (a slipped split offset)",
@@ -113,8 +123,8 @@ CASES = [
     ("t2_32", "video", 4, 2, 32, 32, None, ("fp32", "tf32", "f16")),
     # 57 frames: layer 2's 513 rows leave 1 row in the last statistics tile
     ("t3_24", "video", 19, 3, 24, 24, None, ("fp32", "tf32", "f16")),
-    # 89x89: stride-2 dgrad on odd H and W (layer 2's 23x23 input); 15 frames leave 255 rows in layer 1's last
-    # statistics tile; the second utterance's last two frames are zero padding
+    # 89x89: stride-2 dgrad on odd H and W (layer 2's 23x23 input); 15 frames leave layer 1's last statistics tile one
+    # row short; the second utterance's last two frames are zero padding
     ("t5_89", "video", 3, 5, 89, 89, 3, ("fp32", "tf32", "f16")),
     # non-square; layer 4's BatchNorm sees 32 positions per channel
     ("t4_45x61", "video", 2, 4, 45, 61, None, ("fp32", "tf32", "f16")),

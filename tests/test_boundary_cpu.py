@@ -35,7 +35,7 @@ def test_library_exports_every_declared_symbol(built):
     assert set(syms) <= exported, sorted(set(syms) - exported)
     from auto_avsr_b200 import _cabi
     assert set(_cabi.SIGNATURES) == set(syms)
-    assert _cabi.lib.avsr_abi_version() == _cabi.ABI_VERSION == 10
+    assert _cabi.lib.avsr_abi_version() == _cabi.ABI_VERSION == 11
     assert _cabi.launch_count() == 0
 
 

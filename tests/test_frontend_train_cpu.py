@@ -80,8 +80,8 @@ out["dgrad_ws"] = lib.avsr_frontend_train_dgrad_workspace_bytes(4, 22, 22, 64, 1
 out["dgrad_ws_bad"] = lib.avsr_frontend_train_dgrad_workspace_bytes(4, 22, 22, 64, 100, 3, 3, 2, 1)
 out["wgrad_ws"] = lib.avsr_frontend_train_wgrad_workspace_bytes(0, 4, 1, 22, 22, 64, 128, 1, 1, 2)
 out["wgrad_ws_bad"] = lib.avsr_frontend_train_wgrad_workspace_bytes(0, -1, 1, 22, 22, 64, 128, 1, 1, 2)
-out["bn_ws"] = lib.avsr_frontend_train_bn_bwd_workspace_bytes(1000, 64)
-out["bn_ws_bad"] = lib.avsr_frontend_train_bn_bwd_workspace_bytes(1000, 0)
+out["bn_ws"] = lib.avsr_bn_train_workspace_bytes(1000, 64)
+out["bn_ws_bad"] = lib.avsr_bn_train_workspace_bytes(1000, 0)
 P = 1 << 20          # a non-NULL pointer value: every call below is refused before it could be dereferenced
 need = out["conv_ws_trunk"]
 out["rc_conv_null"] = lib.avsr_frontend_train_conv_fwd(None, P, P, P, 0, 4, 1, 22, 22, 64, 64, 3, 3, 1, P, need, 2, None)
@@ -90,11 +90,11 @@ out["rc_conv_shape"] = lib.avsr_frontend_train_conv_fwd(P, P, P, P, 0, 4, 1, 22,
 out["rc_dgrad_small"] = lib.avsr_frontend_train_conv_dgrad(P, P, P, 4, 22, 22, 64, 128, 3, 3, 2, P, out["dgrad_ws"] - 1, 1, None)
 out["rc_wgrad_null"] = lib.avsr_frontend_train_conv_wgrad(P, None, P, 0, 4, 1, 22, 22, 64, 128, 1, 1, 2, P, out["wgrad_ws"], 1, None)
 out["rc_wgrad_prec"] = lib.avsr_frontend_train_conv_wgrad(P, P, P, 0, 4, 1, 22, 22, 64, 128, 1, 1, 2, P, out["wgrad_ws"], 7, None)
-out["rc_bn_sums_small"] = lib.avsr_frontend_train_bn_bwd_sums(P, P, P, P, P, P, None, 1, P, 1000, 64, P, out["bn_ws"] - 1, None)
-out["rc_finalize_bad"] = lib.avsr_frontend_train_bn_finalize(P, 0, 64, 1e-5, 0.1, None, None, P, P, None)
-out["rc_finalize_half"] = lib.avsr_frontend_train_bn_finalize(P, 1, 64, 1e-5, 0.1, P, None, P, P, None)
-out["rc_bn_fwd_null"] = lib.avsr_frontend_train_bn_act_fwd(P, P, P, P, None, None, 1, P, 10, 64, None)
-out["rc_bn_dx_null"] = lib.avsr_frontend_train_bn_bwd_dx(P, P, P, P, P, P, None, 1, None, 0.1, P, None, 10, 64, None)
+out["rc_bn_sums_small"] = lib.avsr_bn_train_bwd_sums(P, P, P, P, P, P, None, 1, P, 1000, 64, P, out["bn_ws"] - 1, None)
+out["rc_finalize_bad"] = lib.avsr_bn_train_finalize(P, 0, 64, 1e-5, 0.1, None, None, P, P, None)
+out["rc_finalize_half"] = lib.avsr_bn_train_finalize(P, 1, 64, 1e-5, 0.1, P, None, P, P, None)
+out["rc_bn_fwd_null"] = lib.avsr_bn_train_act_fwd(P, P, P, P, None, None, 1, P, 10, 64, None)
+out["rc_bn_dx_null"] = lib.avsr_bn_train_bwd_dx(P, P, P, P, P, P, None, 1, None, 0.1, P, None, 10, 64, None)
 out["rc_pool_null"] = lib.avsr_frontend_train_maxpool_fwd(P, P, None, 1, 4, 4, 64, None)
 out["rc_pool_bwd_shape"] = lib.avsr_frontend_train_maxpool_bwd(P, P, P, 1, 0, 4, 64, None)
 out["rc_mean_null"] = lib.avsr_frontend_train_mean_rows(None, P, 2, 20, 512, None)

@@ -3,7 +3,8 @@ kernels it is there for, and the float64 unit oracle (oracle/frontend_train_stag
 its defects changes it, and its winner-pinned max-pool is torch's max-pool when the winners agree.
 
 The wgrad split counts come from the library itself: ``avsr_frontend_train_wgrad_workspace_bytes`` is
-splits * C_out * Kw * 4 bytes + 256 (Kw = K rounded up to 64), so a change of the split rule shows up here."""
+splits * C_out * Kw * 4 bytes + 256 (Kw = K rounded up to 64), so a change of the split rule shows up here; so do the
+BatchNorm statistics tiles (``avsr_bn_train_workspace_bytes``) against the oracle's tile rule."""
 import pytest
 import torch
 
@@ -16,6 +17,12 @@ def _splits(g):
     b = lib.avsr_frontend_train_wgrad_workspace_bytes(*g.args())
     assert b > 256 and (b - 256) % (g.Cout * Kw * 4) == 0, (g.name, b)
     return (b - 256) // (g.Cout * Kw * 4)
+
+
+def _stats_tiles(g):
+    """avsr_bn_train_workspace_bytes is tiles * 3 * C * 8 bytes + 256 (exact for C a multiple of 64)"""
+    from auto_avsr_b200._cabi import lib
+    return (lib.avsr_bn_train_workspace_bytes(g.rows, g.Cout) - 256) // (3 * g.Cout * 8)
 
 
 def _all_units(prec=None):
@@ -49,14 +56,16 @@ def test_case_list_reaches_every_edge():
                 seen.add("downsample_zero_classes")
         if g.stem == 0 and g.dims == 1 and g.stride == 2:
             seen.add("audio_h1_dgrad")
-        if g.rows % S.FT_ROWS in (1, 255):
-            seen.add(("stats_tail", g.rows % S.FT_ROWS))
+        tile = S.stats_tile_rows(g.rows, g.Cout)
+        assert _stats_tiles(g) == -(-g.rows // tile), (g.name, g.rows, g.Cout)
+        if g.rows % tile in (1, tile - 1):
+            seen.add(("stats_tail", "1 row" if g.rows % tile == 1 else "1 row short"))
         if g.name.startswith("layer4") and g.rows <= 32 and case[1] == "video":
             seen.add("layer4_bn_le_32")
     want = {("tc_multi_split", c) for c in (64, 128, 256, 512)} | {
         "empty_trailing_split", "split_mid_frame", "stem_split_mid_utterance", ("k_not_multiple_of_64", 1),
         ("k_not_multiple_of_64", 2), ("dgrad_s2", 0, 0), ("dgrad_s2", 1, 1), "downsample_zero_classes",
-        "audio_h1_dgrad", ("stats_tail", 1), ("stats_tail", 255), "layer4_bn_le_32"}
+        "audio_h1_dgrad", ("stats_tail", "1 row"), ("stats_tail", "1 row short"), "layer4_bn_le_32"}
     assert want <= seen, sorted(map(str, want - seen))
 
 

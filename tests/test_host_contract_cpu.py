@@ -241,7 +241,9 @@ def _probe(lib, decoder_only):
     code("too small", "avsr_layernorm_bwd", p, p, p, p, p, p, 18, 64, p, 2 * 64 * 4 - 1, None)
     code("too small", "avsr_colsum", p, p, 18, 64, p, 64 * 4 - 1, None)
     code("too small", "avsr_dwconv_raw", p, p, p, p, 2, 9, 64, 15, 0, p, 17 * 64 * 4 - 1, None)
-    code("too small", "avsr_chan_sums", p, None, None, None, None, None, p, 18, 64, p, 2 * 64 * 4 - 1, None)
+    bnw = _c("avsr_bn_train_workspace_bytes", 18, 64)
+    code("NULL input", "avsr_bn_train_stats", None, 18, 64, p, p, bnw, None)
+    code("too small", "avsr_bn_train_stats", p, 18, 64, p, p, bnw - 1, None)
     code("too small", "avsr_dwconv_wgrad", p, p, p, p, 2, 9, 64, 15, p, 63, None)
     st = _c("avsr_ctc_loss_state_bytes", 2, 9, 3)
     code("too small", "avsr_ctc_loss_fwd", p, 41, p, p, 2, 9, 3, 41, -1, 1, p, p, st - 1, None)

@@ -184,20 +184,29 @@ def dwconv_case(dev, B, T, K, C, ratio, seed):
     return x, w, b, bn_w, bn_b, rm, rv, r
 
 
-def run_dwconv(x, w, b, bn_w, bn_b, rm, rv, r):
+# batches the running statistics have seen before the one under test: momentum=None averages with 1 / (this + 1)
+DW_TRACKED = 3
+
+
+def run_dwconv(x, w, b, bn_w, bn_b, rm, rv, r, momentum):
     from auto_avsr_b200.train import DwConvBnSiluFn
     leaves = [t.clone().requires_grad_(True) for t in (x, w, b, bn_w, bn_b)]
-    rm_, rv_ = rm.clone(), rv.clone()
-    y = DwConvBnSiluFn.apply(*leaves, rm_, rv_, 0.1, 1e-5, None)
+    bn = torch.nn.BatchNorm1d(x.size(-1), momentum=momentum, eps=1e-5, device=x.device).train()
+    bn.running_mean.copy_(rm)
+    bn.running_var.copy_(rv)
+    bn.num_batches_tracked.fill_(DW_TRACKED)
+    y = DwConvBnSiluFn.apply(*leaves, bn, None)
     (y * r).sum().backward()
-    return [y.detach()] + [t.grad for t in leaves] + [rm_, rv_]
+    assert int(bn.num_batches_tracked) == DW_TRACKED + 1
+    return [y.detach()] + [t.grad for t in leaves] + [bn.running_mean, bn.running_var]
 
 
-def ref_dwconv(x, w, b, bn_w, bn_b, rm, rv, r, frozen=False):
+def ref_dwconv(x, w, b, bn_w, bn_b, rm, rv, r, momentum, frozen=False):
     """float64 conv1d(groups=C) + F.batch_norm(training) + silu -> [y, dx, dw, db, dgamma, dbeta, running_mean,
-    running_var], rho.  frozen: the batch statistics enter as constants (no gradient through them) -- the scale of the
-    gradients that batch statistics cancel.  rho = max over channels of max |conv| / sqrt(var + eps): what one fp32
-    rounding of the conv output moves x_hat by, in units of 2^-24."""
+    running_var], rho.  momentum None: the cumulative average, factor 1 / num_batches_tracked.  frozen: the batch
+    statistics enter as constants (no gradient through them) -- the scale of the gradients that batch statistics
+    cancel.  rho = max over channels of max |conv| / sqrt(var + eps): what one fp32 rounding of the conv output moves
+    x_hat by, in units of 2^-24."""
     K, C = w.size(-1), w.size(0)
     leaves = [t.double().requires_grad_(True) for t in (x, w, b, bn_w, bn_b)]
     rm_, rv_ = rm.double(), rv.double()
@@ -207,7 +216,8 @@ def ref_dwconv(x, w, b, bn_w, bn_b, rm, rv, r, frozen=False):
     if frozen:
         h = F.batch_norm(conv, mu, var, leaves[3], leaves[4], training=False, eps=1e-5)
     else:
-        h = F.batch_norm(conv, rm_, rv_, leaves[3], leaves[4], training=True, momentum=0.1, eps=1e-5)
+        factor = momentum if momentum is not None else 1.0 / (DW_TRACKED + 1)
+        h = F.batch_norm(conv, rm_, rv_, leaves[3], leaves[4], training=True, momentum=factor, eps=1e-5)
     y = F.silu(h).transpose(1, 2)
     (y * r.double()).sum().backward()
     rho = (cd.abs().amax((0, 2)) / (var + 1e-5).sqrt()).max().item()
@@ -218,17 +228,17 @@ DW_NAMES = ["y", "dx", "dw", "db", "dgamma", "dbeta", "running_mean", "running_v
 DW_SHAPES = [(1, 2), (2, 1), (1, 5), (3, 37), (4, 400), (16, 100), (1, 1600), (200, 8)]
 
 
-def check_dwconv(dev, B, T, K, C, ratio, seed):
+def check_dwconv(dev, B, T, K, C, ratio, seed, momentum=0.1):
     args = dwconv_case(dev, B, T, K, C, ratio, seed)
-    a, b = run_dwconv(*args), run_dwconv(*args)
+    a, b = run_dwconv(*args, momentum), run_dwconv(*args, momentum)
     same_bits(a, b, "DwConvBnSiluFn")
-    ref, rho = ref_dwconv(*args)
+    ref, rho = ref_dwconv(*args, momentum)
     # Gradients the batch statistics cancel are 0 in exact arithmetic (up to eps): the conv bias gradient (the batch
     # mean removes the bias), the tap gradient at K = 1 (BatchNorm removes the tap's scale), every conv gradient of a
     # 2-frame batch (x_hat = +-1 whatever the values).  Those are measured against the gradient with the statistics held
     # constant instead of against their own rounding noise.
     zero = {"db"} | ({"dw"} if K == 1 else set()) | ({"dx", "dw"} if B * T == 2 else set())
-    frozen = ref_dwconv(*args, frozen=True)[0] if zero else None
+    frozen = ref_dwconv(*args, momentum, frozen=True)[0] if zero else None
     errs = {}
     for i, (n, got, want) in enumerate(zip(DW_NAMES, a, ref)):
         if n in zero:
@@ -238,26 +248,31 @@ def check_dwconv(dev, B, T, K, C, ratio, seed):
     # Storing the conv output in fp32 alone moves x_hat by rho * 2^-24 against the fp64 reference.  Up to rho = 100
     # (offsets of 30 standard deviations included) that is inside the base bound; beyond it the bound grows by it.
     bound = DW_TOL + (4 * rho * 2.0 ** -24 if rho > 100 else 0.0)
-    record("train_kernels_dwconv_bn_silu", (B, T, K, C, f"ratio {ratio}", "rho"), rho, 100)
-    check("train_kernels_dwconv_bn_silu", (B, T, K, C, f"ratio {ratio}"), errs, bound)
+    case = (B, T, K, C, f"ratio {ratio}") + (() if momentum == 0.1 else (f"momentum {momentum}",))
+    record("train_kernels_dwconv_bn_silu", (*case, "rho"), rho, 100)
+    check("train_kernels_dwconv_bn_silu", case, errs, bound)
 
 
-@pytest.mark.parametrize("C", [64, 768])
+@pytest.mark.parametrize("C,momentum", [(64, 0.1), (768, 0.1), (64, None), (768, None)],
+                         ids=["64", "768", "64-None", "768-None"])
 @pytest.mark.parametrize("K", [1, 7, 31])
 @pytest.mark.parametrize("B,T", DW_SHAPES)
-def test_dwconv_bn_silu_vs_fp64(dev, B, T, K, C):
-    """conv1d(groups=C) + batch-stat BatchNorm (momentum 0.1, eps 1e-5, running statistics) + SiLU, forward and
-    backward.  (200, 8) has more utterances than CTAs (one CTA per utterance in the tap gradient); (4, 400), (16, 100)
-    and (1, 1600) give segments of several frames whose 31-tap halo crosses segment boundaries."""
-    check_dwconv(dev, B, T, K, C, 0, B * 1000 + T * 10 + K + C)
+def test_dwconv_bn_silu_vs_fp64(dev, B, T, K, C, momentum):
+    """conv1d(groups=C) + batch-stat BatchNorm (momentum 0.1 or None = the cumulative average, eps 1e-5, running
+    statistics) + SiLU, forward and backward.  (200, 8) has more utterances than CTAs (one CTA per utterance in the
+    tap gradient); (4, 400), (16, 100) and (1, 1600) give segments of several frames whose 31-tap halo crosses segment
+    boundaries."""
+    check_dwconv(dev, B, T, K, C, 0, B * 1000 + T * 10 + K + C, momentum)
 
 
-@pytest.mark.parametrize("ratio", [3, 10, 30, 1000])
+@pytest.mark.parametrize("ratio,momentum", [(r, m) for m in (0.1, None) for r in (3, 10, 30, 1000)],
+                         ids=[f"{r}{m}" for m in ("", "-None") for r in (3, 10, 30, 1000)])
 @pytest.mark.parametrize("B,T", [(3, 37), (4, 400), (1, 1600), (200, 8)])
-def test_dwconv_bn_silu_batch_stats_with_channel_offsets(dev, B, T, ratio):
+def test_dwconv_bn_silu_batch_stats_with_channel_offsets(dev, B, T, ratio, momentum):
     """Per-channel means of ratio x the standard deviation (set through the depthwise bias): the batch variance must
-    not cancel.  A one-pass sum(v^2)/n - mean^2 in fp32 loses ratio^2 x 2^-24 of it."""
-    check_dwconv(dev, B, T, 31, 768, ratio, 7 * B + T + ratio)
+    not cancel.  A one-pass sum(v^2)/n - mean^2 in fp32 loses ratio^2 x 2^-24 of it.  A tile mean summed from the raw
+    values loses several times the rounding of the values once the mean is tens of standard deviations off."""
+    check_dwconv(dev, B, T, 31, 768, ratio, 7 * B + T + ratio, momentum)
 
 
 # ------------------------------------------------------------------------------------------------ rel-pos attention backward
