@@ -13,7 +13,7 @@ LIB_PATH = os.environ.get("AVSR_B200_LIB") or os.path.join(_HERE, "csrc", "libav
 
 OK, E_INVALID, E_CUDA, E_WORKSPACE = 0, 1, 2, 3
 PREC_FP32, PREC_TF32, PREC_F16, PREC_BF16 = 0, 1, 2, 16
-ABI_VERSION = 11
+ABI_VERSION = 12
 
 
 class AvsrError(RuntimeError):
@@ -126,11 +126,10 @@ SIGNATURES = {
     "avsr_train_workspace_bytes": (_Z, [_I, _I, _I]),
     "avsr_layernorm_bwd": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _P, _Z, _P]),
     "avsr_colsum": (_I, [_P, _P, _I, _I, _P, _Z, _P]),
-    "avsr_transpose": (_I, [_P, _P, _I, _I, C.c_long, _P]),
     "avsr_relu_bwd": (_I, [_P, _P, _P, C.c_long, _P]),
     "avsr_pack_operand": (_I, [_P, _P, _I, _I, C.c_long, _I, _I, _P]),
-    "avsr_linear_bwd_bf16_workspace_bytes": (_Z, [_I, _I, _I]),
-    "avsr_linear_bwd_bf16": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _Z, _P]),
+    "avsr_linear_bwd_workspace_bytes": (_Z, [_I, _I, _I, _I]),
+    "avsr_linear_bwd": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _Z, _P]),
     "avsr_glu_fwd": (_I, [_P, _P, C.c_long, _I, _P]),
     "avsr_glu_bwd": (_I, [_P, _P, _P, C.c_long, _I, _P]),
     "avsr_dwconv_raw": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _Z, _P]),

@@ -1,6 +1,6 @@
 // Training slice of the encoder path (SURVEY.md 8f #2, first slice): backward of the HBM-bound kernels and the pieces a
 // Linear's backward needs around the tensor-core GEMMs -- LayerNorm backward, bias gradients (column sums), fp32
-// transpose (so that dgrad / wgrad are the SAME wgmma GEMMs on transposed operands), ReLU backward, the depthwise
+// operand packing (so that dgrad / wgrad are the SAME wgmma GEMMs on transposed operands), ReLU backward, the depthwise
 // conv's forward / backward, and the batch-statistics BatchNorm [+ SiLU] of the conformer conv module and the front-end
 // convolutions, forward / backward incl. the running-statistics update.
 // Reference: lightning.py:86-94 (training_step), conformer_encoder.py:26,30-35 (BatchNorm1d in train mode sees ALL B*T
@@ -113,26 +113,12 @@ __global__ void __launch_bounds__(256) colsum_partial_kernel(const float* __rest
   }
 }
 
-// ------------------------------------------------------------------ fp32 transpose (rows x cols) -> (cols x rows)
-__global__ void transpose_kernel(const float* __restrict__ src, float* __restrict__ dst, int rows, int cols, long ld_dst) {
-  __shared__ float tile[32][33];
-  const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
-  for (int j = threadIdx.y; j < 32; j += 8) {
-    const int r = r0 + j, c = c0 + threadIdx.x;
-    tile[j][threadIdx.x] = (r < rows && c < cols) ? src[(long)r * cols + c] : 0.f;
-  }
-  __syncthreads();
-  for (int j = threadIdx.y; j < 32; j += 8) {
-    const int c = c0 + j, r = r0 + threadIdx.x;
-    if (c < cols && r < rows) dst[(long)c * ld_dst + r] = tile[threadIdx.x][j];
-  }
-}
-
-// ------------------------------------------------------------------ fp32 -> bf16 GEMM operands with zero padding
+// ------------------------------------------------------------------ fp32 -> GEMM operands of kind KIND, zero padding
+// (OP_F32 or OP_BF16; a compile-time kind: the runtime-kind branch per store measured 2-3 % slower)
 // transposed: (rows x cols) -> (cols x ld_dst), dst[c][r]; tiles of 32 x 32 through shared memory, the padding columns
 // [rows, ld_dst) written as zeros
-__global__ void pack_bf16_t_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, int rows, int cols,
-                                   long ld_dst) {
+template <int KIND>
+__global__ void pack_t_kernel(const float* __restrict__ src, void* __restrict__ dst, int rows, int cols, long ld_dst) {
   __shared__ float tile[32][33];
   const int c0 = blockIdx.y * 32, r0 = blockIdx.x * 32;
   for (int j = threadIdx.y; j < 32; j += 8) {
@@ -142,17 +128,17 @@ __global__ void pack_bf16_t_kernel(const float* __restrict__ src, __nv_bfloat16*
   __syncthreads();
   for (int j = threadIdx.y; j < 32; j += 8) {
     const int c = c0 + j, r = r0 + threadIdx.x;
-    if (c < cols && r < ld_dst) dst[(long)c * ld_dst + r] = __float2bfloat16_rn(tile[threadIdx.x][j]);
+    if (c < cols && r < ld_dst) store_kind1(dst, (long)c * ld_dst + r, KIND, tile[threadIdx.x][j]);
   }
 }
 // not transposed: (rows x cols) -> (rows x ld_dst), the padding columns [cols, ld_dst) written as zeros
-__global__ void pack_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, int rows, int cols,
-                                 long ld_dst) {
+template <int KIND>
+__global__ void pack_kernel(const float* __restrict__ src, void* __restrict__ dst, int rows, int cols, long ld_dst) {
   const long total = (long)rows * ld_dst;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const long r = i / ld_dst;
     const int c = (int)(i - r * ld_dst);
-    dst[i] = __float2bfloat16_rn(c < cols ? src[r * cols + c] : 0.f);
+    store_kind1(dst, i, KIND, c < cols ? src[r * cols + c] : 0.f);
   }
 }
 
@@ -468,58 +454,82 @@ int avsr_colsum(const float* y, float* out, int rows, int cols, void* workspace,
   return AVSR_OK;
 }
 
-int avsr_transpose(const float* src, float* dst, int rows, int cols, long ld_dst, void* stream) {
-  AVSR_REQUIRE(src && dst && ld_dst >= rows, "transpose: NULL argument or ld_dst < rows");
-  if (rows <= 0 || cols <= 0) return AVSR_OK;
-  transpose_kernel<<<dim3(cdiv(cols, 32), cdiv(rows, 32)), dim3(32, 8), 0, reinterpret_cast<cudaStream_t>(stream)>>>(src, dst, rows, cols, ld_dst);
-  AVSR_CHECK_LAUNCH();
-  return AVSR_OK;
-}
-
 int avsr_pack_operand(const float* src, void* dst, int rows, int cols, long ld_dst, int transpose, int precision,
                       void* stream) {
   AVSR_REQUIRE(src && dst, "NULL argument");
-  AVSR_REQUIRE(precision == AVSR_PREC_BF16, "pack_operand: precision %d is not built; AVSR_PREC_BF16 only", precision);
+  AVSR_REQUIRE(precision == AVSR_PREC_FP32 || precision == AVSR_PREC_BF16,
+               "pack_operand: precision %d is not built; AVSR_PREC_FP32 or AVSR_PREC_BF16", precision);
   AVSR_REQUIRE(rows >= 0 && cols >= 0 && ld_dst >= (transpose ? rows : cols), "pack_operand: bad rows=%d cols=%d ld=%ld",
                rows, cols, ld_dst);
   if (rows <= 0 || cols <= 0) return AVSR_OK;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(dst);
-  if (transpose)
-    pack_bf16_t_kernel<<<dim3((unsigned)((ld_dst + 31) / 32), cdiv(cols, 32)), dim3(32, 8), 0, st>>>(src, d, rows, cols,
-                                                                                                        ld_dst);
-  else
-    pack_bf16_kernel<<<132 * 4, 256, 0, st>>>(src, d, rows, cols, ld_dst);
+  const bool bf16 = precision == AVSR_PREC_BF16;
+  if (transpose) {
+    auto* k = bf16 ? pack_t_kernel<OP_BF16> : pack_t_kernel<OP_F32>;
+    k<<<dim3((unsigned)((ld_dst + 31) / 32), cdiv(cols, 32)), dim3(32, 8), 0, st>>>(src, dst, rows, cols, ld_dst);
+  } else {
+    auto* k = bf16 ? pack_kernel<OP_BF16> : pack_kernel<OP_F32>;
+    k<<<132 * 4, 256, 0, st>>>(src, dst, rows, cols, ld_dst);
+  }
   AVSR_CHECK_LAUNCH();
   return AVSR_OK;
 }
 
-static size_t pad64(int v) { return ((size_t)v + 63) / 64 * 64; }
+// The operands of a Linear's backward GEMMs in the workspace: K padded to 128 bytes (gemm_tc takes K in 128-byte
+// blocks), 32 fp32 elements or 64 bf16 ones.  TF32 operands are packed as plain fp32, unrounded: the tensor core
+// truncates them, as it does the forward's.  dY is read in place for dX when its rows already have that layout (fp32 /
+// TF32 with n a multiple of 32), so no copy of it is made.
+struct LinearBwdOperands {
+  int pack_prec;          // the avsr_pack_operand precision of every operand
+  long np, rp;            // n and rows padded: K of dX and of dW
+  bool dy_in_place;
+  void *dy, *wt, *dyt, *xt;
+  LinearBwdOperands(Carver& cv, int rows, int n, int k, int precision) {
+    pack_prec = precision == AVSR_PREC_BF16 ? AVSR_PREC_BF16 : AVSR_PREC_FP32;
+    const size_t es = operand_bytes(operand_kind(pack_prec));
+    const long e = (long)(128 / es);
+    np = (n + e - 1) / e * e;
+    rp = (rows + e - 1) / e * e;
+    dy_in_place = np == n && pack_prec == AVSR_PREC_FP32;
+    dy = dy_in_place ? nullptr : cv.take<char>((size_t)rows * np * es);
+    wt = cv.take<char>((size_t)k * np * es);
+    dyt = cv.take<char>((size_t)n * rp * es);
+    xt = cv.take<char>((size_t)k * rp * es);
+  }
+};
 
-size_t avsr_linear_bwd_bf16_workspace_bytes(int rows, int n, int k) {
-  if (rows <= 0 || n <= 0 || k <= 0) return 256;
-  return align_up((size_t)rows * pad64(n) * 2, 256) + align_up((size_t)k * pad64(n) * 2, 256) +
-         align_up((size_t)n * pad64(rows) * 2, 256) + align_up((size_t)k * pad64(rows) * 2, 256);
+static bool linear_bwd_precision(int precision) {
+  return precision == AVSR_PREC_FP32 || precision == AVSR_PREC_TF32 || precision == AVSR_PREC_BF16;
 }
 
-int avsr_linear_bwd_bf16(const float* dy, const float* x, const float* w, float* dx, float* dw, int rows, int n, int k,
-                         void* workspace, size_t workspace_bytes, void* stream) {
+size_t avsr_linear_bwd_workspace_bytes(int rows, int n, int k, int precision) {
+  if (!linear_bwd_precision(precision)) return 0;
+  if (rows <= 0 || n <= 0 || k <= 0) return 256;
+  Carver cv{nullptr};
+  const LinearBwdOperands layout(cv, rows, n, k, precision);
+  return cv.off;
+}
+
+int avsr_linear_bwd(const float* dy, const float* x, const float* w, float* dx, float* dw, int rows, int n, int k,
+                    int precision, void* workspace, size_t workspace_bytes, void* stream) {
+  AVSR_REQUIRE(linear_bwd_precision(precision),
+               "linear_bwd: precision %d: AVSR_PREC_FP32, AVSR_PREC_TF32 or AVSR_PREC_BF16 (gradients overflow f16)",
+               precision);
   AVSR_REQUIRE(dy && workspace && (dx || dw) && (!dx || w) && (!dw || x), "NULL argument");
-  AVSR_REQUIRE(rows > 0 && n > 0 && k > 0, "linear_bwd_bf16: bad rows=%d n=%d k=%d", rows, n, k);
-  AVSR_REQUIRE_BYTES(avsr_linear_bwd_bf16_workspace_bytes(rows, n, k), workspace_bytes, "linear_bwd_bf16 workspace");
-  const long np = (long)pad64(n), rp = (long)pad64(rows);
+  AVSR_REQUIRE(rows > 0 && n > 0 && k > 0, "linear_bwd: bad rows=%d n=%d k=%d", rows, n, k);
+  AVSR_REQUIRE_BYTES(avsr_linear_bwd_workspace_bytes(rows, n, k, precision), workspace_bytes, "linear_bwd workspace");
   Carver cv{reinterpret_cast<char*>(workspace)};
-  __nv_bfloat16 *dy_op = cv.take<__nv_bfloat16>((size_t)rows * np), *wt_op = cv.take<__nv_bfloat16>((size_t)k * np),
-                *dyt_op = cv.take<__nv_bfloat16>((size_t)n * rp), *xt_op = cv.take<__nv_bfloat16>((size_t)k * rp);
+  const LinearBwdOperands o(cv, rows, n, k, precision);
   if (dx) {   // dX (rows, k) = dY W = dY (W^T)^T: K = n
-    AVSR_TRY(avsr_pack_operand(dy, dy_op, rows, n, np, 0, AVSR_PREC_BF16, stream));
-    AVSR_TRY(avsr_pack_operand(w, wt_op, n, k, np, 1, AVSR_PREC_BF16, stream));
-    AVSR_TRY(avsr_linear_operands(dy_op, wt_op, nullptr, nullptr, 1.0f, dx, rows, k, (int)np, 0, 0, AVSR_PREC_BF16, stream));
+    if (!o.dy_in_place) AVSR_TRY(avsr_pack_operand(dy, o.dy, rows, n, o.np, 0, o.pack_prec, stream));
+    AVSR_TRY(avsr_pack_operand(w, o.wt, n, k, o.np, 1, o.pack_prec, stream));
+    AVSR_TRY(avsr_linear_operands(o.dy_in_place ? dy : o.dy, o.wt, nullptr, nullptr, 1.0f, dx, rows, k, (int)o.np, 0, 0,
+                                  precision, stream));
   }
   if (dw) {   // dW (n, k) = dY^T X = dY^T (X^T)^T: K = rows
-    AVSR_TRY(avsr_pack_operand(dy, dyt_op, rows, n, rp, 1, AVSR_PREC_BF16, stream));
-    AVSR_TRY(avsr_pack_operand(x, xt_op, rows, k, rp, 1, AVSR_PREC_BF16, stream));
-    AVSR_TRY(avsr_linear_operands(dyt_op, xt_op, nullptr, nullptr, 1.0f, dw, n, k, (int)rp, 0, 0, AVSR_PREC_BF16, stream));
+    AVSR_TRY(avsr_pack_operand(dy, o.dyt, rows, n, o.rp, 1, o.pack_prec, stream));
+    AVSR_TRY(avsr_pack_operand(x, o.xt, rows, k, o.rp, 1, o.pack_prec, stream));
+    AVSR_TRY(avsr_linear_operands(o.dyt, o.xt, nullptr, nullptr, 1.0f, dw, n, k, (int)o.rp, 0, 0, precision, stream));
   }
   return AVSR_OK;
 }

@@ -14,8 +14,9 @@ from ..train import CtcLossFn, LinearFn, ctc_loss_forward
 
 class ProjEncoder(torch.nn.Linear):
     """``torch.nn.Linear(512, 768)`` that runs in libavsr_b200 (same parameters, same state-dict keys).  Eval: on the
-    prepared weights.  Train: ``LinearFn`` (forward GEMM in the module's precision, dgrad / wgrad as TF32 GEMMs), so the
-    input gradient flows back to the front-end.  CPU tensors are refused rather than silently computed elsewhere."""
+    prepared weights.  Train: ``LinearFn`` (forward GEMM in the module's precision, dgrad / wgrad as TF32 GEMMs in one
+    ``avsr_linear_bwd`` call), so the input gradient flows back to the front-end.  CPU tensors are refused rather than
+    silently computed elsewhere."""
 
     precision: Optional[str] = None
     _head: Optional[PreparedHead] = None

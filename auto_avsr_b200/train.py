@@ -1,6 +1,6 @@
 """Training slice of the encoder path (SURVEY.md 8f #2, first slice): ``torch.autograd.Function``s whose forward AND
-backward run in libavsr_b200 -- LayerNorm, Linear (+ReLU) with dgrad / wgrad as the same wgmma GEMMs on transposed
-operands, GLU, the depthwise conv, and the batch-statistics BatchNorm step (``bn_train_forward`` /
+backward run in libavsr_b200 -- LayerNorm, Linear (+ReLU) with dgrad / wgrad as the same wgmma GEMMs on operands the
+library transposes and pads (one avsr_linear_bwd call), GLU, the depthwise conv, and the batch-statistics BatchNorm step (``bn_train_forward`` /
 ``bn_train_backward``) that the conformer conv module and the ResNet front-ends (frontend_train.py) share: per-tile
 (count, mean, M2) merged with Chan's formula in fp64, running statistics as torch keeps them.  Gradients land on the
 original ``nn.Parameter``s (autograd accumulates what ``backward`` returns), so DDP hooks, ``clip_grad_norm_`` and
@@ -13,8 +13,8 @@ SyncBatchNorm (train.py:31) is honoured: the per-rank (count, mean, M2) are all-
 [sum ds, sum ds * x_hat] all-reduced in backward.
 Not built: dropout on attention probabilities (the reference trains with 0.0).
 
-Backward GEMMs run with TF32 operands (fp32 range: gradients do not fit fp16's) unless ``precision="fp32"``; a "bf16"
-forward keeps the TF32 backward too.  The encoder modules take an opt-in ``backward_precision="bf16"`` (env
+Backward GEMMs run with TF32 operands (fp32 range: gradients do not fit fp16's; packed unrounded, the tensor core
+truncates) unless ``precision="fp32"``; a "bf16" forward keeps the TF32 backward too.  The encoder modules take an opt-in ``backward_precision="bf16"`` (env
 AVSR_B200_BWD_PRECISION): every backward GEMM then gets bf16 operands (fp32's exponent range, an 8-bit mantissa) and the
 attention core's backward runs on the tensor cores (avsr_relpos_attention_bwd_tc)."""
 from __future__ import annotations
@@ -94,31 +94,19 @@ def colsum(y):
     return out
 
 
-def transpose_padded(x2d, pad_to: int = 32):
-    """(rows, cols) fp32 -> (cols, rows_padded) with zero padding of the new inner dim to a multiple of ``pad_to`` (the
-    tensor-core GEMMs take K in 128-byte blocks)."""
-    x2d = _c(x2d)
-    rows, cols = x2d.shape
-    ld = (rows + pad_to - 1) // pad_to * pad_to
-    out = torch.zeros(cols, ld, dtype=torch.float32, device=x2d.device) if ld != rows else \
-        torch.empty(cols, ld, dtype=torch.float32, device=x2d.device)
-    with torch.cuda.device(x2d.device):
-        check(lib.avsr_transpose(x2d.data_ptr(), out.data_ptr(), rows, cols, ld, _stream_handle(x2d.device)))
-    return out
-
-
-def linear_bwd_bf16(dy2, x2, w2, want_dx: bool, want_dw: bool):
-    """avsr_linear_bwd_bf16: dX = dY W and dW = dY^T X on bf16 operands (transposed, padded to 64 along K and converted
-    in one pass each inside the library), one call for both -> (dx (rows, k) | None, dw (n, k) | None)."""
+def linear_bwd(dy2, x2, w2, want_dx: bool, want_dw: bool, precision: str):
+    """avsr_linear_bwd: dX = dY W and dW = dY^T X in one call, on "fp32", "tf32" or "bf16" operands (transposed and
+    zero-padded along K in one pass each inside the library) -> (dx (rows, k) | None, dw (n, k) | None)."""
     dy2, x2, w2 = _c(dy2), _c(x2), _c(w2)
     rows, n = dy2.shape
     k = w2.size(1)
+    prec = PRECISIONS[precision]
     dx = torch.empty(rows, k, dtype=torch.float32, device=dy2.device) if want_dx else None
     dw = torch.empty(n, k, dtype=torch.float32, device=dy2.device) if want_dw else None
-    ws = _workspace(dy2.device, int(lib.avsr_linear_bwd_bf16_workspace_bytes(rows, n, k)))
+    ws = _workspace(dy2.device, int(lib.avsr_linear_bwd_workspace_bytes(rows, n, k, prec)))
     with torch.cuda.device(dy2.device):
-        check(lib.avsr_linear_bwd_bf16(dy2.data_ptr(), x2.data_ptr(), w2.data_ptr(), _ptr(dx), _ptr(dw), rows, n, k,
-                                       ws.data_ptr(), ws.numel(), _stream_handle(dy2.device)))
+        check(lib.avsr_linear_bwd(dy2.data_ptr(), x2.data_ptr(), w2.data_ptr(), _ptr(dx), _ptr(dw), rows, n, k, prec,
+                                  ws.data_ptr(), ws.numel(), _stream_handle(dy2.device)))
     return dx, dw
 
 
@@ -149,8 +137,8 @@ class LayerNormFn(torch.autograd.Function):
 
 class LinearFn(torch.autograd.Function):
     """y = act(x W^T + b), act = identity | ReLU (positionwise_feed_forward.py:28-30, the pointwise convs of
-    conformer_encoder.py:31,35).  Backward: dX = dY W and dW = dY^T X through the same GEMM entry on transposed operands,
-    db = column sums of dY."""
+    conformer_encoder.py:31,35).  Backward: dX = dY W and dW = dY^T X in one ``linear_bwd`` call (the same GEMM on
+    operands the library transposes and pads), db = column sums of dY."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, relu: bool, precision: str, backward: Optional[str] = None):
@@ -166,31 +154,17 @@ class LinearFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         x, w2, y = ctx.saved_tensors
-        prec = ctx.backward or bwd_precision(ctx.precision)
         dy = _c(dy)
         if ctx.relu:
             dy = relu_bwd(y, dy)
         n, k = w2.shape
-        dy2, x2 = dy.reshape(-1, n), _c(x).reshape(-1, k)
+        dy2 = dy.reshape(-1, n)
         dx = dw = db = None
-        if prec == "bf16":
-            if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
-                dx, dw = linear_bwd_bf16(dy2, x2, w2, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
-                dx = None if dx is None else dx.reshape(x.shape)
-                dw = None if dw is None else dw.reshape(ctx.wshape)
-            if ctx.has_bias and ctx.needs_input_grad[2]:
-                db = colsum(dy2)
-            return dx, dw, db, None, None, None
-        if ctx.needs_input_grad[0]:
-            wt = transpose_padded(w2, 32)                               # (k, n_padded): dX = dY W = dY (W^T)^T
-            dyp = dy2
-            if wt.size(1) != n:                                         # pad dY's columns like W^T's (zeros contribute 0)
-                dyp = torch.zeros(dy2.size(0), wt.size(1), dtype=torch.float32, device=dy.device)
-                dyp[:, :n] = dy2
-            dx = ops.linear(dyp, wt, None, precision=prec).reshape(x.shape)
-        if ctx.needs_input_grad[1]:
-            dyt, xt = transpose_padded(dy2, 32), transpose_padded(x2, 32)   # (n, rows_p), (k, rows_p)
-            dw = ops.linear(dyt, xt, None, precision=prec).reshape(ctx.wshape)
+        if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
+            dx, dw = linear_bwd(dy2, x.reshape(-1, k), w2, ctx.needs_input_grad[0], ctx.needs_input_grad[1],
+                                ctx.backward or bwd_precision(ctx.precision))
+            dx = None if dx is None else dx.reshape(x.shape)
+            dw = None if dw is None else dw.reshape(ctx.wshape)
         if ctx.has_bias and ctx.needs_input_grad[2]:
             db = colsum(dy2)
         return dx, dw, db, None, None, None

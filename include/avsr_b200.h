@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define AVSR_ABI_VERSION 11
+#define AVSR_ABI_VERSION 12
 
 enum {
   AVSR_OK = 0,
@@ -242,7 +242,7 @@ int avsr_ctc_logprobs(const AvsrEncoderConfig *cfg, const void *prepared_head, c
 
 /* ---- training slice (SURVEY.md 8f #2, first slice) ------------------------------------------------------------
  * Backward of the HBM-bound kernels and what a Linear's backward needs around the tensor-core GEMMs (dgrad / wgrad are
- * avsr_linear on transposed operands).  What they replace is torch.autograd's backward of layer_norm.py:21,
+ * avsr_linear_operands on transposed operands: avsr_linear_bwd).  What they replace is torch.autograd's backward of layer_norm.py:21,
  * positionwise_feed_forward.py:28-30 and conformer_encoder.py:30-35 under lightning.py:86-94.  All fp32; every
  * cross-row reduction is two-stage with a fixed order (deterministic).  workspace >= avsr_train_workspace_bytes. */
 size_t avsr_train_workspace_bytes(int rows, int d, int K);
@@ -251,20 +251,21 @@ int avsr_layernorm_bwd(const float *x, const float *gamma, const float *dy, floa
                        int rows, int d, void *workspace, size_t workspace_bytes, void *stream);
 /* out[c] = sum over rows of y[r][c] (bias gradients) */
 int avsr_colsum(const float *y, float *out, int rows, int cols, void *workspace, size_t workspace_bytes, void *stream);
-/* dst (cols, ld_dst >= rows) = src (rows, cols)^T; columns [rows, ld_dst) of dst are left untouched (pre-zeroed padding) */
-int avsr_transpose(const float *src, float *dst, int rows, int cols, long ld_dst, void *stream);
-/* fp32 (rows, cols) -> a bf16 GEMM operand (precision must be AVSR_PREC_BF16): transposed, dst (cols, ld_dst >= rows)
- * with dst[c][r] = src[r][c]; else dst (rows, ld_dst >= cols).  The padding columns are written as zeros.  The bf16
- * backward's dgrad / wgrad operands, transposed, padded and converted in one pass for avsr_linear_operands. */
+/* fp32 (rows, cols) -> a GEMM operand: AVSR_PREC_FP32 a plain fp32 copy, AVSR_PREC_BF16 converted to bf16; other
+ * precisions are refused.  Transposed, dst (cols, ld_dst >= rows) with dst[c][r] = src[r][c]; else dst
+ * (rows, ld_dst >= cols).  The padding columns are written as zeros.  The backward's dgrad / wgrad operands,
+ * transposed, padded and converted in one pass for avsr_linear_operands. */
 int avsr_pack_operand(const float *src, void *dst, int rows, int cols, long ld_dst, int transpose, int precision,
                       void *stream);
-/* Both GEMMs of a Linear's backward with bf16 operands (fp32 accumulation) in one call: dx (rows, k) = dy w and
- * dw (n, k) = dy^T x, for dy (rows, n), x (rows, k), w (n, k), all fp32.  dx or dw may be NULL (not wanted).  The
- * operands are packed with avsr_pack_operand into the workspace (>= avsr_linear_bwd_bf16_workspace_bytes), then
- * avsr_linear_operands runs on them. */
-size_t avsr_linear_bwd_bf16_workspace_bytes(int rows, int n, int k);
-int avsr_linear_bwd_bf16(const float *dy, const float *x, const float *w, float *dx, float *dw, int rows, int n, int k,
-                         void *workspace, size_t workspace_bytes, void *stream);
+/* Both GEMMs of a Linear's backward in one call: dx (rows, k) = dy w and dw (n, k) = dy^T x, for dy (rows, n),
+ * x (rows, k), w (n, k), all fp32; dx or dw may be NULL (not wanted).  precision: AVSR_PREC_FP32, AVSR_PREC_TF32 or
+ * AVSR_PREC_BF16 (AVSR_PREC_F16 is refused: gradients overflow its range).  The operands are packed with
+ * avsr_pack_operand into the workspace (>= avsr_linear_bwd_workspace_bytes), K zero-padded to 128 bytes (TF32 ones as
+ * unrounded fp32), then avsr_linear_operands runs on them; an fp32 / TF32 dy whose n is a multiple of 32 is read in
+ * place. */
+size_t avsr_linear_bwd_workspace_bytes(int rows, int n, int k, int precision);
+int avsr_linear_bwd(const float *dy, const float *x, const float *w, float *dx, float *dw, int rows, int n, int k,
+                    int precision, void *workspace, size_t workspace_bytes, void *stream);
 /* dx = dy * (y > 0) */
 int avsr_relu_bwd(const float *y, const float *dy, float *dx, long n, void *stream);
 /* F.glu over channels (conformer_encoder.py:32): in (rows, 2C) -> y (rows, C); and its backward din (rows, 2C) */

@@ -96,17 +96,29 @@ class _Ctx:
         self.__dict__.update(kw)
 
 
-def test_linear_backward_arguments(monkeypatch):
-    """backward=None keeps bwd_precision, fp32 transposes padded to 32 rows and ops.linear; "bf16" makes one library
-    call for both GEMMs (avsr_linear_bwd_bf16: operands packed to bf16, K padded to 64)."""
+class _RecordingLib:
+    """Stands in for the library: records the name of every entry looked up and refuses to run it."""
+
+    def __init__(self):
+        self.seen = []
+
+    def __getattr__(self, name):
+        self.seen.append(name)
+        raise AssertionError(f"unexpected library call {name}")
+
+
+def test_linear_backward_is_one_library_call(monkeypatch):
+    """Every backward precision makes one linear_bwd call for both GEMMs (avsr_linear_bwd: the library transposes and
+    pads the operands) with the resolved precision: backward=None keeps bwd_precision, "bf16" passes through.  No
+    ops.linear call and no other library call (no transpose) comes from Python."""
     calls = []
-    monkeypatch.setattr(TR.ops, "linear", lambda a, b, bias, precision: calls.append(("linear", precision)) or
-                        torch.zeros(a.shape[0], b.shape[0]))
-    monkeypatch.setattr(TR, "transpose_padded", lambda t, pad: calls.append(("pad", pad)) or
-                        torch.zeros(t.shape[1], (t.shape[0] + pad - 1) // pad * pad))
-    monkeypatch.setattr(TR, "linear_bwd_bf16", lambda dy2, x2, w2, a, b: calls.append(("bf16", tuple(dy2.shape),
-                        tuple(x2.shape), tuple(w2.shape), a, b)) or (torch.zeros(5, 8), torch.zeros(6, 8)))
+    monkeypatch.setattr(TR.ops, "linear", lambda *a, **kw: calls.append(("linear",)))
+    monkeypatch.setattr(TR, "linear_bwd", lambda dy2, x2, w2, a, b, precision: calls.append((
+        "linear_bwd", tuple(dy2.shape), tuple(x2.shape), tuple(w2.shape), a, b, precision)) or
+        (torch.zeros(5, 8), torch.zeros(6, 8)))
     monkeypatch.setattr(TR, "colsum", lambda t: torch.zeros(t.shape[1]))
+    rec = _RecordingLib()
+    monkeypatch.setattr(TR, "lib", rec)
     x, w, dy = torch.zeros(5, 8), torch.zeros(6, 8), torch.zeros(5, 6)
     for prec, backward, want in (("f16", None, "tf32"), ("bf16", None, "tf32"), ("fp32", None, "fp32"),
                                  ("f16", "bf16", "bf16"), ("fp32", "bf16", "bf16")):
@@ -115,29 +127,42 @@ def test_linear_backward_arguments(monkeypatch):
                    backward=backward, needs_input_grad=(True, True, True))
         out = TR.LinearFn.backward(ctx, dy)
         assert len(out) == 6 and out[0].shape == x.shape and out[1].shape == w.shape
-        if want == "bf16":
-            assert calls == [("bf16", (5, 6), (5, 8), (6, 8), True, True)]
-        else:
-            assert [c[1] for c in calls if c[0] == "linear"] == [want, want]
-            assert {c[1] for c in calls if c[0] == "pad"} == {32}
-            assert not any(c[0] == "bf16" for c in calls)
+        assert calls == [("linear_bwd", (5, 6), (5, 8), (6, 8), True, True, want)]
+    assert rec.seen == []
 
 
-def test_pack_operand_argument_errors_without_gpu():
+def test_pack_operand_and_linear_bwd_argument_errors_without_gpu():
     lib = _cabi.lib
     buf = C.create_string_buffer(1 << 12)
     p = C.addressof(buf)
     assert lib.avsr_pack_operand(None, p, 4, 4, 64, 1, PREC_BF16, None) == 1
-    assert lib.avsr_pack_operand(p, p, 4, 4, 64, 1, PREC_F16, None) == 1
+    for prec in (PREC_F16, PREC_TF32, 7, -1):                                   # fp32 and bf16 only
+        assert lib.avsr_pack_operand(p, p, 4, 4, 64, 1, prec, None) == 1
     assert lib.avsr_pack_operand(p, p, 65, 4, 64, 1, PREC_BF16, None) == 1     # ld < rows (transposed)
     assert lib.avsr_pack_operand(p, p, 4, 65, 64, 0, PREC_BF16, None) == 1     # ld < cols
+    assert lib.avsr_pack_operand(p, p, 65, 4, 64, 1, PREC_FP32, None) == 1
     assert lib.avsr_pack_operand(p, p, 0, 4, 64, 1, PREC_BF16, None) == 0      # empty: nothing launched
-    ws = lib.avsr_linear_bwd_bf16_workspace_bytes(100, 6, 8)
+    assert lib.avsr_pack_operand(p, p, 0, 4, 64, 1, PREC_FP32, None) == 0
+    # workspace: [dY (rows, n padded) unless it is read in place,] W^T (k, n padded), dY^T (n, rows padded),
+    # X^T (k, rows padded); K padded to 128 bytes
+    ws = lib.avsr_linear_bwd_workspace_bytes(100, 6, 8, PREC_BF16)
     assert ws == _align(100 * 64 * 2) + _align(8 * 64 * 2) + _align(6 * 128 * 2) + _align(8 * 128 * 2)
-    assert lib.avsr_linear_bwd_bf16(p, p, p, None, None, 100, 6, 8, p, ws, None) == 1      # neither output wanted
-    assert lib.avsr_linear_bwd_bf16(p, None, p, None, p, 100, 6, 8, p, ws, None) == 1      # dw without x
-    assert lib.avsr_linear_bwd_bf16(p, p, p, p, p, 0, 6, 8, p, ws, None) == 1
-    assert lib.avsr_linear_bwd_bf16(p, p, p, p, p, 100, 6, 8, p, ws - 1, None) == 3
+    for prec in (PREC_FP32, PREC_TF32):
+        assert lib.avsr_linear_bwd_workspace_bytes(100, 6, 8, prec) == (
+            _align(100 * 32 * 4) + _align(8 * 32 * 4) + _align(6 * 128 * 4) + _align(8 * 128 * 4))
+        assert lib.avsr_linear_bwd_workspace_bytes(100, 64, 8, prec) == (     # n % 32 == 0: dY read in place
+            _align(8 * 64 * 4) + _align(64 * 128 * 4) + _align(8 * 128 * 4))
+    assert lib.avsr_linear_bwd_workspace_bytes(100, 64, 8, PREC_BF16) == (
+        _align(100 * 64 * 2) + _align(8 * 64 * 2) + _align(64 * 128 * 2) + _align(8 * 128 * 2))
+    for prec in (PREC_F16, 7, -1):
+        assert lib.avsr_linear_bwd_workspace_bytes(100, 6, 8, prec) == 0
+    assert lib.avsr_linear_bwd(p, p, p, None, None, 100, 6, 8, PREC_BF16, p, ws, None) == 1   # neither output wanted
+    assert lib.avsr_linear_bwd(p, None, p, None, p, 100, 6, 8, PREC_BF16, p, ws, None) == 1   # dw without x
+    assert lib.avsr_linear_bwd(p, p, p, p, p, 0, 6, 8, PREC_BF16, p, ws, None) == 1
+    assert lib.avsr_linear_bwd(p, p, p, p, p, 100, 6, 8, PREC_BF16, p, ws - 1, None) == 3
+    assert lib.avsr_linear_bwd(p, p, p, p, p, 100, 6, 8, PREC_F16, p, ws, None) == 1          # gradients overflow f16
+    assert b"overflow f16" in lib.avsr_last_error()
+    assert lib.avsr_linear_bwd(p, p, p, p, p, 100, 6, 8, 7, p, ws, None) == 1
 
 
 def test_attention_backward_arguments(monkeypatch):

@@ -245,17 +245,17 @@ def test_pack_operand_matches_torch(dev, rows, cols):
 
 
 @pytest.mark.parametrize("rows,n,k", [(5, 6, 8), (111, 768, 768), (799, 768, 768), (1600, 3072, 768), (1600, 768, 3072)])
-def test_linear_bwd_bf16_vs_fp64(dev, rows, n, k):
-    """Both GEMMs of a Linear's bf16 backward (avsr_linear_bwd_bf16) against float64, and each alone."""
-    from auto_avsr_b200.train import linear_bwd_bf16
+def test_bf16_linear_bwd_vs_fp64(dev, rows, n, k):
+    """Both GEMMs of a Linear's bf16 backward (avsr_linear_bwd, "bf16") against float64, and each alone."""
+    from auto_avsr_b200.train import linear_bwd
     g = gen(rows * n + k, dev)
     dy, x, w = (torch.randn(*s, device=dev, generator=g) for s in ((rows, n), (rows, k), (n, k)))
-    dx, dw = linear_bwd_bf16(dy, x, w, True, True)
+    dx, dw = linear_bwd(dy, x, w, True, True, "bf16")
     ex, ew = rel(dx, dy.double() @ w.double()), rel(dw, dy.double().t() @ x.double())
     record("bf16_backward_linear", (rows, n, k), max(ex, ew), 1.2e-2)
     assert ex < 1.2e-2 and ew < 1.2e-2, (ex, ew)
-    dx1, dw1 = linear_bwd_bf16(dy, x, w, True, False)
-    dx2, dw2 = linear_bwd_bf16(dy, x, w, False, True)
+    dx1, dw1 = linear_bwd(dy, x, w, True, False, "bf16")
+    dx2, dw2 = linear_bwd(dy, x, w, False, True, "bf16")
     assert dw1 is None and dx2 is None and torch.equal(dx1, dx) and torch.equal(dw2, dw)
 
 

@@ -107,18 +107,28 @@ def test_colsum_vs_fp64(dev, rows, cols):
     check("train_kernels_colsum", (rows, cols), {"sum": rel(a, y.double().sum(0))}, 2.5e-6)
 
 
-# ------------------------------------------------------------------------------------------------ transpose with padding
+# ------------------------------------------------------------------------------------------------ fp32 operand packing
+@pytest.mark.parametrize("transpose", [1, 0])
 @pytest.mark.parametrize("rows,cols", [(1, 1), (5, 3), (33, 5), (37, 768), (111, 41), (799, 768), (1600, 5049)])
-def test_transpose_padded_exact_with_zero_padding(dev, rows, cols):
-    """(rows, cols) -> (cols, rows padded to 32): a copy, and the padding columns exactly 0 (the GEMMs sum over them)."""
-    from auto_avsr_b200.train import transpose_padded
+def test_pack_operand_fp32_exact_with_zero_padding(dev, rows, cols, transpose):
+    """avsr_pack_operand(AVSR_PREC_FP32): (rows, cols) -> (cols, rows padded to 32) transposed, else (rows, cols padded
+    to 32): an exact copy, and the padding columns exactly 0 (the GEMMs sum over them) over a NaN-filled buffer."""
+    import ctypes as C
+    from auto_avsr_b200._cabi import PREC_FP32, check, lib
     x = torch.randn(rows, cols, device=dev, generator=gen(rows * 31 + cols, dev))
-    t = transpose_padded(x, 32)
-    ld = (rows + 31) // 32 * 32
-    assert t.shape == (cols, ld)
-    assert torch.equal(t[:, :rows], x.t())
-    assert torch.equal(t[:, rows:], torch.zeros(cols, ld - rows, device=dev))
-    same_bits([t], [transpose_padded(x, 32)], "transpose")
+    src = x.t() if transpose else x
+    ld = (src.size(1) + 31) // 32 * 32
+
+    def pack():
+        out = torch.full((src.size(0), ld), float("nan"), device=dev)
+        check(lib.avsr_pack_operand(x.data_ptr(), out.data_ptr(), rows, cols, ld, transpose, PREC_FP32,
+                                    C.c_void_p(torch.cuda.current_stream().cuda_stream)))
+        return out
+
+    t = pack()
+    assert torch.equal(t[:, :src.size(1)], src)
+    assert torch.equal(t[:, src.size(1):], torch.zeros(src.size(0), ld - src.size(1), device=dev))
+    same_bits([t], [pack()], "pack_operand")
 
 
 # ------------------------------------------------------------------------------------------------ ReLU / GLU
@@ -362,22 +372,29 @@ def tile_env(tile):
             os.environ["AVSR_B200_TILE"] = old
 
 
+LIN_SHAPES = [(1, 8, 64), (111, 48, 768), (799, 768, 768), (1600, 3072, 768), (1600, 768, 3072), (1600, 5056, 768)]
+
+
+def linear_case(dev, rows, n, k):
+    g = gen(rows * 7 + n * 3 + k, dev)
+    x = torch.randn(rows, k, device=dev, generator=g)
+    w = torch.rand(n, k, device=dev, generator=g).sub_(0.5).mul_(2 / math.sqrt(k))
+    b = 0.1 * torch.randn(n, device=dev, generator=g)
+    dy = torch.randn(rows, n, device=dev, generator=g)
+    return x, w, b, dy
+
+
 @pytest.mark.parametrize("tile", [None, "64", "128"])
 @pytest.mark.parametrize("prec", ["fp32", "tf32"])
 @pytest.mark.parametrize("relu", [False, True])
-@pytest.mark.parametrize("rows,n,k", [(1, 8, 64), (111, 48, 768), (799, 768, 768), (1600, 3072, 768), (1600, 768, 3072),
-                                      (1600, 5056, 768)])
+@pytest.mark.parametrize("rows,n,k", LIN_SHAPES)
 def test_linear_fwd_bwd_vs_fp64(dev, rows, n, k, relu, prec, tile):
     """y = act(x W^T + b), dX = dY W, dW = dY^T X, db = colsum dY.  n % 32 != 0 pads dY / W^T, rows % 32 != 0 pads
     the wgrad's K; the tile width of every GEMM is left to the cost model or forced to 64 / 128 columns.  With ReLU the
     reference uses the mask the GPU forward produced (a pre-activation within rounding of 0 may flip: a derivative
     discontinuity, not an arithmetic error)."""
     from auto_avsr_b200.train import LinearFn
-    g = gen(rows * 7 + n * 3 + k, dev)
-    x = torch.randn(rows, k, device=dev, generator=g)
-    w = torch.rand(n, k, device=dev, generator=g).sub_(0.5).mul_(2 / math.sqrt(k))
-    b = 0.1 * torch.randn(n, device=dev, generator=g)
-    dy = torch.randn(rows, n, device=dev, generator=g)
+    x, w, b, dy = linear_case(dev, rows, n, k)
     runs = []
     with tile_env(tile):
         for _ in range(2):
@@ -396,6 +413,38 @@ def test_linear_fwd_bwd_vs_fp64(dev, rows, n, k, relu, prec, tile):
     want = {"y": h, "dx": dh @ w64, "dw": dh.t() @ x64, "db": dh.sum(0)}
     errs = {"y": rel(y, want["y"]), "dx": rel(dx, want["dx"]), "dw": rel(dw, want["dw"]), "db": rel(db, want["db"])}
     check("train_kernels_linear", (rows, n, k, "relu" if relu else "id", prec, f"tile {tile}"), errs, LIN_TOL[prec])
+
+
+@pytest.mark.parametrize("tile", [None, "64", "128"])
+@pytest.mark.parametrize("prec", ["fp32", "tf32"])
+@pytest.mark.parametrize("relu", [False, True])
+@pytest.mark.parametrize("rows,n,k", LIN_SHAPES)
+def test_linear_bwd_bit_identical_to_torch_packed_operands(dev, rows, n, k, relu, prec, tile):
+    """LinearFn's default backward (one avsr_linear_bwd call) gives the same bits as the per-op GEMM entry on operands
+    laid out with torch ops: W^T, dY^T and X^T zero-padded along K to a multiple of 32, dY's columns zero-padded when
+    n % 32 != 0, then ops.linear for dX and for dW; db from colsum.  So the library's packing (TF32 operands unrounded,
+    the same K, the same epilogue) leaves every GEMM exactly as the per-op entry runs it."""
+    from auto_avsr_b200 import ops
+    from auto_avsr_b200.train import LinearFn, colsum
+    x, w, b, dy = linear_case(dev, rows, n, k)
+
+    def t_pad(a):
+        out = torch.zeros(a.size(1), (a.size(0) + 31) // 32 * 32, device=dev)
+        out[:, :a.size(0)] = a.t()
+        return out
+
+    with tile_env(tile):
+        leaves = [t.clone().requires_grad_(True) for t in (x, w, b)]
+        y = LinearFn.apply(*leaves, relu, prec)
+        y.backward(dy)
+        dh = torch.where(y > 0, dy, torch.zeros_like(dy)) if relu else dy
+        wt = t_pad(w)
+        dhp = torch.zeros(rows, wt.size(1), device=dev)
+        dhp[:, :n] = dh
+        want = [ops.linear(dhp, wt, None, precision=prec), ops.linear(t_pad(dh), t_pad(x), None, precision=prec),
+                colsum(dh)]
+    for name, got, ref in zip(("dx", "dw", "db"), [t.grad for t in leaves], want):
+        assert torch.equal(got, ref), (name, (got - ref).abs().max().item())
 
 
 # ------------------------------------------------------------------------------------------------ encoder vs the reference
