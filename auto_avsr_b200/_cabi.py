@@ -151,6 +151,9 @@ SIGNATURES = {
     "avsr_mha_core_bwd_workspace_bytes": (_Z, [_I, _I, _I]),
     "avsr_mha_core_bwd": (_I, [_P, C.c_long, _P, C.c_long, _P, C.c_long, _I, _I, _I, _I, _I, _P, _P, _F, _P, _P, _P,
                                C.c_long, _P, _P, C.c_long, _P, _Z, _P]),
+    "avsr_mha_core_bwd_tc_workspace_bytes": (_Z, [_I, _I, _I, _I, _I]),
+    "avsr_mha_core_bwd_tc": (_I, [_P, C.c_long, _P, C.c_long, _P, C.c_long, _I, _I, _I, _I, _I, _P, _P, _F, _P, _P, _P,
+                                  _P, C.c_long, _P, _P, C.c_long, _I, _P, _Z, _P]),
     "avsr_label_smoothing_fwd": (_I, [_P, C.c_long, _P, _I, _I, _I, _F, _P, _P, _P]),
     "avsr_label_smoothing_bwd": (_I, [_P, C.c_long, _P, _I, _I, _I, _F, _P, _P, _P, C.c_long, _P]),
     "avsr_embed_fwd": (_I, [_P, _P, _I, _I, _I, _I, _P, _P]),

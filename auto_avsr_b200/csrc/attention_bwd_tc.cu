@@ -24,18 +24,14 @@
 // Keys j >= len[b] get A = 0; a zero-length utterance gives zero gradients; padded query rows (len <= i < T) are computed
 // like any other row, rows i >= T of a tile (the next head's data) get A = 0 through an infinite log-sum-exp.  No atomics
 // and every sum in a fixed order: repeated calls are bit-identical.
-#include "common.cuh"
-#include "sm90.cuh"
+#include "bwd_tc_tiles.cuh"
 
 namespace avsr {
 
 using namespace sm90;
 
-constexpr int BW_TILE = 64;                 // queries / keys per tile (= wgmma M)
 constexpr int BW_BAND = 128;                // table rows per tile pair (>= 2 * 64 - 1)
-constexpr int BW_THREADS = 128;             // one warpgroup
 constexpr int BW_GLD = 64 + 4;              // fp32 row stride of the pre-skewed G tile
-constexpr uint32_t BW_TB = 64 * 128;        // one [64 rows][64 bf16] 128B-swizzled tile
 constexpr uint32_t BW_BB = BW_BAND * 128;   // the band: [128 rows][64 bf16]
 constexpr uint32_t BW_GSK = 64 * BW_GLD * 4;
 constexpr float BW_SCALE = 0.125f * 1.4426950408889634f;   // 1/sqrt(64) * log2(e): scores in log2 units
@@ -52,17 +48,6 @@ struct BwKv {   // K, V | Qu, Qv, dO, Pband | A, g (or g_band for the dp kernel)
                             kRows = kGsk + BW_GSK, kBars = kRows + 2 * 64 * 4, kSmem = kBars + 64 + 1024;
 };
 
-// MMA-K step ks (16 bf16 = 32 bytes) of a K-major [rows][K] tile stored as atoms of [rows][128 B]
-__device__ __forceinline__ uint64_t bw_kdesc(uint32_t tile, int rows, int ks) {
-  const int bytes = ks * 32;
-  return wgmma_desc_sw128(tile + (bytes >> 7) * (rows * 128) + (bytes & 127));
-}
-// MMA-K step ks of an MN-major [K rows][64] tile: rows 16 ks .. 16 ks + 15
-__device__ __forceinline__ uint64_t bw_mdesc(uint32_t tile, int ks) { return wgmma_desc_sw128(tile + ks * 16 * 128); }
-// byte offset of element (r, c) of a [64 rows][C bf16] tile stored as 128B-swizzled atoms of 64 columns
-__device__ __forceinline__ uint32_t bw_off(int r, int c) {
-  return (c >> 6) * BW_TB + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4) + (c & 7) * 2;
-}
 // utterance chunks of the dp kernel: enough (h, diagonal, chunk) CTAs for 2 per SM on 132 SMs, each chunk non-empty;
 // a function of the shape only, so the summation order is fixed
 static inline void bw_dp_chunks(int B, int T, int H, int* chunks, int* per_chunk) {
@@ -120,16 +105,6 @@ __device__ __forceinline__ void bw_scores(uint32_t qu, uint32_t qv, uint32_t kt,
   __syncwarp();   // this warp's reads of gsk are done before its next writes
 }
 
-// dP[64 x 64] = dO.V^T (both K-major), the same layout as S
-__device__ __forceinline__ void bw_dprod(uint32_t o, uint32_t v, float (&dp)[32]) {
-  wgmma_fence();
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks) wgmma_bf16_n64(dp, bw_kdesc(o, 64, ks), bw_kdesc(v, 64, ks), ks != 0);
-  wgmma_commit();
-  wgmma_wait<0>();
-  wgmma_fence_regs<32>(dp);
-}
-
 // sc (log2 scores) -> A, dp (dO.V^T) -> g, with keys j0 + c >= L masked; lse2 / dl: this thread's two rows
 __device__ __forceinline__ void bw_probs(float (&sc)[32], float (&dp)[32], const float (&lse2)[2], const float (&dl)[2],
                                          int j0, int L, int cq) {
@@ -146,16 +121,6 @@ __device__ __forceinline__ void bw_probs(float (&sc)[32], float (&dp)[32], const
       }
 }
 
-// a [64 x 64] accumulator -> bf16 [64 rows][64] 128B-swizzled tile (readable K-major and, transposed, MN-major)
-__device__ __forceinline__ void bw_store_tile(uint8_t* tile, const float (&x)[32], int r0, int cq) {
-#pragma unroll
-  for (int rr = 0; rr < 2; ++rr)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int r = r0 + 8 * rr;
-      *reinterpret_cast<uint32_t*>(tile + bw_off(r, 8 * j + cq)) = pack_bf162(x[4 * j + 2 * rr], x[4 * j + 2 * rr + 1]);
-    }
-}
 // g -> g_band: g_band[r][c + 63 - r] = g[r][c].  Every tile writes the same positions; the rest stays zero.
 __device__ __forceinline__ void bw_store_band(uint8_t* band, const float (&g)[32], int r0, int cq) {
 #pragma unroll
@@ -169,21 +134,6 @@ __device__ __forceinline__ void bw_store_band(uint8_t* band, const float (&g)[32
             __float2bfloat16_rn(g[4 * j + 2 * rr + e]);
       }
 }
-__device__ __forceinline__ void bw_zero(uint8_t* p, uint32_t bytes) {
-  for (uint32_t x = threadIdx.x; x < bytes / 16; x += BW_THREADS) reinterpret_cast<uint4*>(p)[x] = make_uint4(0, 0, 0, 0);
-}
-// accumulator rows r (+ row_off) < rows_valid of a [64 x 64] tile -> fp32 rows of `dst` (row stride ld)
-__device__ __forceinline__ void bw_store_out(float* dst, long ld, const float (&x)[32], int r0, int cq, int rows_valid) {
-#pragma unroll
-  for (int rr = 0; rr < 2; ++rr) {
-    const int r = r0 + 8 * rr;
-    if (r >= rows_valid) continue;
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-      *reinterpret_cast<float2*>(dst + (long)r * ld + 8 * j + cq) = make_float2(x[4 * j + 2 * rr], x[4 * j + 2 * rr + 1]);
-  }
-}
-
 // ---------------------------------------------------------------- Delta_i = dctx_i . ctx_i (fp32), one warp per (b, t, h)
 __global__ void attn_bwd_tc_delta_kernel(const float* __restrict__ ctx, const float* __restrict__ dctx,
                                          float* __restrict__ delta, int B, int T, int H) {
@@ -540,11 +490,6 @@ static BwTcWork bwtc_layout(void* ws, int B, int T, int H) {
   w.part = cv.take((size_t)H * nd * chunks * BW_BAND * kHeadDim);
   w.bytes = cv.off;
   return w;
-}
-
-static const char* precision_name(int p) {
-  return p == AVSR_PREC_FP32 ? "AVSR_PREC_FP32" : p == AVSR_PREC_TF32 ? "AVSR_PREC_TF32"
-       : p == AVSR_PREC_F16 ? "AVSR_PREC_F16" : p == AVSR_PREC_BF16 ? "AVSR_PREC_BF16" : "unknown";
 }
 
 }  // namespace avsr

@@ -14,7 +14,11 @@ encoder path's ``LinearFn`` / ``LayerNormFn`` / ``feed_forward_train`` into ``Tr
 
 torch supplies device memory, the autograd tape, dropout masks and the residual adds.  Gradients land on the original
 ``Parameter``s; the memory gradient flows back into the encoder.  Under ``torch.no_grad()`` or in ``eval()`` the same
-kernels run without storing probabilities and without dropout."""
+kernels run without storing probabilities and without dropout.
+
+``TransformerDecoder.backward_precision = "bf16"`` gives every backward GEMM of the decoder bf16 operands and runs the
+attention core's backward on the tensor cores (avsr_mha_core_bwd_tc); None (the default) keeps the TF32 / fp32 backward.
+Embedding, LayerNorm and the label-smoothing loss keep their fp32 kernels."""
 from __future__ import annotations
 
 from typing import Optional
@@ -24,6 +28,7 @@ import torch.nn.functional as F
 
 from ._cabi import check, lib
 from .engine import _ptr, _stream_handle
+from .engine import PRECISIONS
 from .train import LayerNormFn, LinearFn, _c, _workspace, feed_forward_train
 
 
@@ -80,6 +85,25 @@ def mha_core_backward(q, k, v, n_heads: int, causal: bool, lengths, keep, keep_s
                                     ws.data_ptr(), ws.numel(), _stream_handle(q.device)))
 
 
+def mha_core_backward_tc(q, k, v, n_heads: int, causal: bool, lengths, keep, keep_scale: float, probs, out, dctx, dq, dk,
+                         dv):
+    """avsr_mha_core_bwd_tc (bf16 operands on the tensor cores, fp32 accumulation): ``mha_core_backward`` plus the
+    forward's output ``out`` (B, Lq, H*64), from which Delta = rowsum(dctx o out) is taken."""
+    (q, ldq), (k, ldk), (v, ldv) = _rows(q.detach()), _rows(k.detach()), _rows(v.detach())
+    B, Lq, _ = q.shape
+    Lk = k.size(1)
+    dctx, out = _c(dctx), _c(out)
+    assert dk.stride(1) == dv.stride(1)
+    prec = PRECISIONS["bf16"]
+    ws = _workspace(q.device, int(lib.avsr_mha_core_bwd_tc_workspace_bytes(B, n_heads, Lq, Lk, prec)))
+    with torch.cuda.device(q.device):
+        check(lib.avsr_mha_core_bwd_tc(q.data_ptr(), ldq, k.data_ptr(), ldk, v.data_ptr(), ldv, B, n_heads, Lq, Lk,
+                                       int(causal), _ptr(lengths), _ptr(keep), float(keep_scale), probs.data_ptr(),
+                                       out.data_ptr(), dctx.data_ptr(), dq.data_ptr(), dq.stride(1), dk.data_ptr(),
+                                       dv.data_ptr(), dk.stride(1), prec, ws.data_ptr(), ws.numel(),
+                                       _stream_handle(q.device)))
+
+
 def _split(qsrc, kvsrc, self_attn: bool, D: int):
     if self_attn:
         return qsrc[..., :D], qsrc[..., D:2 * D], qsrc[..., 2 * D:3 * D]
@@ -89,38 +113,49 @@ def _split(qsrc, kvsrc, self_attn: bool, D: int):
 class MhaCoreFn(torch.autograd.Function):
     """ctx = dropout(softmax(q k^T / 8, mask)) v  (attention.py:59-88).  Self attention: ``qsrc`` is the (B, L, 3d)
     q|k|v GEMM output and ``kvsrc`` the same tensor; source attention: ``qsrc`` (B, L, d) and ``kvsrc`` the (B, T, 2d)
-    k|v GEMM output.  The gradient comes back in the same fused layouts (no slicing copies)."""
+    k|v GEMM output.  The gradient comes back in the same fused layouts (no slicing copies).  Backward: the fp32 kernels
+    (``mha_core_backward``), or with ``backward="bf16"`` the tensor-core kernels (``mha_core_backward_tc``), which also
+    need the output, so only then is it saved."""
 
     @staticmethod
-    def forward(ctx_, qsrc, kvsrc, self_attn: bool, n_heads: int, causal: bool, lengths, keep, keep_scale: float):
+    def forward(ctx_, qsrc, kvsrc, self_attn: bool, n_heads: int, causal: bool, lengths, keep, keep_scale: float,
+                backward: Optional[str] = None):
         D = n_heads * 64
         q, k, v = _split(qsrc, kvsrc, self_attn, D)
         out, probs = mha_core_forward(q, k, v, n_heads, causal, lengths, keep, keep_scale, want_probs=True)
-        ctx_.save_for_backward(qsrc, kvsrc, lengths, keep, probs)
+        ctx_.save_for_backward(qsrc, kvsrc, lengths, keep, probs, out if backward == "bf16" else None)
         ctx_.cfg = (self_attn, n_heads, causal, keep_scale)
+        ctx_.backward = backward
         return out
 
     @staticmethod
     def backward(ctx_, dout):
-        qsrc, kvsrc, lengths, keep, probs = ctx_.saved_tensors
+        qsrc, kvsrc, lengths, keep, probs, out = ctx_.saved_tensors
         self_attn, n_heads, causal, keep_scale = ctx_.cfg
         D = n_heads * 64
         q, k, v = _split(qsrc, kvsrc, self_attn, D)
+
+        def core_bwd(dq, dk, dv):
+            if ctx_.backward == "bf16":
+                mha_core_backward_tc(q, k, v, n_heads, causal, lengths, keep, keep_scale, probs, out, dout, dq, dk, dv)
+            else:
+                mha_core_backward(q, k, v, n_heads, causal, lengths, keep, keep_scale, probs, dout, dq, dk, dv)
+
         if self_attn:
             dsrc = torch.empty(qsrc.shape, dtype=torch.float32, device=qsrc.device)
-            dq, dk, dv = _split(dsrc, None, True, D)
-            mha_core_backward(q, k, v, n_heads, causal, lengths, keep, keep_scale, probs, dout, dq, dk, dv)
-            return dsrc, None, None, None, None, None, None, None
+            core_bwd(*_split(dsrc, None, True, D))
+            return dsrc, None, None, None, None, None, None, None, None
         dq = torch.empty(qsrc.shape, dtype=torch.float32, device=qsrc.device)
         dkv = torch.empty(kvsrc.shape, dtype=torch.float32, device=kvsrc.device)
-        mha_core_backward(q, k, v, n_heads, causal, lengths, keep, keep_scale, probs, dout, dq, dkv[..., :D], dkv[..., D:])
-        return dq, dkv, None, None, None, None, None, None
+        core_bwd(dq, dkv[..., :D], dkv[..., D:])
+        return dq, dkv, None, None, None, None, None, None, None
 
 
-def mha_core(qsrc, kvsrc, self_attn: bool, n_heads: int, causal: bool, lengths, keep, keep_scale: float):
+def mha_core(qsrc, kvsrc, self_attn: bool, n_heads: int, causal: bool, lengths, keep, keep_scale: float,
+             backward: Optional[str] = None):
     """``MhaCoreFn`` when a gradient is wanted; otherwise the forward kernel alone (no probabilities stored)."""
     if torch.is_grad_enabled() and (qsrc.requires_grad or kvsrc.requires_grad):
-        return MhaCoreFn.apply(qsrc, kvsrc, self_attn, n_heads, causal, lengths, keep, keep_scale)
+        return MhaCoreFn.apply(qsrc, kvsrc, self_attn, n_heads, causal, lengths, keep, keep_scale, backward)
     q, k, v = _split(qsrc, kvsrc, self_attn, n_heads * 64)
     return mha_core_forward(q, k, v, n_heads, causal, lengths, keep, keep_scale, want_probs=False)[0]
 
@@ -229,57 +264,58 @@ def _check_heads(m):
         raise NotImplementedError(f"decoder attention: d_k = 64 only (got {m.d_k})")
 
 
-def self_attention_train(m, x, lengths, precision: str):
+def self_attention_train(m, x, lengths, precision: str, backward: Optional[str] = None):
     """MultiHeadedAttention(x, x, x, tgt_mask) (attention.py:90-110) with the causal target mask: one q|k|v GEMM."""
     _check_heads(m)
     B, L, _ = x.shape
     w = torch.cat([m.linear_q.weight, m.linear_k.weight, m.linear_v.weight])
     b = torch.cat([m.linear_q.bias, m.linear_k.bias, m.linear_v.bias])
-    qkv = LinearFn.apply(x, w, b, False, precision)
+    qkv = LinearFn.apply(x, w, b, False, precision, backward)
     keep, scale = _keep(m, B, L, L, x.device)
-    ctx = mha_core(qkv, qkv, True, m.h, True, lengths, keep, scale)
-    return LinearFn.apply(ctx, m.linear_out.weight, m.linear_out.bias, False, precision)
+    ctx = mha_core(qkv, qkv, True, m.h, True, lengths, keep, scale, backward)
+    return LinearFn.apply(ctx, m.linear_out.weight, m.linear_out.bias, False, precision, backward)
 
 
-def source_attention_train(m, x, memory, mem_lengths, precision: str):
+def source_attention_train(m, x, memory, mem_lengths, precision: str, backward: Optional[str] = None):
     """MultiHeadedAttention(x, memory, memory, memory_mask): q GEMM on x, one k|v GEMM on the memory."""
     _check_heads(m)
     B, L, _ = x.shape
-    q = LinearFn.apply(x, m.linear_q.weight, m.linear_q.bias, False, precision)
+    q = LinearFn.apply(x, m.linear_q.weight, m.linear_q.bias, False, precision, backward)
     kv = LinearFn.apply(memory, torch.cat([m.linear_k.weight, m.linear_v.weight]),
-                        torch.cat([m.linear_k.bias, m.linear_v.bias]), False, precision)
+                        torch.cat([m.linear_k.bias, m.linear_v.bias]), False, precision, backward)
     keep, scale = _keep(m, B, L, memory.size(1), x.device)
-    ctx = mha_core(q, kv, False, m.h, False, mem_lengths, keep, scale)
-    return LinearFn.apply(ctx, m.linear_out.weight, m.linear_out.bias, False, precision)
+    ctx = mha_core(q, kv, False, m.h, False, mem_lengths, keep, scale, backward)
+    return LinearFn.apply(ctx, m.linear_out.weight, m.linear_out.bias, False, precision, backward)
 
 
-def decoder_layer_train(layer, x, tgt_lengths, memory, mem_lengths, precision: str):
+def decoder_layer_train(layer, x, tgt_lengths, memory, mem_lengths, precision: str, backward: Optional[str] = None):
     """DecoderLayer.forward (transformer_decoder.py:65-128): pre-norm, concat_after=False, no cache."""
     if getattr(layer.feed_forward, "backward_precision", None) is not None:
-        raise ValueError("feed_forward.backward_precision is set on a decoder layer: the bf16 backward is an encoder "
-                         "option; the decoder trains with the default backward")
+        raise ValueError("feed_forward.backward_precision is set on a decoder layer: the per-module knob is an encoder "
+                         "option; set TransformerDecoder.backward_precision for the whole decoder")
     h = LayerNormFn.apply(x, layer.norm1.weight, layer.norm1.bias)
-    x = x + layer.dropout(self_attention_train(layer.self_attn, h, tgt_lengths, precision))
+    x = x + layer.dropout(self_attention_train(layer.self_attn, h, tgt_lengths, precision, backward))
     h = LayerNormFn.apply(x, layer.norm2.weight, layer.norm2.bias)
-    x = x + layer.dropout(source_attention_train(layer.src_attn, h, memory, mem_lengths, precision))
+    x = x + layer.dropout(source_attention_train(layer.src_attn, h, memory, mem_lengths, precision, backward))
     h = LayerNormFn.apply(x, layer.norm3.weight, layer.norm3.bias)
-    return x + layer.dropout(feed_forward_train(layer.feed_forward, h, precision))
+    return x + layer.dropout(feed_forward_train(layer.feed_forward, h, precision, backward))
 
 
-def decoder_forward(dec, tgt, tgt_lengths, memory, mem_lengths, precision: str):
+def decoder_forward(dec, tgt, tgt_lengths, memory, mem_lengths, precision: str, backward: Optional[str] = None):
     """TransformerDecoder.forward (transformer_decoder.py:229-258) -> (B, L, odim) logits: a column view of the
-    (B, L, odim padded to a multiple of 8) output-layer GEMM."""
+    (B, L, odim padded to a multiple of 8) output-layer GEMM.  ``backward`` (None | "bf16") goes to every GEMM and
+    attention core of the pass."""
     emb = dec.embed[0].weight
     x = dec.embed[1].dropout(EmbedFn.apply(tgt, emb))
     for layer in dec.decoders:
-        x = decoder_layer_train(layer, x, tgt_lengths, memory, mem_lengths, precision)
+        x = decoder_layer_train(layer, x, tgt_lengths, memory, mem_lengths, precision, backward)
     x = LayerNormFn.apply(x, dec.after_norm.weight, dec.after_norm.bias)
     w, b = dec.output_layer.weight, dec.output_layer.bias
     odim = w.size(0)
     npad = (odim + 7) // 8 * 8
     if npad != odim:
         w, b = F.pad(w, (0, 0, 0, npad - odim)), F.pad(b, (0, npad - odim))
-    return LinearFn.apply(x, w, b, False, precision)[..., :odim]
+    return LinearFn.apply(x, w, b, False, precision, backward)[..., :odim]
 
 
 def label_smoothing_loss(x, target, ignore_id: int, smoothing: float):

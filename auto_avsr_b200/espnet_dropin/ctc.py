@@ -9,22 +9,25 @@ import torch.nn.functional as F
 from .. import ops
 from ..engine import default_precision, require_cuda
 from ..head import PreparedHead, ctc_log_probs, proj_forward
-from ..train import CtcLossFn, LinearFn, ctc_loss_forward
+from ..train import CtcLossFn, LinearFn, ctc_loss_forward, explicit_backward_precision
 
 
 class ProjEncoder(torch.nn.Linear):
     """``torch.nn.Linear(512, 768)`` that runs in libavsr_b200 (same parameters, same state-dict keys).  Eval: on the
     prepared weights.  Train: ``LinearFn`` (forward GEMM in the module's precision, dgrad / wgrad as TF32 GEMMs in one
-    ``avsr_linear_bwd`` call), so the input gradient flows back to the front-end.  CPU tensors are refused rather than
-    silently computed elsewhere."""
+    ``avsr_linear_bwd`` call, bf16 ones with ``backward_precision="bf16"``), so the input gradient flows back to the
+    front-end.  CPU tensors are refused rather than silently computed elsewhere."""
 
     precision: Optional[str] = None
+    #: training backward: None (default) | "bf16"; AVSR_B200_BWD_PRECISION does not apply here
+    backward_precision: Optional[str] = None
     _head: Optional[PreparedHead] = None
 
     def forward(self, x):
         prec = self.precision or default_precision()
         if self.training:
-            return LinearFn.apply(x, self.weight, self.bias, False, prec)
+            return LinearFn.apply(x, self.weight, self.bias, False, prec,
+                                  explicit_backward_precision(self.backward_precision))
         require_cuda(x, "ProjEncoder input")
         if self._head is None:
             self._head = PreparedHead(self.out_features, max(1, self.out_features // 64))
@@ -47,6 +50,8 @@ class CTC(torch.nn.Module):
         self.ignore_id = -1
         self.reduce = reduce
         self.precision: Optional[str] = None
+        #: backward of the ctc_lo GEMM: None (default) | "bf16"; AVSR_B200_BWD_PRECISION does not apply here
+        self.backward_precision: Optional[str] = None
         self._head: Optional[PreparedHead] = None
 
     # ------------------------------------------------------------------ helpers
@@ -66,13 +71,15 @@ class CTC(torch.nn.Module):
         """CTC loss (ctc.py:41-65) -> (loss, ys_hat).  hs_pad (B, Tmax, eprojs), hlens (B), ys_pad (B, Lmax) with
         ``ignore_id`` (-1) entries dropped wherever they sit; loss = CTCLoss(zero_infinity) / B, summed when ``reduce``;
         ys_hat = the (Tmax, B, odim) logits.  ctc_lo is ``LinearFn`` on the weight padded to a multiple of 8 rows (the
-        tensor-core GEMM's N), the loss ``CtcLossFn``; labels and lengths stay on the device.  Without autograd
+        tensor-core GEMM's N; its backward bf16 with ``backward_precision="bf16"``), the loss ``CtcLossFn`` (fp32);
+        labels and lengths stay on the device.  Without autograd
         (``torch.no_grad()``, as in Lightning's validation step, or when nothing involved needs a gradient) the loss is
         computed without the beta recursion and nothing is kept for a backward."""
         if not hs_pad.is_cuda:
             raise NotImplementedError("CTC.forward: the CTC loss runs on CUDA tensors only (no CPU fallback)")
         require_cuda(hs_pad, "CTC input")
         prec = self.precision or default_precision()
+        backward = explicit_backward_precision(self.backward_precision)
         B = hs_pad.size(0)
         odim = self.ctc_lo.out_features
         w, b = self.ctc_lo.weight, self.ctc_lo.bias
@@ -81,7 +88,7 @@ class CTC(torch.nn.Module):
             w, b = F.pad(w, (0, 0, 0, npad - odim)), F.pad(b, (0, npad - odim))
         x = self.dropout(hs_pad)
         if torch.is_grad_enabled() and (x.requires_grad or w.requires_grad or b.requires_grad):
-            logits = LinearFn.apply(x, w, b, False, prec)
+            logits = LinearFn.apply(x, w, b, False, prec, backward)
             nll = CtcLossFn.apply(logits, hlens, ys_pad, odim, self.ignore_id)
         else:
             with torch.no_grad():

@@ -113,6 +113,9 @@ class TransformerDecoder(_si.BatchScorerInterface, torch.nn.Module):
         self.odim = odim
         self._cfg = (odim, attention_dim, attention_heads, linear_units, num_blocks)
         self.precision: Optional[str] = None
+        #: training backward: None (TF32 GEMMs, fp32 attention core) | "bf16" (bf16 GEMM operands, tensor-core attention
+        #: core).  AVSR_B200_BWD_PRECISION does not apply here: only this attribute selects it.
+        self.backward_precision: Optional[str] = None
         #: verify that forward's tgt_mask / memory_mask have the form passed on as lengths (one host sync each)
         self.check_mask = os.environ.get("AVSR_B200_CHECK_MASK", "0") == "1"
         #: beam slots per position the per-utterance session is sized for (>= the beam size of the search)
@@ -136,15 +139,19 @@ class TransformerDecoder(_si.BatchScorerInterface, torch.nn.Module):
         mode, forward and backward in libavsr_b200 (auto_avsr_b200/decoder_train.py).  tgt (B, L) int64 token ids;
         tgt_mask (B, L, L) = target_mask(tgt, ignore_id) (key prefix AND causal: passed on as key lengths + a causal
         flag); memory (B, T, d) fp32; memory_mask (B, 1, T) prefix mask or None.  GEMMs run in ``precision`` (backward
-        GEMMs TF32 unless fp32); pred_pad is a column view of the output-layer GEMM padded to a multiple of 8 columns."""
+        GEMMs TF32 unless fp32, or bf16 with ``backward_precision="bf16"``); pred_pad is a column view of the
+        output-layer GEMM padded to a multiple of 8 columns."""
         if not (tgt.is_cuda and memory.is_cuda):
             raise NotImplementedError("TransformerDecoder.forward runs on CUDA tensors only (no CPU fallback)")
         from ..decoder_train import decoder_forward, target_lengths
+        from ..train import explicit_backward_precision
         from .attention import mask_to_lengths
+        backward = explicit_backward_precision(self.backward_precision)
         B, L = tgt.shape
         tgt_lengths = target_lengths(tgt_mask, B, L, self.check_mask)
         mem_lengths = None if memory_mask is None else mask_to_lengths(memory_mask, B, memory.size(1), check=self.check_mask)
-        pred = decoder_forward(self, tgt, tgt_lengths, memory, mem_lengths, self.precision or default_precision())
+        pred = decoder_forward(self, tgt, tgt_lengths, memory, mem_lengths, self.precision or default_precision(),
+                               backward)
         return pred, tgt_mask
 
     def forward_one_step(self, tgt, tgt_mask, memory, memory_mask=None, cache=None):

@@ -16,7 +16,9 @@ Not built: dropout on attention probabilities (the reference trains with 0.0).
 Backward GEMMs run with TF32 operands (fp32 range: gradients do not fit fp16's; packed unrounded, the tensor core
 truncates) unless ``precision="fp32"``; a "bf16" forward keeps the TF32 backward too.  The encoder modules take an opt-in ``backward_precision="bf16"`` (env
 AVSR_B200_BWD_PRECISION): every backward GEMM then gets bf16 operands (fp32's exponent range, an 8-bit mantissa) and the
-attention core's backward runs on the tensor cores (avsr_relpos_attention_bwd_tc)."""
+attention core's backward runs on the tensor cores (avsr_relpos_attention_bwd_tc).  ``TransformerDecoder``,
+``ProjEncoder`` and ``CTC`` take the same attribute (decoder_train.py, espnet_dropin/ctc.py), without the environment
+fallback."""
 from __future__ import annotations
 
 import ctypes as C
@@ -56,6 +58,12 @@ def resolve_backward_precision(value: Optional[str]) -> Optional[str]:
     ``bwd_precision``).  "bf16" is the only other choice: an f16 backward is not offered, gradients overflow its range."""
     if value is None:
         value = os.environ.get("AVSR_B200_BWD_PRECISION") or None
+    return explicit_backward_precision(value)
+
+
+def explicit_backward_precision(value: Optional[str]) -> Optional[str]:
+    """``value`` checked, without the environment fallback: what the decoder, ``ProjEncoder`` and ``CTC`` use, so that
+    only their own attribute turns them to the bf16 backward (AVSR_B200_BWD_PRECISION reaches the encoder only)."""
     if value not in BACKWARD_PRECISIONS:
         raise ValueError(f"backward_precision={value!r}: expected None (default backward) or 'bf16'; f16 is not "
                          "offered (gradients overflow its 65504 range)")

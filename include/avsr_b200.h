@@ -380,6 +380,18 @@ int avsr_mha_core_bwd(const float *q, long ldq, const float *k, long ldk, const 
                       int Lk, int causal, const int32_t *key_lengths, const uint8_t *keep, float keep_scale,
                       const float *probs, const float *dctx, float *dq, long lddq, float *dk, float *dv, long lddkv,
                       void *workspace, size_t workspace_bytes, void *stream);
+/* The same backward on the tensor cores (wgmma): the arguments and outputs of avsr_mha_core_bwd, plus ctx (B, Lq, H*64)
+ * contiguous, the forward's output, and `precision`, which must be AVSR_PREC_BF16 (bf16 operands, fp32 accumulation;
+ * any other value is an error naming it).  Delta = rowsum(dctx o ctx) is computed in fp32; the stored probabilities are
+ * read tile by tile (nothing is recomputed).  Row strides, dq / dk / dv strides included, are multiples of 4 and
+ * >= H*64; q / k / v / ctx / dctx / dq / dk / dv are 16-byte aligned.  Two launches, no atomics, every sum in a fixed
+ * order: repeated calls are bit-identical.  Keys at or past the key length, and a zero-length utterance, get exact zeros.
+ * avsr_mha_core_bwd_tc_workspace_bytes returns 0 for a precision other than AVSR_PREC_BF16. */
+size_t avsr_mha_core_bwd_tc_workspace_bytes(int B, int H, int Lq, int Lk, int precision);
+int avsr_mha_core_bwd_tc(const float *q, long ldq, const float *k, long ldk, const float *v, long ldv, int B, int H,
+                         int Lq, int Lk, int causal, const int32_t *key_lengths, const uint8_t *keep, float keep_scale,
+                         const float *probs, const float *ctx, const float *dctx, float *dq, long lddq, float *dk,
+                         float *dv, long lddkv, int precision, void *workspace, size_t workspace_bytes, void *stream);
 int avsr_label_smoothing_fwd(const float *logits, long ld, const int64_t *target, int rows, int odim, int ignore_id,
                              float smoothing, float *row_loss, float *lse, void *stream);
 int avsr_label_smoothing_bwd(const float *logits, long ld, const int64_t *target, int rows, int odim, int ignore_id,

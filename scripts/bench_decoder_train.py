@@ -3,14 +3,17 @@
 (e2e_asr_conformer.py:77-80): token ids and encoder memory -> loss -> gradients of the memory and of every decoder
 parameter -- with CUDA events, for the drop-in and for the reference modules in eager PyTorch on the same GPU.
 
-    python scripts/bench_decoder_train.py [--steps 30] [--warmup 5]
+    python scripts/bench_decoder_train.py [--steps 30] [--warmup 5] [--profile]
 
 Synthetic bucket: memory lengths [400, 350, 300, 250, 300] (S2-like), label lengths [80, 70, 60, 50, 60], d 768, 12 heads,
 ff 3072, 6 layers, odim 5049, dropout as E2E builds the decoder (0.1 everywhere, attention probabilities included).
-Arms: the drop-in at f16 / tf32 / fp32 GEMM precision; the reference decoder + LabelSmoothingLoss (oracle/_ref, skipped
+Arms: the drop-in at f16 / tf32 / fp32 GEMM precision, and at f16 with backward_precision="bf16"; the reference decoder + LabelSmoothingLoss (oracle/_ref, skipped
 when it was not built) in fp32 and with allow_tf32.  Also the arithmetic of one step counted from shapes (GEMMs and
-attention, forward + backward).  Prints one JSON object with the device name and its power limit; writes nothing to the
-tree."""
+attention, forward + backward), and the per-call device time of the attention core's backward, fp32 kernels
+(avsr_mha_core_bwd) against the tensor-core kernels (avsr_mha_core_bwd_tc), at the bucket's self and source attention
+and at a long bucket.  ``--profile`` adds one step each of the default and the bf16 backward under torch.profiler: the
+device time per kernel, and its split into attention-core kernels, GEMMs and the rest.  Prints one JSON object with the
+device name and its power limit; writes nothing to the tree."""
 import argparse
 import json
 import os
@@ -91,10 +94,72 @@ def step_fn(dec, crit, data):
     return fn
 
 
+def attention_core_calls(dev, steps):
+    """ms per call (CUDA events over `steps` calls after a warm-up) of the two attention-core backwards on the same
+    stored probabilities, dropout 0.1 as in training."""
+    from auto_avsr_b200 import decoder_train as DT
+    shapes = {"self_5x81x81": (LAB, max(LAB) + 1, max(LAB) + 1, True),
+              "source_5x81x400": (MEM, max(LAB) + 1, max(MEM), False),
+              "source_long_5x151x600": ([600, 550, 500, 450, 500], 151, 600, False)}
+    g = torch.Generator(device=dev).manual_seed(1)
+    out = {}
+    for tag, (klen, Lq, Lk, causal) in shapes.items():
+        B = len(klen)
+        if causal:
+            src = torch.randn(B, Lq, 3 * D, device=dev, generator=g)
+            q, k, v = src[..., :D], src[..., D:2 * D], src[..., 2 * D:]
+            ln = torch.tensor([n + 1 for n in LAB], dtype=torch.int32, device=dev)
+        else:
+            q = torch.randn(B, Lq, D, device=dev, generator=g)
+            kv = torch.randn(B, Lk, 2 * D, device=dev, generator=g)
+            k, v = kv[..., :D], kv[..., D:]
+            ln = torch.tensor(klen, dtype=torch.int32, device=dev)
+        dctx = torch.randn(B, Lq, D, device=dev, generator=g)
+        keep, scale = DT.draw_keep_mask(0.1, (B, H, Lq, Lk), dev), 1.0 / 0.9
+        ctx, probs = DT.mha_core_forward(q, k, v, H, causal, ln, keep, scale, want_probs=True)
+        dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+        fp32 = lambda: DT.mha_core_backward(q, k, v, H, causal, ln, keep, scale, probs, dctx, dq, dk, dv)   # noqa: E731
+        tc = lambda: DT.mha_core_backward_tc(q, k, v, H, causal, ln, keep, scale, probs, ctx, dctx, dq, dk, dv)  # noqa
+        t32, ttc = time_ms(fp32, steps, 5), time_ms(tc, steps, 5)
+        out[tag] = {"fp32_ms": round(t32, 4), "bf16_tc_ms": round(ttc, 4), "speedup": round(t32 / ttc, 2)}
+    return out
+
+
+def profile_steps(dec, crit, data):
+    """One step each of the default and the bf16 backward under torch.profiler -> device ms per kernel and the split."""
+    from torch.profiler import ProfilerActivity, profile
+    res = {}
+    for tag, backward in (("default", None), ("bf16", "bf16")):
+        dec.backward_precision = backward
+        fn = step_fn(dec, crit, data)
+        fn()
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        kernels = {}
+        for e in prof.key_averages():
+            t = getattr(e, "device_time_total", None)
+            if t is None:
+                t = e.cuda_time_total
+            if t > 0:
+                kernels[e.key] = round(t / 1e3, 4)
+        split = {"attention_core": 0.0, "gemm": 0.0, "other": 0.0}
+        for name, ms in kernels.items():
+            kind = ("attention_core" if "mha_" in name else
+                    "gemm" if ("gemm" in name or "pack" in name or "linear" in name) else "other")
+            split[kind] += ms
+        res[tag] = {"split_ms": {k: round(v, 3) for k, v in split.items()},
+                    "kernels_ms": dict(sorted(kernels.items(), key=lambda kv: -kv[1])[:25])}
+    dec.backward_precision = None
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=30)
     ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--profile", action="store_true")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_decoder_train: needs a CUDA device")
@@ -110,6 +175,12 @@ def main():
     for prec in ("f16", "tf32", "fp32"):
         dec.precision = prec
         out["ms_per_step"]["dropin_" + prec] = round(time_ms(step_fn(dec, crit, data), args.steps, args.warmup), 3)
+    dec.precision, dec.backward_precision = "f16", "bf16"
+    out["ms_per_step"]["dropin_f16_bwd_bf16"] = round(time_ms(step_fn(dec, crit, data), args.steps, args.warmup), 3)
+    dec.backward_precision = None
+    out["attention_core_bwd_ms_per_call"] = attention_core_calls(dev, max(args.steps, 20))
+    if args.profile:
+        out["profile_one_step"] = profile_steps(dec, crit, data)
     del dec
     try:
         from oracle import build_ref
